@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- BASELINE.json's metric on the B200 path.
+"""bench.py -- BASELINE.json's metric on the H100 (sm_90a) path.
 
     python bench.py --gpus 1 --steps 10 --warmup 3                      # images/s, ViT-g/14 + Q-Former + VQ, B=256
     python bench.py --workload llama_prefill --steps 10 --warmup 3      # tokens/s, LLaMA-7B prefill, S=2048
@@ -16,6 +16,9 @@ With the default workload the line also carries `secondary` records for the LLaM
 reference-facing Python API (models.seed_llama_tokenizer.ImageTokenizer.encode / models.llama_xformer
 .LlamaForCausalLM.forward) starting from PINNED HOST buffers and ending with the ids / last-token logits on
 the host, copies inside the timed region.  Prints ONE JSON line on rank 0.
+--dump-outputs DIR writes what the last timed step of each GPU arm computed as DIR/<name>.npy (float32 / float64, a few
+MB in all): encode ids, LLaMA prefill last-token logits plus a seeded sample of logit rows, pipeline last-token logits,
+decode token ids, 8 seeded preprocessed images.  The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -34,7 +37,7 @@ if REPO not in sys.path:
     sys.path.insert(0, REPO)
 
 VIT_DEPTH, QF_LAYERS = 39, 12
-# algorithmic work per image (2 FLOP per MAC), SURVEY.md section 8d / DESIGN.md
+# algorithmic work per image (2 FLOP per MAC), SURVEY.md section 8d / BASELINE.md
 T_TOK, D, FF = 257, 1408, 6144
 GEMM_FLOPS_PER_IMAGE = (
     2 * 256 * 588 * D                                                   # patch embed
@@ -55,8 +58,9 @@ def measured_peaks():
         d = json.load(open(p))
         return {"tflops_burst": d.get("bf16_tflops"), "tflops_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d.get("hbm_gbs"), "source": "MEASURED_PEAKS.json (of measured)"}
-    return {"tflops_burst": 1590.0, "tflops_sustained": 1400.0, "hbm_gbs": 6650.0,
-            "source": "B200_PROFILING.md fallback (of fallback)"}
+    # NVIDIA H100 SXM data sheet (700 W card): dense FP16 tensor rate and HBM3 bandwidth -- not reached, a bound
+    return {"tflops_burst": 989.0, "tflops_sustained": 989.0, "hbm_gbs": 3350.0,
+            "source": "H100 SXM data sheet, 700 W (not measured)"}
 
 
 class ClockSampler:
@@ -141,6 +145,19 @@ def max_over_ranks(ms: float, world: int) -> float:
 
 
 LAST_LOCAL_MS = [0.0]
+
+
+def dump_outputs(args, rank, arrays):
+    """--dump-outputs: {name: tensor} -> DIR/<name>.npy on rank 0; integer tensors as float64, the rest as float32."""
+    if not args.dump_outputs or rank != 0:
+        return
+    import numpy as np
+
+    os.makedirs(args.dump_outputs, exist_ok=True)
+    for name, t in arrays.items():
+        t = t.detach().cpu()
+        a = t.double().numpy() if not t.is_floating_point() else t.float().numpy()
+        np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
 
 
 def timed(fn, steps, warmup, world):
@@ -293,8 +310,8 @@ def cpu_encode_images_per_s(sd, n_images: int, target_s: float = 20.0):
 
 
 def reference_arm(args, world, rank):
-    """--impl reference: the reference algorithm (oracle port: /root/reference is Python and does not travel to
-    the GPU box; oracle/restatement.py is pinned to it by tests/golden) on the host cores, same metric/config."""
+    """--impl reference: the reference algorithm on the host cores (oracle/restatement.py, pinned to the reference's
+    own outputs by tests/golden), same metric/config."""
     if rank != 0:
         return None
     from seed_b200 import synth
@@ -343,7 +360,7 @@ def reference_arm(args, world, rank):
             for _ in range(max(1, min(args.warmup, 1))):
                 R.llama_forward(sd, ids, 32, layers)
             t0 = time.perf_counter()
-            n = max(1, min(args.steps, 3))
+            n = max(1, args.steps)
             for _ in range(n):
                 R.llama_forward(sd, ids, 32, layers)
             dt = (time.perf_counter() - t0) / n
@@ -402,11 +419,12 @@ def encode_arm(args, world, rank, local, keep=None):
     L.reset_launch_count()
     with ClockSampler(local) as cs:
         ms = timed(step_device, args.steps, args.warmup, world)
+    dump_outputs(args, rank, {"ids": out["ids"]})
     rank_ms = per_rank_stats(LAST_LOCAL_MS[0] / args.steps, world)
     launches = L.launch_count() // (args.steps + args.warmup)
     clocks = cs.summary()
     ms_e2e = timed(step_e2e, args.steps, max(1, args.warmup), world)
-    # roofline of the dominant kernel (tcgen05 GEMM): one more identical step with every GEMM launch bracketed
+    # roofline of the dominant kernel (wgmma GEMM): one more identical step with every GEMM launch bracketed
     # by CUDA events on its stream
     torch.cuda.synchronize()
     L.profile_begin()
@@ -416,14 +434,8 @@ def encode_arm(args, world, rank, local, keep=None):
     gemm_ms, gemm_n = prof["gemm"]["ms"], prof["gemm"]["launches"]
     gemm_flops = GEMM_FLOPS_PER_IMAGE * B
     ach = gemm_flops / (gemm_ms * 1e-3) / 1e12
-    traffic, traffic_src = None, None
-    for name in ("r02_gemm_traffic.json", "r01_gemm_traffic.json"):
-        tp = os.path.join(REPO, "profiles", name)
-        if os.path.exists(tp):
-            traffic = json.load(open(tp)).get("dram_bytes_per_launch_avg")
-            traffic_src = f"static: ncu --set full capture committed as profiles/{name} (dram__bytes_read.sum + dram__bytes_write.sum per launch, average over the ViT shapes); not measured in this run"
-            break
-    roofline = {"kernel": "sb::gemm_tcgen05_kernel", "bound": "tensor", "achieved": round(ach, 1),
+    traffic, traffic_src = None, "not measured"
+    roofline = {"kernel": "sb::gemm_wgmma_kernel", "bound": "tensor", "achieved": round(ach, 1),
                 "peak": peaks["tflops_sustained"], "unit": "TFLOP/s", "frac": round(ach / peaks["tflops_sustained"], 4),
                 "traffic": traffic, "traffic_source": traffic_src,
                 "peak_source": peaks["source"] + ", sustained figure (kernel timed inside a long step)",
@@ -511,6 +523,7 @@ def llama_decode_arm(args, world, rank, local):
     L.reset_launch_count()
     with ClockSampler(local) as cs:
         ms = timed(step_device, args.steps, args.warmup, world)
+    dump_outputs(args, rank, {"llama_decode_tokens": out["seq"]})
     rank_ms = per_rank_stats(LAST_LOCAL_MS[0] / args.steps, world)
     launches = L.launch_count() // (args.steps + args.warmup)
     clocks = cs.summary()
@@ -583,6 +596,10 @@ def preprocess_arm(args, world, rank, local):
     L.reset_launch_count()
     with ClockSampler(local) as cs:
         ms = timed(step_device, args.steps, args.warmup, world)
+    if args.dump_outputs:                                             # 8 seeded images of the batch
+        pick = torch.randperm(B, generator=torch.Generator().manual_seed(0))[:8].sort().values
+        dump_outputs(args, rank, {"preprocess_images_sample": out["y"][pick.to(out["y"].device)],
+                                  "preprocess_image_index": pick})
     launches = L.launch_count() // (args.steps + args.warmup)
     clocks = cs.summary()
     ms_e2e = timed(step_e2e, args.steps, max(1, args.warmup), world)
@@ -642,6 +659,11 @@ def llama_arm(args, world, rank, local, keep=None):
     L.reset_launch_count()
     with ClockSampler(local) as cs:
         ms = timed(step_device, args.steps, args.warmup, world)
+    if args.dump_outputs:
+        lg = out["o"].logits[0]                                       # [S, V]: 16 seeded rows + the last one
+        rows = torch.randperm(S - 1, generator=torch.Generator().manual_seed(0))[:16].sort().values.to(lg.device)
+        dump_outputs(args, rank, {"llama_prefill_last_logits": lg[-1], "llama_prefill_logit_rows": rows,
+                                  "llama_prefill_logits_sample": lg[rows]})
     rank_ms = per_rank_stats(LAST_LOCAL_MS[0] / args.steps, world)
     launches = L.launch_count() // (args.steps + args.warmup)
     clocks = cs.summary()
@@ -669,7 +691,7 @@ def llama_arm(args, world, rank, local, keep=None):
                 "d2h_bytes_per_step": V * 4,
                 "api": "models.llama_xformer.LlamaForCausalLM.forward(pinned ids.to(cuda)) -> logits[:, -1].cpu()"},
         "gpu_launches": int(launches) * args.steps,
-        "roofline": {"kernel": "sb::gemm_tcgen05_kernel", "bound": "tensor", "achieved": round(ach, 1),
+        "roofline": {"kernel": "sb::gemm_wgmma_kernel", "bound": "tensor", "achieved": round(ach, 1),
                      "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
                      "frac": round(ach / peaks["tflops_sustained"], 4), "traffic": None,
                      "peak_source": peaks["source"], "launches_per_step": prof["gemm"]["launches"],
@@ -724,6 +746,7 @@ def pipeline_arm(args, world, rank, local, tok=None, model=None):
     L.reset_launch_count()
     with ClockSampler(local) as cs:
         ms = timed(step_device, args.steps, args.warmup, world)
+    dump_outputs(args, rank, {"pipeline_last_logits": out["o"].logits[:, -1]})
     rank_ms = per_rank_stats(LAST_LOCAL_MS[0] / args.steps, world)
     launches = L.launch_count() // (args.steps + args.warmup)
     clocks = cs.summary()
@@ -744,7 +767,7 @@ def pipeline_arm(args, world, rank, local, tok=None, model=None):
                 "api": "ImageTokenizer.encode(pinned.to(cuda)) -> all_gather_ids -> image_ids_to_tokens(out=prompt span) "
                        "-> LlamaForCausalLM.forward(last_logits_only) -> logits.cpu()"},
         "gpu_launches": int(launches) * args.steps,
-        "roofline": {"kernel": "whole chain (tcgen05 GEMMs dominate)", "bound": "tensor",
+        "roofline": {"kernel": "whole chain (wgmma GEMMs dominate)", "bound": "tensor",
                      "achieved": round(flops / step_s / 1e12, 1), "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
                      "frac": round(flops / step_s / 1e12 / peaks["tflops_sustained"], 4), "traffic": None,
                      "peak_source": peaks["source"]},
@@ -775,14 +798,18 @@ def main():
     ap.add_argument("--seq", type=int, default=2048, help="prompt length (llama_prefill)")
     ap.add_argument("--prompt", type=int, default=256, help="prompt length (llama_decode)")
     ap.add_argument("--new-tokens", type=int, default=128, help="generated tokens (llama_decode)")
-    ap.add_argument("--ctas", type=int, default=2, help="tcgen05 cta_group of the GEMMs (1 or 2)")
+    ap.add_argument("--ctas", type=int, default=2, help="GEMM ctas field (1 or 2; the H100 kernel runs single-CTA tiles)")
     ap.add_argument("--vq", default="fp16", choices=["fp16", "fp32"], help="VQ distance arithmetic")
     ap.add_argument("--cpu-images", type=int, default=0, help="images timed by the cpu_baseline leg (0 = ~20 s worth)")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-secondary", action="store_true",
                     help="encode workload only: skip the LLaMA half of BASELINE.json's metric (secondary records)")
     ap.add_argument("--ref-seconds", type=float, default=150.0, help="wall-clock budget of the --impl reference run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step of every GPU arm as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "seedb200":
+        raise SystemExit("bench.py: --dump-outputs needs the seedb200 arm (the reference arm times bounded samples)")
     args.warmup = max(args.warmup, 3) if args.impl == "seedb200" else args.warmup
 
     if args.impl == "reference":
@@ -796,7 +823,7 @@ def main():
                 "ms_per_step": round(r["ms_per_step"], 2), "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "dtype": "f32", "data": "synthetic",
                 "config": workload_config(args, max(world, args.gpus)),
-                "note": "reference algorithm on the host CPU (oracle port of /root/reference, pinned by tests/golden); "
+                "note": "reference algorithm on the host CPU (oracle port of the reference, pinned by tests/golden); "
                         "no GPU involved; every step is a BOUNDED SAMPLE of the workload: " + r["sample"],
                 "cpu_baseline": {"value": round(r["value"], 3), "unit": r["unit"], "cores": r["cores"], "kind": "port",
                                  "sample": r["sample"]},
@@ -819,10 +846,10 @@ def main():
         if not args.no_secondary:
             sec = {}
             a2 = copy.copy(args)
-            a2.workload, a2.steps = "llama_prefill", min(args.steps, 10)
+            a2.workload = "llama_prefill"
             sec["llama_prefill"] = compact(llama_arm(a2, world, rank, local, keep=keep))
             a3 = copy.copy(args)
-            a3.workload, a3.steps = "pipeline", min(args.steps, 5)
+            a3.workload = "pipeline"
             sec["pipeline"] = compact(pipeline_arm(a3, world, rank, local, tok=keep["tok"], model=keep["llama7b"]))
             keep.clear()
             import gc
@@ -830,7 +857,7 @@ def main():
             gc.collect()
             torch.cuda.empty_cache()
             a4 = copy.copy(args)
-            a4.workload, a4.steps = "llama_decode", min(args.steps, 3)
+            a4.workload = "llama_decode"
             sec["llama_decode"] = compact(llama_decode_arm(a4, world, rank, local))
             res["secondary"] = sec
     else:

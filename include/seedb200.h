@@ -1,5 +1,5 @@
 /*
- * seedb200.h -- C ABI of libseedb200.so: the B200 (sm_100a) replacement for the
+ * seedb200.h -- C ABI of libseedb200.so: the H100 (sm_90a) replacement for the
  * SEED visual-tokenizer encode path and the llama_xformer forward path.
  *
  * The reference (AILab-CVC/SEED) has no FFI of its own: its "plugin interface"
@@ -55,26 +55,16 @@ int64_t seedb200_launch_count(void);
 void seedb200_reset_launch_count(void);
 /* Optional per-kernel timing for bench.py's roofline: between begin and end every GEMM / attention launch of
  * the calling thread is bracketed by CUDA events on its stream.  end() synchronises, then reports for
- * kind 0 (tcgen05 GEMM) and kind 1 (attention): launches, summed device milliseconds and, for the GEMM, the
+ * kind 0 (wgmma GEMM) and kind 1 (attention): launches, summed device milliseconds and, for the GEMM, the
  * summed algorithmic FLOPs (2*M*N*K per launch).  out[kind*3 + {0,1,2}] = {launches, ms, flops}. */
-/* Process-wide switches (tests / A-B measurements).  "vit_attention_tc": 1 (default) routes the 257x257x88
- * ViT attention to the tcgen05 kernel attention_tc.cu, 2 to its staggered-pipeline variant attention_tc2.cu (same
- * results; measured slower while both are bound by the per-SM load/store unit, profiles/r02_attention.md), 0 to the
- * mma.sync kernel (attention.cu).
- * "causal_attention_tc": 1 (default) routes causal head_dim-128 attention with nq >= 128 (LLaMA prefill) to the
- * tcgen05 kernel (attention_causal_tc.cu), 0 to the mma.sync kernel.
- * "causal_attention_tma": 1 (default) = that kernel's Q / K / V tiles arrive by TMA when the layouts fit a 4-D tensor
- * map (the LLaMA projection buffer and KV caches do), 0 = cp.async loader warps.
+/* Process-wide switches (tests / A-B measurements).
  * "decode_pdl": 1 (default) launches the kernels of the cached decode step (q_len 1) with programmatic stream
  * serialization (each starts while its predecessor drains and waits on griddepcontrol before reading activations).
- * "gemm_ksub": 0 (default) = heuristic, 1 = 64-deep GEMM pipeline stages, 2 = 128-deep.
- * "gemm_tail": 1 (default) = a ragged last column of tiles runs at its own width, 0 = as a full tile.
  * "decode_fused_attention": 1 (default) = the cached decode step runs RoPE + KV append + attention as one kernel per
  * layer when max_seq <= 2048 (seedb200_decode_attention_rope), 0 = rope_kv_append + split-KV decode attention.
  * "gemv_no_allocate": 1 (default) = the decode GEMVs stream their weights with ld.global.nc.L1::no_allocate, 0 = ld.global.nc.
- * "gemm_sched": 1 (default) = a GEMM with a single row of tiles (M <= 256: a short LLaMA prompt) picks its tile width
- * from a busy-SM model (seedb200_gemm_plan), 0 = the fixed heuristics, 2 = balanced-tail tile order with an explicit
- * bn (A/B runs: measured equal to the rotated round robin, tools/llama_gemm_ab.py).
+ * "gemm_sched": 1 (default) = a GEMM of a short LLaMA prompt (M <= 256) picks its tile width from a busy-SM
+ * model (seedb200_gemm_plan), 0 = the fixed heuristics, 2 = balanced-tail tile order with an explicit bn.
  * "encoder_ln_fold" (read by seedb200_encoder_create): 1 (default) = norm1 / norm2 of the ViT blocks are folded
  * into the qkv / fc1 GEMMs (seedb200_gemm_desc.ln_stats), 0 = standalone LayerNorm kernels.                    */
 int seedb200_set_option(const char* key, int value);
@@ -99,7 +89,7 @@ typedef struct seedb200_tensor {
 
 /* out = epilogue(A[M,K] . W[N,K]^T): torch.nn.functional.linear as used at
  * eva_vit.py:133-135/:157/:60-65, qformer_causual.py:176-181/:251-255/:320-337,
- * llama_xformer.py:186/:223-225/:258/:718.  tcgen05 + TMA + TMEM kernel.     */
+ * llama_xformer.py:186/:223-225/:258/:718.  wgmma + TMA kernel.               */
 typedef struct seedb200_gemm_desc {
   int32_t M, N, K;
   const void* A;  int64_t lda;        /* fp16 [M,K]                              */
@@ -119,7 +109,7 @@ typedef struct seedb200_gemm_desc {
   int32_t row_group, row_stride, row_offset;
   int32_t res_mod, res_offset;
   int32_t bn;                         /* tile-N hint, 0 = auto                   */
-  int32_t ctas;                       /* 1 or 2 (cta_group::2 pair), 0 = auto    */
+  int32_t ctas;                       /* 0, 1 or 2: accepted; single-CTA tiles    */
   /* LayerNorm folded into the GEMM (eva_vit.py:201-202: x + attn(norm1(x)), x + mlp(norm2(x))): with
    * W' = W diag(gamma) as the W operand and A = the UN-normalised rows x,
    *   linear(LayerNorm(x), W, bias) = rstd_m * (acc_mn - mean_m * c_n) + b'_n,
@@ -129,17 +119,17 @@ typedef struct seedb200_gemm_desc {
    * rounding of LN(x) to fp16 is replaced by the rounding of W gamma to fp16 -- same order, bounded in the tests. */
   const void* ln_stats; const void* ln_c; const void* ln_b;
   /* optional: float2 [M, N/64] -- (sum, sum of squares) of every 64-column group of the OUTPUT row as stored (after
-   * bias / activation / residual, rounded to fp16); a warp that covers several groups writes its total into the first
-   * and zeros into the others.  seedb200_row_stats_from_moments turns the groups into the (mean, rstd) of the next
+   * bias / activation / residual, rounded to fp16); every group holds its own sums.  seedb200_row_stats_from_moments turns the groups into the (mean, rstd) of the next
    * LayerNorm-folded GEMM, so the residual stream is not re-read for its statistics (eva_vit.py:201-202: the output of
    * x + attn(..) / x + mlp(..) is what norm2 / the next block's norm1 normalise).  Needs mode 0, N % 64 == 0, no row
-   * remap and a 64-column-divisible tiling (the staged epilogue); otherwise SEEDB200_ERR_UNSUPPORTED.              */
+   * remap and a tile width that is a multiple of 64; otherwise SEEDB200_ERR_UNSUPPORTED.                          */
   void* row_moments;
 } seedb200_gemm_desc;
 int seedb200_gemm(const seedb200_gemm_desc* d, void* stream);
 /* Host-only views of the GEMM's persistent tile schedule (no GPU needed; tests/test_capi_cpu.py checks that every
  * tile is handed out exactly once).  gemm_plan: what seedb200_gemm would pick for `d` on a device with `sms` SMs --
- * out9 = {bn, ctas, sched, ksub, m_tiles, n_tiles, units, tile_shift, tail_w}; pointers in `d` are not dereferenced.
+ * out9 = {bn, ctas, sched, ksub, m_tiles, n_tiles, units, tile_shift, tail_w} (ctas = ksub = 1, tile_shift = tail_w = 0
+ * on H100); pointers in `d` are not dereferenced.
  * gemm_schedule_tile: the tile (mt * n_tiles + nt) of unit `unit`'s round-th iteration, m_tiles * n_tiles when the
  * unit is done.  sched 0 = rotated round robin (default), 1 = balanced tail (full-width tiles round robin, then the
  * units that got one fewer take the last-column tiles; option "gemm_sched" = 2).                                    */
@@ -273,7 +263,7 @@ typedef struct seedb200_encoder_config {
   int32_t n_codes;          /* 8192                                              */
   int32_t max_batch;        /* workspace is sized for this many images per call  */
   int32_t vq_mode;          /* seedb200_vq_mode                                  */
-  int32_t gemm_ctas;        /* 0 auto, 1, 2: cta_group used by the GEMMs         */
+  int32_t gemm_ctas;        /* 0, 1, 2: passed to the GEMMs' ctas field          */
 } seedb200_encoder_config;
 
 int seedb200_encoder_create(const seedb200_encoder_config* cfg, const seedb200_tensor* weights, int n_weights,

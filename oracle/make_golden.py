@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE ONLY -- generate tests/golden/*.pt by running the UNMODIFIED reference code
-(/root/reference, through oracle/ref_shim.py) on the seeded synthetic weights of oracle/synth.py.
+(through oracle/ref_shim.py; its location is SEED_REFERENCE_ROOT) on the seeded synthetic weights of oracle/synth.py.
 
-The reference ships no tests, golden vectors or fixtures (SURVEY.md section 4), so these files are the
-known-answer vectors for the path.  Run in the build container (the GPU box has no /root/reference):
+The reference ships no tests, golden vectors or fixtures, so these files are the
+known-answer vectors for the path.  Run where a checkout of the reference is available:
 
     python -m oracle.make_golden [--full]
 
@@ -97,8 +97,11 @@ def llama_golden(name: str = "llama_tiny.pt") -> None:
     print(f"{name}: logits {tuple(out.logits.shape)} next {nxt.flatten().tolist()}")
 
 
-def vq_golden(name: str = "vq_reference_expr.pt") -> None:
-    """The reference distance/argmin expression itself (qformer_quantizer.py:94-98) in fp32 and in half."""
+def vq_golden(name: str = "vq_reference_expr.npz") -> None:
+    """The reference distance/argmin expression itself (qformer_quantizer.py:94-98) in fp32 and in half.
+    Compressed numpy archive: the reference's ids, the default-init codebook, and sums of the seeded inputs."""
+    import numpy as np
+
     qq = ref_shim.load_quantizer_module()
     g = torch.Generator().manual_seed(99)
     res = {}
@@ -115,15 +118,39 @@ def vq_golden(name: str = "vq_reference_expr.pt") -> None:
             _, _, ids16 = vq16(z.view(n // 32, 32, 32))
         res[tag] = {"z": z, "codebook": cb, "ids_fp32": ids32.flatten().clone(), "ids_fp16": ids16.flatten().clone()}
         print(f"{name}/{tag}: fp32 vs fp16 agreement {(ids32 == ids16).float().mean():.4f}")
+    # ids as int16; z and the "spread" codebook are seed-99 draws the tests regenerate, stored as sums only
+    arrs = {f"{t}__{k}": v[k].numpy().astype(np.int16) for t, v in res.items() for k in ("ids_fp32", "ids_fp16")}
+    arrs["default_init__codebook"] = res["default_init"]["codebook"].numpy()
+    for t, k in (("spread", "z"), ("spread", "codebook"), ("default_init", "z")):
+        arrs[f"{t}__{k}_sum"] = np.array(res[t][k].double().sum().item())
+    np.savez_compressed(os.path.join(GOLDEN_DIR, name), **arrs)
+
+
+def encoder_seeded_golden(name: str = "encoder_d1_q2_seed77.pt") -> None:
+    """Depth-1 ViT, 2 Q-Former layers, 1 de-tokenizer block on weights seed 77 / images seed 78: the reference's
+    get_codebook_indices (ids, query_output_up) and get_codebook_entry outputs, stored whole."""
+    vd, ql, dd = 1, 2, 1
+    model = ref_shim.build_reference_quantizer(vd, ql, dd)
+    sd = synth.encoder_state_dict(vd, ql, dd, seed=77)
+    model.load_state_dict(sd, strict=False)
+    x = synth.images(2, seed=78)
+    with torch.no_grad():
+        ids, up = model.get_codebook_indices(x)
+        emb = model.get_codebook_entry(ids)
+    res = {"config": {"vit_depth": vd, "qformer_layers": ql, "detok_depth": dd, "weights_seed": 77, "images_seed": 78,
+                      "batch": 2, "dtype": "fp32 (reference CPU mode)"},
+           "ids": ids.clone(), "query_output_up": up.clone(), "image_embeds_out": emb.clone()}
     torch.save(res, os.path.join(GOLDEN_DIR, name))
+    print(f"{name}: ids[0,:8]={ids[0, :8].tolist()}")
 
 
 def main() -> None:
-    assert ref_shim.available(), "the reference must be mounted at /root/reference"
+    assert ref_shim.available(), f"no reference checkout at {ref_shim.REFERENCE_ROOT} (set SEED_REFERENCE_ROOT)"
     torch.manual_seed(0)
     vq_golden()
     llama_golden()
     encoder_golden("encoder_d2_q2.pt", 2, 2, 1, 2)
+    encoder_seeded_golden()
     if "--full" in sys.argv:
         encoder_golden("encoder_full.pt", 39, 12, 4, 2)
 

@@ -1,11 +1,10 @@
-"""TEST INFRASTRUCTURE ONLY -- import the UNMODIFIED reference modules from /root/reference on CPU.
+"""TEST INFRASTRUCTURE ONLY -- import the UNMODIFIED reference modules from a reference checkout on CPU.
 
 The reference pins transformers 4.30 / timm / xformers / diffusers, none of which match this image.  This
 module registers ~40 lines of stub modules and back-fills three removed transformers helpers so that
 `models.seed_qformer.qformer_quantizer` and `models.llama_xformer` import and run as shipped (recipe and
-probes: SURVEY.md section 8c).  It exists only in the build container (the GPU box has no /root/reference);
-it is used by oracle/make_golden.py to generate tests/golden/* and by tests that pin oracle/restatement.py
-against the real reference when it is available.
+probes: SURVEY.md section 8c).  The checkout is found at SEED_REFERENCE_ROOT; this module is used by
+oracle/make_golden.py to generate tests/golden/*, against which the tests pin oracle/restatement.py.
 
 Nothing here is arithmetic: the stubs replace (a) timm init helpers (trunc_normal_, to_2tuple, DropPath),
 (b) three network-touching factories (BertTokenizer / BertLMHeadModel.from_pretrained / eva_vit_g.pth

@@ -1,7 +1,6 @@
-"""Build libseedb200.so (sm_100a only) and the C oracle, in-tree.
+"""Build libseedb200.so (sm_90a, H100) and the C oracle, in-tree.
 
-nvcc cross-compiles here without a GPU; the resulting .so files travel to the GPU box with the repo
-snapshot.  `python -m seed_b200.build [--force]` or `__graft_entry__.build()`.
+nvcc cross-compiles without a GPU.  `python -m seed_b200.build [--force]` or `__graft_entry__.build()`.
 """
 from __future__ import annotations
 
@@ -18,12 +17,12 @@ LIB = os.path.join(ROOT, "libseedb200.so")
 ORACLE_DIR = os.path.join(REPO, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "libvq_oracle.so")
 
-SOURCES = ["capi.cu", "gemm_tcgen05.cu", "attention.cu", "attention_tc.cu", "attention_tc2.cu", "attention_causal_tc.cu", "rowwise.cu", "vq.cu", "misc.cu", "sampler.cu", "encoder.cu", "llama.cu", "preprocess.cu"]
-HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "ops.h"), os.path.join(CSRC, "attention_tc_common.cuh"), os.path.join(REPO, "include", "seedb200.h")]
+SOURCES = ["capi.cu", "gemm_wgmma.cu", "attention.cu", "rowwise.cu", "vq.cu", "misc.cu", "sampler.cu", "encoder.cu", "llama.cu", "preprocess.cu"]
+HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "ops.h"), os.path.join(REPO, "include", "seedb200.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xptxas", "-v",
@@ -61,7 +60,7 @@ def build_cuda(force: bool = False) -> str:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(lambda j: _run(*j), jobs))
     if force or jobs or not _newer(LIB, objs):
-        _run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"])
+        _run([NVCC, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

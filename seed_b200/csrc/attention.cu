@@ -14,8 +14,8 @@
 // memory only.  The additive -10000 causal mask of the Q-Former underflows to exactly 0 after exp in
 // fp32, so it is implemented as a hard mask.
 //
-// This is ~3% of the encode FLOPs; the tcgen05 budget went to the GEMM first.  A tcgen05/TMEM version
-// of this kernel is the next step for the LLaMA prefill path.
+// This is ~3% of the encode FLOPs; the tensor-core budget went to the GEMM first.  A wgmma version of
+// this kernel is the next step for the LLaMA prefill path.
 #include "common.cuh"
 
 namespace sb {
@@ -326,13 +326,6 @@ static int launch_attn(const seedb200_attn_desc& d, cudaStream_t stream) {
   return 0;
 }
 
-bool vit_attention_tc_applicable(const seedb200_attn_desc& d);
-int vit_attention_tc(const seedb200_attn_desc& d, cudaStream_t stream);
-int vit_attention_tc2(const seedb200_attn_desc& d, cudaStream_t stream);
-bool causal_attention_tc_applicable(const seedb200_attn_desc& d);
-int causal_attention_tc(const seedb200_attn_desc& d, cudaStream_t stream);
-int get_option(const char* key);
-
 int attention(const seedb200_attn_desc& d, cudaStream_t stream) {
   SB_REQUIRE(d.q && d.k && d.v && d.o, "attention: null operand");
   SB_REQUIRE(d.batch > 0 && d.heads > 0 && d.nq > 0 && d.nk > 0, "attention: empty problem");
@@ -347,9 +340,6 @@ int attention(const seedb200_attn_desc& d, cudaStream_t stream) {
   SB_REQUIRE(((uintptr_t)d.q % 16 == 0) && ((uintptr_t)d.k % 16 == 0) && ((uintptr_t)d.v % 16 == 0) &&
                  ((uintptr_t)d.o % 4 == 0),
              "attention: misaligned pointer");
-  if (vit_attention_tc_applicable(d) && get_option("vit_attention_tc") != 0)
-    return get_option("vit_attention_tc") == 2 ? vit_attention_tc2(d, stream) : vit_attention_tc(d, stream);
-  if (causal_attention_tc_applicable(d) && get_option("causal_attention_tc") != 0) return causal_attention_tc(d, stream);
   if (d.head_dim == 64) {
     if (d.nq <= 32) return launch_attn<64, 2>(d, stream);
     return launch_attn<64, 4>(d, stream);

@@ -49,8 +49,8 @@ void profile_mark_end(int kind, cudaStream_t stream, double flops) {
 
 static std::map<std::string, int>& options() {
   static std::map<std::string, int> o = [] {
-    std::map<std::string, int> m = {{"vit_attention_tc", 1}, {"causal_attention_tc", 1}, {"decode_pdl", 1}, {"gemv_ksplit", 0},
-                                    {"gemm_ksub", 0}, {"gemm_tail", 1}, {"encoder_ln_fold", 1}, {"gemv_prefetch_mb", 0}, {"vit_attention_tma", 1}, {"gemm_out_tma", 1}, {"encoder_stats_fused", 1}, {"gemm_sched", 1}, {"decode_fused_attention", 1}, {"gemv_no_allocate", 1}, {"causal_attention_tma", 1}};
+    std::map<std::string, int> m = {{"decode_pdl", 1}, {"gemv_ksplit", 0},
+                                    {"encoder_ln_fold", 1}, {"gemv_prefetch_mb", 0}, {"encoder_stats_fused", 1}, {"gemm_sched", 1}, {"decode_fused_attention", 1}, {"gemv_no_allocate", 1}};
     // A/B runs of unmodified commands (bench.py): SEEDB200_OPT_<KEY>=<int> overrides a default at load time
     for (auto& kv : m) {
       std::string env = "SEEDB200_OPT_";

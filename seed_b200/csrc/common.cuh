@@ -1,8 +1,8 @@
-// common.cuh -- shared host/device helpers for libseedb200 (sm_100a only).
+// common.cuh -- shared host/device helpers for libseedb200 (sm_90a, H100).
 //
-// Device side: thin inline-PTX wrappers for the Blackwell primitives the kernels
-// use (mbarrier, TMA bulk-tensor loads, tcgen05 alloc/mma/commit/ld, cluster
-// helpers).  Host side: error plumbing for the C ABI (no exceptions cross it).
+// Device side: thin inline-PTX wrappers for the Hopper primitives the kernels
+// use (mbarrier, TMA bulk-tensor loads, programmatic dependent launch).
+// Host side: error plumbing for the C ABI (no exceptions cross it).
 #pragma once
 
 #include <cuda.h>
@@ -108,25 +108,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n"
-               "barrier.cluster.wait.acquire.aligned;\n" ::
-                   : "memory");
-}
-
-// shared::cluster address of the same smem offset in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-
 // ---- mbarrier ---------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
@@ -136,12 +117,6 @@ __device__ __forceinline__ void fence_mbar_init() {
 }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// arrive on a barrier addressed in the shared::cluster window (local or remote CTA)
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_bar) {
-  // default (.release.cta) semantics on purpose: the .release.cluster form makes ptxas emit
-  // MEMBAR.ALL.GPU + CCTL.IVALL in front of every arrive (measured: 4x slower 2-CTA GEMM)
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_bar) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes)
@@ -160,24 +135,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Non-blocking test of a phase (mbarrier.try_wait may park the thread for an implementation-defined time before it
-// answers "not yet": fine inside a wait loop, wrong for a poll that has something else to do)
-__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 // Bounded waits: a protocol bug traps (kernel error) instead of hanging the GPU.  The deadline is checked once every
-// 4096 polls only: a clock64() + compare per poll made the wait loops ~half of all instructions the attention kernel
-// issued (profiles/r02_attention.md) -- issue slots and power taken from the warps doing work.
+// 4096 polls only, so that the wait loops do not take issue slots from the warps doing work.
 #ifndef SB_MBAR_TIMEOUT_CYCLES
 #define SB_MBAR_TIMEOUT_CYCLES (8000000000LL)
 #endif
@@ -199,7 +158,7 @@ static __device__ __noinline__ void mbar_timeout_trap(uint32_t bar, uint32_t par
   printf("seedb200: mbarrier timeout block %d thread %d bar 0x%x parity %u\n", blockIdx.x, threadIdx.x, bar, parity);
   __trap();
 }
-// latency-critical waits (MMA issuer, TMA producer): plain polling, deadline check amortised
+// latency-critical waits: plain polling, deadline check amortised
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
@@ -209,7 +168,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
-// waits that are expected to be long (epilogue / softmax warps waiting for an MMA, loaders waiting for a free buffer):
+// waits that are expected to be long (the TMA producer waiting for a free buffer):
 // the thread is parked by the hardware (suspend-time hint) instead of spinning, so it neither steals issue slots from
 // the warps doing work nor burns power polling.
 __device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
@@ -233,159 +192,6 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, uint
       "%4}], [%2];" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
-}
-// 3-D tiled load (attention: elements of a head, head slot, token row)
-__device__ __forceinline__ void tma_load_3d(uint32_t dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1,
-                                            int32_t c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::
-          "r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1,
-                                            int32_t c2, int32_t c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];" ::
-          "r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d(uint32_t dst, const void* tmap, uint32_t bar, int32_t c0, int32_t c1,
-                                            int32_t c2, int32_t c3, int32_t c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], "
-      "[%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-// cta_group::2 variant: data lands in the executing CTA's smem, the transaction
-// bytes are signalled on `cluster_bar` (a shared::cluster address, normally the
-// leader CTA's barrier).
-__device__ __forceinline__ void tma_load_2d_2cta(uint32_t dst, const void* tmap, uint32_t cluster_bar,
-                                                 int32_t c0, int32_t c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], "
-      "[%1, {%3, %4}], [%2];" ::"r"(dst),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(cluster_bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-
-// ---- tcgen05 ----------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-template <int CTAS>
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  if constexpr (CTAS == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int CTAS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  if constexpr (CTAS == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-  }
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16/bf16 inputs, issued by ONE thread.
-template <int CTAS>
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  if constexpr (CTAS == 1) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  }
-}
-
-// Arrive on `bar` when all previously issued tcgen05.mma of this thread retire.
-// CTAS == 2: the arrive is multicast to the same barrier offset in both CTAs.
-template <int CTAS>
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  if constexpr (CTAS == 1) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-                 : "memory");
-  } else {
-    const uint16_t mask = 3;
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-            "r"(bar),
-        "h"(mask)
-        : "memory");
-  }
-}
-
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, "
-      "%14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 64-bit shared-memory matrix descriptor, K-major operand, 128-byte swizzle:
-// rows are 128 B (64 halves), 8-row groups 1024 B apart (SBO), LBO unused.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);   // start address  [0,14)
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;              // stride byte offset [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                      // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                      // layout type: SWIZZLE_128B
-  return d;
-}
-
-// same for the 64-byte swizzle: rows are 64 B (32 halves), 8-row groups 512 B apart
-__device__ __forceinline__ uint64_t make_smem_desc_sw64(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(512 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(4) << 61;                      // layout type: SWIZZLE_64B
-  return d;
-}
-
-// 32-bit instruction descriptor for kind::f16: fp16 A/B (K-major), fp32 accumulate.
-__host__ __device__ constexpr uint32_t make_idesc_f16(int umma_m, int umma_n) {
-  return (1u << 4)                                   // c_format = F32
-         | (0u << 7)                                 // a_format = F16
-         | (0u << 10)                                // b_format = F16
-         | (0u << 15) | (0u << 16)                   // a_major, b_major = K
-         | (static_cast<uint32_t>(umma_n >> 3) << 17)  // n_dim
-         | (static_cast<uint32_t>(umma_m >> 4) << 24); // m_dim
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,5 +1,5 @@
 // encoder.cu -- seedb200_encoder: the SEED image tokenizer forward (Blip2QformerQuantizer,
-// qformer_quantizer.py:143-338) as a fixed sequence of sm_100a kernel launches on the caller's stream.
+// qformer_quantizer.py:143-338) as a fixed sequence of sm_90a kernel launches on the caller's stream.
 //
 //   encode      = get_codebook_indices (qformer_quantizer.py:288-307):
 //                 EVA ViT-g/14 forward_features (eva_vit.py:369-385, 39 x Block :199-206)
@@ -508,7 +508,7 @@ int seedb200_encoder_create(const seedb200_encoder_config* cfg, const seedb200_t
   e->last_B = 0;
   e->device = sb::cur_device();
   e->ln_fold = sb::get_option("encoder_ln_fold") != 0;
-  e->stats_fused = sb::get_option("encoder_stats_fused") != 0 && sb::get_option("gemm_out_tma") != 0;
+  e->stats_fused = sb::get_option("encoder_stats_fused") != 0;
   for (int i = 0; i < n_weights; ++i) e->w[std::string(weights[i].name)] = weights[i];
   int s = sb::build(e);
   if (s != 0) {

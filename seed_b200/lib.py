@@ -95,7 +95,7 @@ def load() -> C.CDLL:
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
-            f"{LIB_PATH} not found: build it with `python -m seed_b200.build` (needs nvcc, sm_100a). "
+            f"{LIB_PATH} not found: build it with `python -m seed_b200.build` (needs nvcc, sm_90a). "
             "seed_b200 has no CPU or PyTorch fallback path.")
     lib = C.CDLL(LIB_PATH)
     lib.seedb200_version.restype = C.c_int

@@ -2,7 +2,7 @@
 
 Same public surface as the reference class on the inference path -- `from_pretrained`,
 `get_codebook_indices(image) -> (embed_ind, query_output_up)`, `get_codebook_entry(indices)`, `n_embed`,
-`codebook_embed_dim`, `.eval()/.half()/.to()` -- but every forward runs as hand-written sm_100a kernels behind
+`codebook_embed_dim`, `.eval()/.half()/.to()` -- but every forward runs as hand-written sm_90a kernels behind
 the C ABI (include/seedb200.h).  There is no eager-PyTorch path: without a CUDA device or without the built
 library the constructor raises.
 """

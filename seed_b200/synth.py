@@ -6,7 +6,7 @@ Weights are drawn per tensor from a generator seeded by a hash of (seed, tensor 
 regenerated independently and identically on any machine with the same torch.  Every value is rounded to
 fp16 so that the fp32 CPU oracle and the fp16 GPU path consume bit-identical parameters.
 
-Deviation from the reference initialisers (documented in DESIGN.md and bench output):
+Deviation from the reference initialisers (documented in the bench output):
   * the codebook is drawn N(0, CODEBOOK_STD) instead of U(+-1/8192) (qformer_quantizer.py:39): with the default
     init every distance rounds to |z|^2 in fp16 and argmin is 0 for all tokens, which makes id parity vacuous
     (SURVEY.md section 7 "degenerate synthetic codebook");

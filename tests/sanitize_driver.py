@@ -55,8 +55,8 @@ def gemm():
 
 
 def attention():
-    for (B, H, Nq, Nk, D, causal) in [(2, 16, 257, 257, 88, False),      # tcgen05 ViT kernel
-                                      (1, 4, 300, 300, 128, True),        # tcgen05 causal kernel, ragged tiles
+    for (B, H, Nq, Nk, D, causal) in [(2, 16, 257, 257, 88, False),      # ViT shape
+                                      (1, 4, 300, 300, 128, True),        # causal, ragged tiles
                                       (1, 4, 128, 428, 128, True),        # ... with a past
                                       (2, 12, 32, 32, 64, True),          # mma.sync kernel: Q-Former self
                                       (2, 12, 32, 257, 64, False)]:       # Q-Former cross

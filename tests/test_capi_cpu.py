@@ -111,7 +111,7 @@ def test_image_ids_to_tokens_and_transform_contract():
         get_transform("other")
 
 
-def _plan(L, M, N, K, ctas=2, mode=0, bn=0, sms=148):
+def _plan(L, M, N, K, ctas=2, mode=0, bn=0, sms=132):
     d = L.GemmDesc()
     d.M, d.N, d.K, d.ctas, d.mode, d.bn = M, N, K, ctas, mode, bn
     out = (C.c_int32 * 9)()
@@ -159,13 +159,14 @@ def test_gemm_tile_schedules_hand_out_every_tile_exactly_once(L, shape):
 
 
 def test_gemm_plan_for_single_tile_rows_and_tuned_shapes(L):
-    """A 256-token prompt (one row of tiles on CTA pairs): N = 5120 runs on 128-wide tiles (40 busy pairs instead of
-    20), N = 15360 keeps 256; the M = 2048 prefill shapes and the ViT shapes keep their tuned 256-wide tiling (narrower
-    tiles were measured and lost, profiles/r02_summary.md)."""
+    """A 256-token prompt (two rows of 128-row tiles): N = 5120 runs on 128-wide tiles (80 busy SMs instead of 40),
+    N = 15360 keeps 256; the M = 2048 prefill shapes and the ViT shapes take the widest tile that divides N (no
+    half-empty last column), all on single CTAs (ctas = 2 is accepted and runs the same tiles)."""
     assert _plan(L, 256, 5120, 5120)["bn"] == 128
     assert _plan(L, 256, 5120, 13824)["bn"] == 128
     assert _plan(L, 256, 15360, 5120)["bn"] == 256
-    for M, N, K in ((2048, 4096, 4096), (2048, 12288, 4096), (2048, 4096, 11008), (65792, 1408, 1408), (65792, 4224, 1408),
-                    (65792, 6144, 1408), (65792, 1408, 6144)):
+    for M, N, K, bn in ((2048, 4096, 4096, 256), (2048, 12288, 4096, 256), (2048, 4096, 11008, 256),
+                        (65792, 1408, 1408, 176), (65792, 4224, 1408, 192), (65792, 6144, 1408, 256),
+                        (65792, 1408, 6144, 176)):
         p = _plan(L, M, N, K)
-        assert (p["bn"], p["ctas"], p["sched"]) == (256, 2, 0), p
+        assert (p["bn"], p["ctas"], p["sched"]) == (bn, 1, 0), p

@@ -130,7 +130,7 @@ def _greedy_agree(gpu_logits, ref_logits, gap=5e-2):
 
 def test_llama7b_dims_prefill_s2048_matches_oracle():
     """config #3 shapes: h=4096, 32 heads, ffn=11008, V=40194 (rows 4-byte aligned -> padded stride), S=2048 with an
-    image span; 2 of the 32 layers.  K = 4096 and 11008 GEMMs, BN=256 SiLU-gate tiles, causal tcgen05 attention at
+    image span; 2 of the 32 layers.  K = 4096 and 11008 GEMMs, BN=256 SiLU-gate tiles, causal attention at
     2048 x 2048, lm_head over all positions (llama_xformer.py:661-743)."""
     hidden, layers, heads, ffn, vocab, S = 4096, 2, 32, 11008, 40194, 2048
     model, sd = make(hidden, layers, heads, ffn, vocab, seed=31, max_batch=1, max_seq=S, ctas=2)

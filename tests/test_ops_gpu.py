@@ -13,7 +13,6 @@ from oracle import ops_ref as R
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-VIT_TC_DEFAULT = 1        # seedb200_set_option("vit_attention_tc"): 1 = lock-step tcgen05 kernel (default), 2 = staggered variant
 
 
 def rel_err(a, b):
@@ -50,7 +49,8 @@ def rand16(*shape, scale=1.0, seed=0):
 
 
 # ----------------------------------------------------------------------------------------------
-# GEMM (tcgen05): every tile shape x cta_group, tails in M/N/K, persistent multi-tile schedules
+# GEMM (wgmma): every tile width, tails in M/N/K, persistent multi-tile schedules; ctas = 2 is accepted and runs
+# the same single-CTA tiles
 # ----------------------------------------------------------------------------------------------
 GEMM_SHAPES = [
     # M, N, K, bn, ctas
@@ -63,19 +63,19 @@ GEMM_SHAPES = [
     (1000, 768, 768, 128, 1),
     (96, 96, 768, 64, 1),         # N tail inside a 64-wide tile (scalar store path)
     (64, 32, 768, 32, 1),         # z projection
-    (4096, 1024, 256, 32, 1),     # 1024 tiles over 148 CTAs: >= 6 accumulator hand-offs per CTA
+    (4096, 1024, 256, 32, 1),     # 1024 tiles over 132 CTAs: >= 7 tiles per persistent CTA
     (2048, 40194, 512, 256, 1),   # lm_head-like: odd ldo -> unaligned rows, N tail
-    (512, 512, 1408, 256, 2),     # cta_group::2
+    (512, 512, 1408, 256, 2),
     (300, 256, 592, 256, 2),
     (1028, 4224, 1408, 192, 2),
     (1028, 1408, 1408, 176, 2),
     (1000, 768, 768, 128, 2),
     (4096, 1024, 256, 64, 2),
-    (1028, 1408, 1408, 256, 2),   # ragged N on a CTA pair: 5 full tiles + a 128-wide tail tile (proj / fc2 tiling)
-    (513, 1408, 6144, 256, 2),    # same with the 128-deep pipeline stages (fc2)
-    (300, 40194, 512, 256, 2),    # tail of 2 columns -> 32-wide UMMA on the pair (lm_head)
-    (300, 1000, 768, 256, 1),     # single CTA, tail 232 -> 240
-    (200, 272, 256, 256, 1),      # tail of one 16-column chunk: the second epilogue warp of each quarter has no chunk
+    (1028, 1408, 1408, 256, 2),   # ragged N: 5 full tiles + a half-empty last column
+    (513, 1408, 6144, 256, 2),    # same with a long reduction (fc2)
+    (300, 40194, 512, 256, 2),    # last column holds 2 columns (lm_head)
+    (300, 1000, 768, 256, 1),     # last column 232 of 256 wide
+    (200, 272, 256, 256, 1),      # last column 16 of 256 wide
 ]
 
 
@@ -91,8 +91,7 @@ def test_gemm_plain(lib, M, N, K, bn, ctas):
     assert_close16(out, ref, what="gemm")
 
 
-# one row of tiles (a 256-token prompt on the 13B shapes): the plan picks 128-wide tiles when 256-wide ones leave most
-# CTA pairs idle; the M = 2048 shapes keep the 256-wide tiling.  K kept short so the fp32 oracle stays cheap
+# a 256-token prompt on the 13B shapes: the plan picks 128-wide tiles when 256-wide ones leave most SMs idle; the M = 2048 shapes keep the 256-wide tiling.  K kept short so the fp32 oracle stays cheap
 PLANNED_SHAPES = [(256, 5120, 320), (256, 15360, 128), (200, 5120, 192), (2048, 4096, 320), (2048, 5120, 192)]
 
 
@@ -247,10 +246,10 @@ ATTN_CASES = [
     (1, 2, 5, 133, 128, True),        # chunked prefill with past: bottom-right aligned causal
     (2, 8, 100, 200, 128, True),      # 100 new tokens after a 100-token past (8-warp tile, nk != nq)
     (1, 2, 130, 300, 128, True),
-    (1, 3, 512, 640, 128, True),      # tcgen05 causal kernel: two tile pairs after a 128-token past
+    (1, 3, 512, 640, 128, True),      # two 128-row query tiles after a 128-token past
     (2, 5, 257, 257, 128, True),      # ragged second pair (one row)
     (1, 2, 128, 128, 128, True),      # single tile, second tile of the pair absent
-    (1, 40, 1024, 1024, 128, True),   # 160 items > 148 CTAs: snake schedule, several items per CTA
+    (1, 40, 1024, 1024, 128, True),   # 160 (head, query tile) items and more
     (1, 3, 1, 77, 128, False),        # single query through the prefill kernel
     (1, 2, 100, 100, 64, False),
 ]
@@ -270,54 +269,41 @@ def test_attention(lib, B, H, Nq, Nk, D, causal):
     assert (o.float() - ref.float()).abs().max().item() < 1e-2
 
 
-@pytest.mark.parametrize("use_tc", [2, 1, 0])
-@pytest.mark.parametrize("B", [1, 5, 40])
-def test_vit_attention_tcgen05_vs_mma_paths(lib, B, use_tc):
-    """the 257x257x88 ViT shape on the tcgen05 kernels (2: attention_tc2.cu, staggered tile pipelines; 1:
-    attention_tc.cu, lock step) and on the mma.sync kernel; B=40 gives 640 (image, head) items so every persistent
-    CTA walks several of them"""
+@pytest.mark.parametrize("B", [1, 2, 3, 5, 8, 13, 40, 64, 100])
+def test_vit_attention_packed_qkv_batches(lib, B):
+    """the 257x257x88 ViT shape read from the packed [B*257, 3*16*88] qkv GEMM output; B=40..100 give 640..1600
+    (image, head) items, several waves of CTAs"""
     H, N, D = 16, 257, 88
     qkv = rand16(B * N, 3 * H * D, seed=34)
     v4 = qkv.view(B, N, 3, H, D)
     q, k, v = (v4[:, :, i].permute(0, 2, 1, 3) for i in range(3))
     ref = R.attention_ref(q, k, v, D ** -0.5, False)
-    for tma in ((1, 0) if use_tc == 1 else (1,)):     # kernel 1: Q/K by TMA (swizzled blocks) and by cp.async (no swizzle)
-        lib.set_option("vit_attention_tc", use_tc)
-        lib.set_option("vit_attention_tma", tma)
-        try:
-            o = lib.attention(q, k, v, D ** -0.5, False)
-            torch.cuda.synchronize()
-        finally:
-            lib.set_option("vit_attention_tc", VIT_TC_DEFAULT)
-            lib.set_option("vit_attention_tma", 1)
-        assert rel_err(o, ref) < 2e-3, (tma, rel_err(o, ref))
-        assert (o.float() - ref.float()).abs().max().item() < 1e-2
-        # the 257th query row is computed outside the MMA tiles: check it on its own
-        assert rel_err(o[:, 256], ref[:, 256]) < 2e-3
+    o = lib.attention(q, k, v, D ** -0.5, False)
+    torch.cuda.synchronize()
+    assert rel_err(o, ref) < 2e-3, rel_err(o, ref)
+    assert (o.float() - ref.float()).abs().max().item() < 1e-2
+    # the 257th query row sits alone in the last query tile: check it on its own
+    assert rel_err(o[:, 256], ref[:, 256]) < 2e-3
 
 
-def test_vit_attention_variants_agree_on_large_scores(lib):
-    """scores up to ~+-60 (peaked softmax, fp16 P underflow in the tail), every variant against the fp32 reference"""
+def test_vit_attention_large_scores(lib):
+    """scores up to ~+-60 (peaked softmax, fp16 P underflow in the tail) at head_dim 88 against the fp32 reference"""
     B, H, N, D = 3, 16, 257, 88
     q = rand16(B, H, N, D, scale=3.0, seed=71)
     k = rand16(B, H, N, D, scale=3.0, seed=72)
     v = rand16(B, H, N, D, seed=73)
     ref = R.attention_ref(q, k, v, D ** -0.5, False)
-    for use_tc in (2, 1):
-        lib.set_option("vit_attention_tc", use_tc)
-        try:
-            o = lib.attention(q, k, v, D ** -0.5, False)
-            torch.cuda.synchronize()
-        finally:
-            lib.set_option("vit_attention_tc", VIT_TC_DEFAULT)
-        assert rel_err(o, ref) < 3e-3, (use_tc, rel_err(o, ref))
+    o = lib.attention(q, k, v, D ** -0.5, False)
+    torch.cuda.synchronize()
+    assert rel_err(o, ref) < 3e-3, rel_err(o, ref)
 
 
-@pytest.mark.parametrize("B,S,past,max_seq", [(2, 700, 333, 1200), (1, 2048, 0, 2048), (3, 130, 7, 200)])
-@pytest.mark.parametrize("use_tc,use_tma", [(1, 1), (1, 0), (0, 0)])
-def test_causal_attention_tcgen05_vs_mma_paths(lib, use_tc, use_tma, B, S, past, max_seq):
-    """LLaMA prefill layout (q from a fused projection buffer, K/V in a [B,H,max_seq,D] cache with a past) on the
-    tcgen05 kernel (attention_causal_tc.cu) with TMA and with cp.async loaders, and on the mma.sync kernel"""
+@pytest.mark.parametrize("B,S,past,max_seq", [(2, 700, 333, 1200), (1, 2048, 0, 2048), (3, 130, 7, 200),
+                                              (1, 128, 0, 128), (1, 129, 64, 256), (2, 256, 1, 300),
+                                              (1, 1000, 1048, 2048), (4, 64, 500, 600), (1, 513, 2, 1024)])
+def test_causal_attention_prefill_cache_layout(lib, B, S, past, max_seq):
+    """LLaMA prefill layout: q sliced from a fused projection buffer, K/V from a [B,H,max_seq,D] cache holding a past;
+    the cache rows behind the sequence are NaN, so any read of them that reaches the MMAs shows in the output"""
     H, D = 4, 128
     qbuf = rand16(B * S, H * D, seed=35)
     kc = rand16(B, H, max_seq, D, seed=36)
@@ -326,35 +312,12 @@ def test_causal_attention_tcgen05_vs_mma_paths(lib, use_tc, use_tma, B, S, past,
     k, v = kc[:, :, :past + S], vc[:, :, :past + S]
     kc[:, :, past + S:] = float("nan")          # rows past the sequence must never reach the MMAs
     vc[:, :, past + S:] = float("nan")
-    lib.set_option("causal_attention_tc", use_tc)
-    lib.set_option("causal_attention_tma", use_tma)
-    try:
-        o = lib.attention(q, k, v, D ** -0.5, True)
-        torch.cuda.synchronize()
-    finally:
-        lib.set_option("causal_attention_tc", 1)
-        lib.set_option("causal_attention_tma", 1)
+    o = lib.attention(q, k, v, D ** -0.5, True)
+    torch.cuda.synchronize()
     ref = R.attention_ref(q, k, v, D ** -0.5, True)
     assert torch.isfinite(o.float()).all()
     assert rel_err(o, ref) < 2e-3, rel_err(o, ref)
     assert (o.float() - ref.float()).abs().max().item() < 1e-2
-
-
-def test_causal_attention_tma_and_cp_async_loaders_agree_bitwise(lib):
-    B, H, S, D = 2, 3, 515, 128
-    qbuf = rand16(B * S, H * D, seed=41)
-    kc = rand16(B, H, 600, D, seed=42)
-    vc = rand16(B, H, 600, D, seed=43)
-    q = qbuf.view(B, S, H, D).permute(0, 2, 1, 3)
-    outs = []
-    for tma in (1, 0):
-        lib.set_option("causal_attention_tma", tma)
-        try:
-            outs.append(lib.attention(q, kc[:, :, :S], vc[:, :, :S], D ** -0.5, True))
-            torch.cuda.synchronize()
-        finally:
-            lib.set_option("causal_attention_tma", 1)
-    assert torch.equal(outs[0], outs[1])
 
 
 def test_causal_attention_large_scores_rescale(lib):
@@ -714,17 +677,30 @@ def test_gemm_row_moments_give_the_layernorm_statistics_of_the_output(lib, M, N,
     """x += linear(a) with the (sum, sum of squares) of every 64-column group of the NEW x left by the epilogue
     (seedb200_gemm_desc.row_moments): row_stats_from_moments == row_stats of the stored rows, so the next
     LayerNorm-folded GEMM does not have to re-read x (eva_vit.py:201-202)."""
+    _check_row_moments(lib, M, N, K, ctas, 0)
+
+
+# the last column of tiles reaches past N (320 = 256 + 64 with the planned 256-wide tiles, 1408 = 5.5 x 256): the groups
+# beyond N belong to no row and must not be written -- not into the next row's slots, not behind the buffer
+@pytest.mark.parametrize("M,N,K,bn", [(257, 320, 256, 0), (300, 1408, 1408, 256), (129, 1408, 512, 256)])
+def test_gemm_row_moments_when_the_last_tile_reaches_past_n(lib, M, N, K, bn):
+    _check_row_moments(lib, M, N, K, 1, bn)
+
+
+def _check_row_moments(lib, M, N, K, ctas, bn):
     a = rand16(M, K, seed=85)
     w = rand16(N, K, scale=K ** -0.5, seed=86)
     bias = rand16(N, scale=0.1, seed=87)
     x = rand16(M, N, scale=2.0, seed=88) + 0.25
     x[:, 7] += 20.0
-    plain = lib.gemm(a, w, bias, residual=x, ctas=ctas)
-    mom = torch.full((M, N // 64, 2), float("nan"), dtype=torch.float32, device=DEV)
-    out = lib.gemm(a, w, bias, residual=x, out=x, ctas=ctas, row_moments=mom)          # in place, like proj / fc2
+    plain = lib.gemm(a, w, bias, residual=x, ctas=ctas, bn=bn)
+    mom_buf = torch.full((M + 1, N // 64, 2), float("nan"), dtype=torch.float32, device=DEV)
+    mom = mom_buf[:M]                                          # one guard row behind the buffer the GEMM gets
+    out = lib.gemm(a, w, bias, residual=x, out=x, ctas=ctas, bn=bn, row_moments=mom)   # in place, like proj / fc2
     torch.cuda.synchronize()
     assert torch.equal(out, plain)                             # the moments do not change the result
     assert not torch.isnan(mom).any()                          # every group slot was written
+    assert torch.isnan(mom_buf[M]).all()                       # and nothing behind the last row
     of = out.float()
     assert torch.allclose(mom[:, :, 0].sum(-1), of.sum(-1), rtol=1e-5, atol=1e-2)
     assert torch.allclose(mom[:, :, 1].sum(-1), (of * of).sum(-1), rtol=1e-5, atol=1e-2)
@@ -736,7 +712,7 @@ def test_gemm_row_moments_give_the_layernorm_statistics_of_the_output(lib, M, N,
     x2 = rand16(M, N, scale=2.0, seed=88) + 0.25
     x2[:, 7] += 20.0
     mom2 = torch.empty_like(mom)
-    lib.gemm(a, w, bias, residual=x2, out=x2, ctas=ctas, row_moments=mom2)
+    lib.gemm(a, w, bias, residual=x2, out=x2, ctas=ctas, bn=bn, row_moments=mom2)
     torch.cuda.synchronize()
     assert torch.equal(mom, mom2)
 

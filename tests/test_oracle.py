@@ -1,7 +1,7 @@
 """CPU tests (-m "not gpu") that PIN the oracle:
   * oracle/restatement.py (plain-torch restatement) and oracle/vq_oracle.c (C restatement of the VQ search)
     against tests/golden/*.pt, which oracle/make_golden.py produced by running the unmodified reference;
-  * and, when /root/reference is mounted (build container only), against the live reference itself.
+  * including tests/golden/encoder_d1_q2_seed77.pt, a second configuration stored whole.
 """
 import ctypes as C
 import os
@@ -10,13 +10,29 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import ref_shim, restatement as R, synth
+from oracle import restatement as R, synth
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def _load(name):
     return torch.load(os.path.join(GOLDEN, name), map_location="cpu", weights_only=False)
+
+
+def _load_vq(tag):
+    """vq_reference_expr.npz: the reference's ids (int16) per tag and the default-init codebook; z and the "spread"
+    codebook are the seed-99 draws of oracle/make_golden.py vq_golden, regenerated here and checked by their sums."""
+    g = torch.Generator().manual_seed(99)
+    z = {"spread": (torch.randn(512, 32, generator=g) * 0.28).half()}
+    cb = (torch.randn(8192, 32, generator=g) * 0.28).half()
+    z["default_init"] = (torch.randn(128, 32, generator=g) * 0.28).half()
+    with np.load(os.path.join(GOLDEN, "vq_reference_expr.npz")) as f:
+        codebook = cb if tag == "spread" else torch.from_numpy(f["default_init__codebook"])
+        out = {"z": z[tag], "codebook": codebook}
+        for k in ("z", "codebook") if tag == "spread" else ("z",):
+            assert out[k].double().sum().item() == float(f[f"{tag}__{k}_sum"]), f"seeded {tag} {k} did not regenerate"
+        out.update({k: torch.from_numpy(f[f"{tag}__{k}"]).long() for k in ("ids_fp32", "ids_fp16")})
+    return out
 
 
 def _check_sample(t, s, rtol=2e-5):
@@ -53,7 +69,7 @@ def c_oracle(lib, z16, cb16, mode):
 # ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("tag", ["spread", "default_init"])
 def test_c_vq_oracle_matches_reference_vectors(vq_lib, tag):
-    g = _load("vq_reference_expr.pt")[tag]
+    g = _load_vq(tag)
     ids32, m32 = c_oracle(vq_lib, g["z"], g["codebook"], 1)
     ids16, m16 = c_oracle(vq_lib, g["z"], g["codebook"], 0)
     # exact wherever the oracle's own top-2 margin is not a floating-point tie; report would-be flips
@@ -112,16 +128,14 @@ def test_encoder_restatement_matches_golden_full_depth():
     _encoder_vs_golden("encoder_full.pt")
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="/root/reference not mounted (GPU box)")
 def test_encoder_restatement_matches_live_reference():
+    """the reference's outputs on a second weight / image seed (oracle/make_golden.py encoder_seeded_golden)"""
+    g = _load("encoder_d1_q2_seed77.pt")
+    ids, up, emb = g["ids"], g["query_output_up"], g["image_embeds_out"]
     vd, ql, dd = 1, 2, 1
-    model = ref_shim.build_reference_quantizer(vd, ql, dd)
     sd = synth.encoder_state_dict(vd, ql, dd, seed=77)
-    model.load_state_dict(sd, strict=False)
     x = synth.images(2, seed=78)
     with torch.no_grad():
-        ids, up = model.get_codebook_indices(x)
-        emb = model.get_codebook_entry(ids)
         out = R.encode(x, sd, vd, ql)
         emb2 = R.detokenize(ids, sd, dd)
     assert torch.equal(ids, out["ids"])
