@@ -97,6 +97,8 @@ typedef struct seedb200_gemm_desc {
   void* out;      int64_t ldo;        /* fp16 [rows, N] (N/2 columns in mode 1)  */
   const void* bias;                   /* fp16 [N] or NULL                        */
   const void* residual; int64_t ldr;  /* fp16, added after bias/act, or NULL     */
+  /* leading dimensions in elements; 0 = packed rows (K for lda / ldw, the output width for ldo / ldr).  A nonzero
+   * value below that width is refused (SEEDB200_ERR_INVALID), as is a residual in mode 1.                          */
   int32_t act;                        /* seedb200_act                            */
   int32_t mode;                       /* 0 linear; 1 SiLU-gate: W rows are blocks
                                          of [128 gate | 128 up], out[m,j] =

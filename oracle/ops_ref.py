@@ -3,7 +3,8 @@ CUDA kernel replaces.  Only tests/, __graft_entry__.smoke() and bench.py's cpu_b
 
 Every function takes fp16 (or int) tensors, computes in fp32 on whatever device they live on, and rounds to
 fp16 at the points where the reference's fp16 GPU mode rounds (SURVEY.md section 8a precision table), so the
-kernels can be compared with a tolerance of a few fp16 ulps.
+kernels can be compared with a tolerance of a few fp16 ulps.  `dtype=torch.float64` computes the same expression
+with the same fp16 rounding points in double precision (tests/test_kernel_edges_gpu.py bounds the kernels against it).
 """
 from __future__ import annotations
 
@@ -15,16 +16,16 @@ import torch.nn.functional as F
 
 
 def r16(x: torch.Tensor) -> torch.Tensor:
-    """round an fp32 tensor to fp16 and back (the rounding torch applies when it stores an fp16 result)."""
-    return x.to(torch.float16).to(torch.float32)
+    """round an fp32 / fp64 tensor to fp16 and back (the rounding torch applies when it stores an fp16 result)."""
+    return x.to(torch.float16).to(x.dtype)
 
 
-def linear_ref(a, w, bias=None, act: int = 0, residual=None):
+def linear_ref(a, w, bias=None, act: int = 0, residual=None, dtype=torch.float32):
     """torch.nn.functional.linear + activation + residual with fp16 rounding after each torch op
     (eva_vit.py:133-135,157,60-65; qformer_causual.py:251-255,320-337)."""
-    y = a.float() @ w.float().t()
+    y = a.to(dtype) @ w.to(dtype).t()
     if bias is not None:
-        y = y + bias.float()
+        y = y + bias.to(dtype)
     y = r16(y)
     if act == 1:
         y = r16(F.gelu(y))            # exact erf GELU (nn.GELU / ACT2FN['gelu'])
@@ -33,14 +34,14 @@ def linear_ref(a, w, bias=None, act: int = 0, residual=None):
     elif act == 3:
         y = r16(torch.relu(y))
     if residual is not None:
-        y = r16(y + residual.float())
+        y = r16(y + residual.to(dtype))
     return y.to(torch.float16)
 
 
-def silu_gate_ref(a, w_gate, w_up):
+def silu_gate_ref(a, w_gate, w_up, dtype=torch.float32):
     """LlamaMLP: act_fn(gate_proj(x)) * up_proj(x)  (llama_xformer.py:186), fp16 tensors at every step."""
-    g = r16(a.float() @ w_gate.float().t())
-    u = r16(a.float() @ w_up.float().t())
+    g = r16(a.to(dtype) @ w_gate.to(dtype).t())
+    u = r16(a.to(dtype) @ w_up.to(dtype).t())
     s = r16(F.silu(g))
     return r16(s * u).to(torch.float16)
 
@@ -54,23 +55,24 @@ def interleave_gate_up(w_gate, w_up):
     return torch.cat([g, u], dim=1).reshape(2 * ffn, h).contiguous()
 
 
-def layernorm_ref(x, w, b, eps: float):
+def layernorm_ref(x, w, b, eps: float, dtype=torch.float32):
     """nn.LayerNorm evaluated in fp32, result cast to fp16 (blip2.py:179-184; autocast fp32 LN in eva_vit.py:201)."""
-    return F.layer_norm(x.float(), (x.shape[-1],), w.float(), b.float(), eps).to(torch.float16)
+    return F.layer_norm(x.to(dtype), (x.shape[-1],), w.to(dtype), b.to(dtype), eps).to(torch.float16)
 
 
-def rmsnorm_ref(x, w, eps: float):
-    """LlamaRMSNorm.forward (llama_xformer.py:105-113)."""
-    xf = x.float()
+def rmsnorm_ref(x, w, eps: float, dtype=torch.float32):
+    """LlamaRMSNorm.forward (llama_xformer.py:105-113): the normalised row is rounded to fp16 before the fp16
+    multiply by the weight (a product of two fp16 values is exact in fp32, so that multiply rounds once)."""
+    xf = x.to(dtype)
     var = xf.pow(2).mean(-1, keepdim=True)
     h = (xf * torch.rsqrt(var + eps)).to(torch.float16)
-    return (w * h).to(torch.float16)
+    return (w.to(dtype) * h.to(dtype)).to(torch.float16)
 
 
-def attention_ref(q, k, v, scale: float, causal: bool = False):
+def attention_ref(q, k, v, scale: float, causal: bool = False, dtype=torch.float32):
     """softmax(scale * q k^T [+ causal mask]) v in fp32; q [B,H,Nq,D], k/v [B,H,Nk,D] -> [B,Nq,H,D] fp16
     (eva_vit.py:139-156; qformer_causual.py:189-236; llama_xformer.py:240-256)."""
-    qf, kf, vf = q.float(), k.float(), v.float()
+    qf, kf, vf = q.to(dtype), k.to(dtype), v.to(dtype)
     s = (qf @ kf.transpose(-1, -2)) * scale
     if causal:
         nq, nk = q.shape[2], k.shape[2]

@@ -110,7 +110,7 @@ __device__ __forceinline__ float apply_act(float x, int act) {
   switch (act) {
     case SEEDB200_ACT_GELU: return gelu_erf(x);
     case SEEDB200_ACT_TANH: return tanhf(x);
-    case SEEDB200_ACT_RELU: return fmaxf(x, 0.0f);
+    case SEEDB200_ACT_RELU: return x < 0.0f ? 0.0f : x;   // NaN stays NaN, as torch.relu (fmaxf would give 0)
     default: return x;
   }
 }
@@ -536,6 +536,17 @@ static int plan_short_prompt(const seedb200_gemm_desc& d, int sms) {
   return bn;
 }
 
+// A leading dimension of 0 means packed rows (K for A and W, the output width for out and the residual), as
+// seedb200_gemv's ldo <= 0: a zero-initialised descriptor describes contiguous operands.
+static seedb200_gemm_desc with_packed_defaults(seedb200_gemm_desc d) {
+  const int n_out = d.mode == 1 ? d.N / 2 : d.N;
+  if (d.lda == 0) d.lda = d.K;
+  if (d.ldw == 0) d.ldw = d.K;
+  if (d.ldo == 0) d.ldo = n_out;
+  if (d.ldr == 0) d.ldr = n_out;
+  return d;
+}
+
 struct GemmPlan { int bn, sched; };
 static int choose_plan(const seedb200_gemm_desc& d, int sms, GemmPlan& plan) {
   SB_REQUIRE(d.M > 0 && d.N > 0 && d.K > 0, "gemm: non-positive shape M=%d N=%d K=%d", d.M, d.N, d.K);
@@ -547,8 +558,17 @@ static int choose_plan(const seedb200_gemm_desc& d, int sms, GemmPlan& plan) {
   }
   if (d.mode == 1) {
     SB_REQUIRE(d.N % 256 == 0, "gemm: SiLU-gate mode needs N %% 256 == 0 (got %d)", d.N);
-    SB_REQUIRE(d.bias == nullptr && d.act == 0, "gemm: SiLU-gate mode takes no bias/activation");
+    SB_REQUIRE(d.bias == nullptr && d.act == 0 && d.residual == nullptr,
+               "gemm: SiLU-gate mode takes no bias/activation/residual");
   }
+  // the operand rows are read K wide and the output rows written n_out wide: a shorter leading dimension would make
+  // rows overlap
+  const int n_out = d.mode == 1 ? d.N / 2 : d.N;
+  SB_REQUIRE(d.lda >= d.K && d.ldw >= d.K, "gemm: lda=%lld / ldw=%lld below K=%d", (long long)d.lda,
+             (long long)d.ldw, d.K);
+  SB_REQUIRE(d.ldo >= n_out, "gemm: ldo=%lld below the %d output columns", (long long)d.ldo, n_out);
+  SB_REQUIRE(d.residual == nullptr || d.ldr >= n_out, "gemm: ldr=%lld below the %d output columns",
+             (long long)d.ldr, n_out);
   SB_REQUIRE(d.ctas >= 0 && d.ctas <= 2, "gemm: ctas must be 0, 1 or 2 (got %d)", d.ctas);
   if (d.row_moments != nullptr) {
     SB_REQUIRE(d.mode == 0 && d.N % 64 == 0, "gemm: row_moments needs mode 0 and N %% 64 == 0 (N=%d)", d.N);
@@ -572,7 +592,8 @@ static int choose_plan(const seedb200_gemm_desc& d, int sms, GemmPlan& plan) {
   return 0;
 }
 
-int gemm(const seedb200_gemm_desc& d, cudaStream_t stream) {
+int gemm(const seedb200_gemm_desc& desc, cudaStream_t stream) {
+  const seedb200_gemm_desc d = with_packed_defaults(desc);
   GemmPlan plan;
   SB_PROPAGATE(choose_plan(d, num_sms(), plan));
   SB_REQUIRE(d.A && d.W && d.out, "gemm: null operand");
@@ -594,7 +615,7 @@ extern "C" int seedb200_gemm_plan(const seedb200_gemm_desc* d, int sms, int32_t*
     return SEEDB200_ERR_INVALID;
   }
   sb::GemmPlan plan;
-  SB_PROPAGATE(sb::choose_plan(*d, sms, plan));
+  SB_PROPAGATE(sb::choose_plan(sb::with_packed_defaults(*d), sms, plan));
   const sb::TileSchedule t = sb::make_schedule(d->M, d->N, plan.bn, plan.sched, sms);
   const int32_t v[9] = {plan.bn, 1, t.sched, 1, t.m_tiles, t.n_tiles, t.units, 0, 0};
   for (int i = 0; i < 9; ++i) out9[i] = v[i];

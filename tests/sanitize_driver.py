@@ -5,9 +5,10 @@
     compute-sanitizer --tool synccheck --error-exitcode 1 python tests/sanitize_driver.py
     compute-sanitizer --tool initcheck --error-exitcode 1 python tests/sanitize_driver.py
 
-Shapes are the smallest that still walk every code path (pipeline wrap-around, CTA pairs, ragged tail tile, both
-attention tensor-core kernels, split-KV decode attention, top-p sampler); each result is also compared with the
-per-op oracle so a sanitizer-clean run is known to have computed the right thing.  `--only name` runs one family.
+Shapes are the smallest that still walk every code path (pipeline wrap-around, ragged tail tile, K below one k-block,
+strided operand views, every head_dim variant of the attention kernel, split-KV decode attention, top-p sampler); each
+result is also compared with the per-op oracle so a sanitizer-clean run is known to have computed the right thing.
+`--only name` runs one family.
 """
 import argparse
 import os
@@ -39,6 +40,16 @@ def gemm():
         res = r16(M, N, seed=4)
         out = L.gemm(a, w, bias=b, act=L.ACT_GELU, residual=res, bn=bn, ctas=ctas)
         assert rel(out, R.linear_ref(a, w, b, 1, res)) < 2e-3, (M, N, K)
+    # K below one k-block (the encoder's K = 32 linears), on views into wider buffers with trailing rows: lda, ldw, ldr
+    # and ldo all above the logical widths
+    for (M, N, K, bn) in [(65, 40, 8, 64), (129, 200, 24, 176), (64, 768, 32, 256), (1, 33, 32, 32)]:
+        a = r16(M + 3, K + 16, seed=5)[:M, :K]
+        w = r16(N + 5, K + 8, scale=K ** -0.5, seed=6)[:N, :K]
+        res = r16(M + 1, N + 24, seed=7)[:M, :N]
+        obuf = torch.zeros((M + 2, N + 40), dtype=torch.float16, device=DEV)
+        out = L.gemm(a, w, act=L.ACT_RELU, residual=res, out=obuf[:M, :N], bn=bn)
+        assert rel(out, R.linear_ref(a, w, None, 3, res)) < 2e-3, (M, N, K)
+        assert (obuf[M:] == 0).all() and (obuf[:, N:] == 0).all()
     # staged epilogue with TMA residual boxes, in place, leaving the row moments (the encoder's proj / fc2 calls)
     a, w, b = r16(520, 768, seed=1), r16(1408, 768, scale=768 ** -0.5, seed=2), r16(1408, seed=3)
     x = r16(520, 1408, seed=4)
@@ -59,7 +70,9 @@ def attention():
                                       (1, 4, 300, 300, 128, True),        # causal, ragged tiles
                                       (1, 4, 128, 428, 128, True),        # ... with a past
                                       (2, 12, 32, 32, 64, True),          # mma.sync kernel: Q-Former self
-                                      (2, 12, 32, 257, 64, False)]:       # Q-Former cross
+                                      (2, 12, 32, 257, 64, False),        # Q-Former cross
+                                      (2, 3, 40, 100, 88, True),          # head_dim 88, short query tile <96,4>
+                                      (1, 2, 300, 64, 88, False)]:        # head_dim 88, nq > 288, nq > nk
         q, k, v = r16(B, H, Nq, D, seed=11), r16(B, H, Nk, D, seed=12), r16(B, H, Nk, D, seed=13)
         out = L.attention(q, k, v, D ** -0.5, causal)
         assert rel(out, R.attention_ref(q, k, v, D ** -0.5, causal)) < 3e-3, (B, H, Nq, Nk, D, causal)

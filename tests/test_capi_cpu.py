@@ -42,6 +42,30 @@ def test_errors_are_reported_not_thrown(L):
     d.A = d.W = d.out = 16
     assert handle.seedb200_gemm(C.byref(d), None) == 1
     assert b"multiple of 8" in handle.seedb200_last_error()
+    # inconsistent GEMM descriptors are refused by the planner, before any device work
+    out9 = (C.c_int32 * 9)()
+
+    def plan_error(**fields):
+        g = L.GemmDesc()
+        g.M, g.N, g.K, g.lda, g.ldw, g.ldo = 64, 512, 64, 64, 64, 512
+        for k, v in fields.items():
+            setattr(g, k, v)
+        if handle.seedb200_gemm_plan(C.byref(g), 132, out9) == 0:
+            return None
+        return handle.seedb200_last_error()
+
+    assert plan_error() is None and plan_error(mode=1, ldo=256) is None
+    assert plan_error(lda=0, ldw=0, ldo=0) is None                             # 0 = packed rows
+    assert plan_error(mode=1, ldo=0) is None
+    assert b"residual" in plan_error(mode=1, ldo=256, residual=16, ldr=256)      # SiLU-gate has no residual (as the GEMV)
+    assert b"lda=56" in plan_error(lda=56)
+    assert b"ldw=8" in plan_error(ldw=8)
+    assert b"ldo=504" in plan_error(ldo=504)
+    assert b"ldo=248" in plan_error(mode=1, ldo=248)                           # mode 1 writes N / 2 columns
+    assert plan_error(residual=16) is None                                     # ldr = 0: packed, N
+    assert b"ldo=-8" in plan_error(ldo=-8)
+    assert b"ldr=511" in plan_error(residual=16, ldr=511)
+    assert plan_error(residual=16, ldr=520, ldo=520, lda=72, ldw=128) is None
     a = L.AttnDesc()
     a.q = a.k = a.v = a.o = 16
     a.batch = a.heads = a.nq = a.nk = 1

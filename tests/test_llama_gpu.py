@@ -182,6 +182,32 @@ def test_llama13b_dims_prefill_and_cached_decode_match_oracle():
     assert rel(k_gpu, ref_past[1][0]) <= 5e-3 and rel(v_gpu, ref_past[1][1]) <= 5e-3
 
 
+def test_batch_above_the_gemv_limit_prefill_and_cached_decode():
+    """B = 6 sequences: the cached decode steps run 6-row linears on the wgmma GEMM (M <= 4 goes to the GEMV), the
+    SiLU-gate and residual epilogues at M = 6, and decode attention over 6 caches; each step is fed the oracle's
+    greedy tokens so both sides see the same inputs"""
+    hidden, layers, heads, ffn, vocab, B, P, steps = 512, 2, 4, 1408, 1056, 6, 40, 4
+    model, sd = make(hidden, layers, heads, ffn, vocab, seed=13, max_batch=B, max_seq=P + steps + 4)
+    ids = synth.prompt_ids(B, P, n_image_spans=1, text_vocab=vocab - 66, n_codes=64, seed=14)
+    with torch.no_grad():
+        ref_logits, _, ref_past = R.llama_forward(sd, ids, heads, layers)
+    out = model(input_ids=ids.cuda(), use_cache=True)
+    assert rel(out.logits, ref_logits) <= LOGIT_TOL, rel(out.logits, ref_logits)
+    past = out.past_key_values
+    for t in range(steps):
+        nxt = ref_logits[:, -1].argmax(-1, keepdim=True)
+        with torch.no_grad():
+            ref_logits, _, ref_past = R.llama_forward(sd, nxt, heads, layers, past=ref_past)
+        o = model(input_ids=nxt.cuda(), past_key_values=past, use_cache=True)
+        past = o.past_key_values
+        assert tuple(o.logits.shape) == (B, 1, vocab)
+        assert rel(o.logits, ref_logits) <= LOGIT_TOL, (t, rel(o.logits, ref_logits))
+        for b in range(B):                                 # every sequence, not just the batch average
+            assert rel(o.logits[b], ref_logits[b]) <= LOGIT_TOL, (t, b, rel(o.logits[b], ref_logits[b]))
+    assert past[0][0].shape[2] == P + steps
+    assert rel(past[1][0], ref_past[1][0]) <= 5e-3 and rel(past[1][1], ref_past[1][1]) <= 5e-3
+
+
 # --------------------------------------------------------------------------------------------------
 # device-resident generation loop (seedb200_llama_generate): sampler + graph-replayed decode steps
 # --------------------------------------------------------------------------------------------------
