@@ -13,7 +13,9 @@
 //   * the consumers run wgmma.mma_async m64nBNk16 straight from shared memory, accumulators in
 //     registers (setmaxnreg moves the producer's register budget to them);
 //   * epilogue from registers: bias / activation / residual with the reference's fp16 rounding
-//     points.  While it runs, the producer already streams the next tile's operands.  SiLU-gate
+//     points.  Its operands are fetched while the k-loop runs (column vectors staged in shared memory, LayerNorm
+//     statistics in registers, residual rows prefetched into L2), and its kind is chosen once per tile, so the
+//     per-column work is arithmetic and stores.  While it runs, the producer already streams the next tile's operands.  SiLU-gate
 //     mode reads the gate and up halves of the same accumulator tile (llama_xformer.py:186).
 #include <stdio.h>
 
@@ -73,7 +75,7 @@ struct GemmCfg {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES_RAW = (200 * 1024) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
-  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * STAGES * 8;
+  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * STAGES * 8 + 2 * 2 * BN * 4;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
   static_assert(B_BYTES % 1024 == 0, "W stage must keep 1024-byte alignment for SWIZZLE_128B");
   static_assert(BN % 16 == 0 && BN <= 256, "invalid wgmma N");
@@ -196,28 +198,31 @@ template <> __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint
                : "l"(a), "l"(b));
 }
 
-// Two adjacent columns (n, n+1) of one output row, MODE 0: (LN fold | bias) -> fp16 -> act -> fp16 -> (+residual) -> fp16
-__device__ __forceinline__ __half2 epilogue_pair(const GemmParams& p, float v0, float v1, int n, bool pair_ok,
-                                                 float2 ln_st, const __half* res_row) {
-  if (p.ln_stats != nullptr) {
+// Per-tile epilogue kinds of MODE 0 (one branch per tile, not per output pair)
+enum EpiCols { EPI_NONE = 0, EPI_BIAS = 1, EPI_LN = 2 };
+
+// Two adjacent columns of one output row, MODE 0: (LN fold | bias) -> fp16 -> act -> fp16 -> (+residual) -> fp16.
+// c, b: the columns' ln_c / ln_b (EPI_LN) or bias (b, EPI_BIAS), staged in shared memory per tile.
+template <int COLS>
+__device__ __forceinline__ __half2 epilogue_pair(float v0, float v1, float2 c, float2 b, float2 ln_st, int act,
+                                                 bool has_res, __half2 res) {
+  if (COLS == EPI_LN) {
     // LayerNorm folded into the GEMM: acc = sum_k W'[n,k] x[m,k] with W' = W diag(gamma), so
     // W LN(x) + bias = rstd * (acc - mean * c[n]) + b'[n]   (fp32, one rounding to fp16 below)
-    const float c0 = p.ln_c[n], b0 = p.ln_b[n];
-    const float c1 = pair_ok ? p.ln_c[n + 1] : 0.0f, b1 = pair_ok ? p.ln_b[n + 1] : 0.0f;
-    v0 = fmaf(ln_st.y, fmaf(-ln_st.x, c0, v0), b0);
-    v1 = fmaf(ln_st.y, fmaf(-ln_st.x, c1, v1), b1);
-  } else if (p.bias != nullptr) {
-    v0 += __half2float(p.bias[n]);
-    if (pair_ok) v1 += __half2float(p.bias[n + 1]);
+    v0 = fmaf(ln_st.y, fmaf(-ln_st.x, c.x, v0), b.x);
+    v1 = fmaf(ln_st.y, fmaf(-ln_st.x, c.y, v1), b.y);
+  } else if (COLS == EPI_BIAS) {
+    v0 += b.x;
+    v1 += b.y;
   }
   __half h0 = __float2half_rn(v0), h1 = __float2half_rn(v1);
-  if (p.act != SEEDB200_ACT_NONE) {
-    h0 = __float2half_rn(apply_act(__half2float(h0), p.act));
-    h1 = __float2half_rn(apply_act(__half2float(h1), p.act));
+  if (act != SEEDB200_ACT_NONE) {
+    h0 = __float2half_rn(apply_act(__half2float(h0), act));
+    h1 = __float2half_rn(apply_act(__half2float(h1), act));
   }
-  if (res_row != nullptr) {
-    h0 = __float2half_rn(__half2float(h0) + __half2float(res_row[n]));
-    if (pair_ok) h1 = __float2half_rn(__half2float(h1) + __half2float(res_row[n + 1]));
+  if (has_res) {
+    h0 = __float2half_rn(__half2float(h0) + __half2float(__low2half(res)));
+    h1 = __float2half_rn(__half2float(h1) + __half2float(__high2half(res)));
   }
   return __halves2half2(h0, h1);
 }
@@ -229,6 +234,99 @@ __device__ __forceinline__ void store_pair(__half* op, __half2 h, bool pair_ok) 
     op[0] = __low2half(h);
     if (pair_ok) op[1] = __high2half(h);
   }
+}
+
+__device__ __forceinline__ __half2 load_pair(const __half* ip, bool pair_ok) {
+  if (pair_ok && (reinterpret_cast<uintptr_t>(ip) & 3) == 0) return *reinterpret_cast<const __half2*>(ip);
+  return __halves2half2(ip[0], pair_ok ? ip[1] : __float2half_rn(0.0f));
+}
+
+// Output row of GEMM row m (row remap of the patch embed) and the residual row it adds
+__device__ __forceinline__ long long out_row_of(const GemmParams& p, int m) {
+  return p.row_group > 0 ? (long long)(m / p.row_group) * p.row_stride + (m % p.row_group) + p.row_offset : m;
+}
+__device__ __forceinline__ long long res_row_of(const GemmParams& p, int m) {
+  return p.res_mod > 0 ? (long long)(m % p.res_mod) + p.res_offset : out_row_of(p, m);
+}
+
+// MODE 0 epilogue of one tile for one consumer thread: rows m0 and m0 + 8 (row_ok, out_row, res_row per row), per
+// 8-column group j the columns n0 + 8 j + col_in_pair (+1).  One 64-column chunk per call, J0 = its first group;
+// the chunks are unrolled by recursion so that acc stays in registers.  The chunk's residual is loaded for both rows
+// before any of its results is stored (the output may be the residual, so the compiler cannot hoist these loads
+// above the stores itself): one memory latency per chunk instead of one per column pair.
+template <int BN, int COLS, int J0>
+__device__ __forceinline__ void epilogue_chunks(const GemmParams& p, const float (&acc)[BN / 2], int m0, int n0,
+                                                int col_in_pair, int lane, const float* col_c, const float* col_b,
+                                                const float2 (&ln_st)[2], const bool (&row_ok)[2],
+                                                __half* const (&out_row)[2], const __half* const (&res_row)[2]) {
+  constexpr int NJ = BN / 8, CH = 8;
+  if constexpr (J0 < NJ) {
+    const bool has_res = p.residual != nullptr;
+    __half2 rv[2][CH];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int jj = 0; jj < CH; ++jj) {
+        const int n = n0 + 8 * (J0 + jj) + col_in_pair;
+        rv[h][jj] = __float2half2_rn(0.0f);
+        if (has_res && J0 + jj < NJ && row_ok[h] && n < p.N) rv[h][jj] = load_pair(res_row[h] + n, n + 1 < p.N);
+      }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mom_s = 0.0f, mom_q = 0.0f;
+#pragma unroll
+      for (int jj = 0; jj < CH && J0 + jj < NJ; ++jj) {
+        const int j = J0 + jj;
+        const int nl = 8 * j + col_in_pair, n = n0 + nl;
+        const bool col_ok = row_ok[h] && n < p.N;
+        __half2 o = __float2half2_rn(0.0f);
+        if (col_ok) {
+          float2 c = make_float2(0.0f, 0.0f), b = make_float2(0.0f, 0.0f);
+          if (COLS == EPI_LN) c = *reinterpret_cast<const float2*>(col_c + nl);
+          if (COLS != EPI_NONE) b = *reinterpret_cast<const float2*>(col_b + nl);
+          o = epilogue_pair<COLS>(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], c, b, ln_st[h], p.act, has_res,
+                                  rv[h][jj]);
+          store_pair(out_row[h] + n, o, n + 1 < p.N);
+        }
+        if (p.row_moments != nullptr) {
+          const float2 f = __half22float2(o);
+          mom_s += f.x + f.y;
+          mom_q = fmaf(f.x, f.x, mom_q);
+          mom_q = fmaf(f.y, f.y, mom_q);
+          if ((j & 7) == 7) {          // a 64-column group is complete: reduce over the 4 threads of the row
+            mom_s += __shfl_xor_sync(0xffffffffu, mom_s, 1);
+            mom_q += __shfl_xor_sync(0xffffffffu, mom_q, 1);
+            mom_s += __shfl_xor_sync(0xffffffffu, mom_s, 2);
+            mom_q += __shfl_xor_sync(0xffffffffu, mom_q, 2);
+            // a last tile that reaches past N (N % BN != 0) has groups beyond the row: they belong to no one
+            const int groups = p.N >> 6, g = (n0 >> 6) + (j >> 3);
+            if (row_ok[h] && (lane & 3) == 0 && g < groups)
+              p.row_moments[(long long)(m0 + 8 * h) * groups + g] = make_float2(mom_s, mom_q);
+            mom_s = 0.0f; mom_q = 0.0f;
+          }
+        }
+      }
+    }
+    epilogue_chunks<BN, COLS, J0 + CH>(p, acc, m0, n0, col_in_pair, lane, col_c, col_b, ln_st, row_ok, out_row,
+                                       res_row);
+  }
+}
+
+template <int BN, int COLS>
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[BN / 2], int m0, int n0,
+                                              int col_in_pair, int lane, const float* col_c, const float* col_b,
+                                              const float2 (&ln_st)[2]) {
+  bool row_ok[2];
+  __half* out_row[2];
+  const __half* res_row[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = m0 + 8 * h;
+    row_ok[h] = m < p.M;
+    out_row[h] = p.out + out_row_of(p, m) * p.ldo;
+    res_row[h] = (p.residual != nullptr && row_ok[h]) ? p.residual + res_row_of(p, m) * p.ldr : nullptr;
+  }
+  epilogue_chunks<BN, COLS, 0>(p, acc, m0, n0, col_in_pair, lane, col_c, col_b, ln_st, row_ok, out_row, res_row);
 }
 
 template <int BN, int MODE>
@@ -244,6 +342,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const uint32_t smem_b = smem_base + STAGES * Cfg::A_BYTES;
   const uint32_t full_bar = smem_base + STAGES * Cfg::STAGE_BYTES;   // [STAGES]
   const uint32_t empty_bar = full_bar + STAGES * 8;                  // [STAGES]
+  const uint32_t col_vecs = empty_bar + STAGES * 8;                // epilogue column vectors, 2 x 2 x BN floats
 
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int lane = threadIdx.x & 31;
@@ -292,12 +391,41 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const int row_in_tile = (wg - 1) * 64 + cw * 16 + (lane >> 2);
   const int col_in_pair = (lane & 3) * 2;
   const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;   // this warpgroup's 64 rows of the A stage
+  const int ct = threadIdx.x - 128;               // 0 .. 255 over both consumer warpgroups
+  const int cols = p.ln_stats != nullptr ? EPI_LN : p.bias != nullptr ? EPI_BIAS : EPI_NONE;
+  float* col_smem = reinterpret_cast<float*>(smem_raw + (col_vecs - smem_u32(smem_raw)));   // [2][c | b][BN]
   int stage = 0; uint32_t phase = 0;
   float acc[BN / 2];
   for (int round = 0;; ++round) {
     const int tile = tile_of(round);
     if (tile >= total_tiles) break;
     const int mt = tile / p.n_tiles, nt = tile % p.n_tiles;
+    const int n0 = nt * BN;
+    // MODE 0: fetch what the epilogue reads besides the accumulators while the k-loop runs -- this thread's column of
+    // ln_c / ln_b or bias (staged in shared memory after the k-loop), its rows' LayerNorm statistics, and the tile's
+    // residual rows into L2
+    float col_c = 0.0f, col_b = 0.0f;
+    float2 ln_st[2] = {make_float2(0.0f, 1.0f), make_float2(0.0f, 1.0f)};
+    if constexpr (MODE == 0) {
+      if (ct < BN && n0 + ct < p.N) {
+        if (cols == EPI_LN) { col_c = p.ln_c[n0 + ct]; col_b = p.ln_b[n0 + ct]; }
+        else if (cols == EPI_BIAS) col_b = __half2float(p.bias[n0 + ct]);
+      }
+      if (cols == EPI_LN) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = mt * GEMM_BLOCK_M + row_in_tile + 8 * h;
+          if (m < p.M) ln_st[h] = p.ln_stats[m];
+        }
+      }
+      const int m = mt * GEMM_BLOCK_M + (ct >> 1);
+      if (p.residual != nullptr && m < p.M) {
+        const uintptr_t lo = reinterpret_cast<uintptr_t>(p.residual + res_row_of(p, m) * p.ldr + n0);
+        const uintptr_t hi = lo + 2 * (uintptr_t)min(BN, p.N - n0);
+        for (uintptr_t a = (lo & ~(uintptr_t)127) + (ct & 1) * 128; a < hi; a += 256)
+          prefetch_l2(reinterpret_cast<const void*>(a));
+      }
+    }
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
     int prev_stage = -1;
@@ -326,16 +454,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
 
     // ---- epilogue: thread holds rows r, r + 8 and, per 8-column group j, columns 8 j + col_in_pair (+1) ----
+    const int m0 = mt * GEMM_BLOCK_M + row_in_tile;
+    if constexpr (MODE == 1) {
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = mt * GEMM_BLOCK_M + row_in_tile + 8 * h;
-      const bool row_ok = m < p.M;
-      long long orow = m;
-      if (p.row_group > 0) orow = (long long)(m / p.row_group) * p.row_stride + (m % p.row_group) + p.row_offset;
-      long long rrow = orow;
-      if (p.res_mod > 0) rrow = (m % p.res_mod) + p.res_offset;
-      __half* out_row = p.out + orow * p.ldo;
-      if constexpr (MODE == 1) {
+      for (int h = 0; h < 2; ++h) {
+        const int m = m0 + 8 * h;
+        const bool row_ok = m < p.M;
+        __half* out_row = p.out + out_row_of(p, m) * p.ldo;
         // SiLU-gate: columns [0,128) of the tile are gates, [128,256) the matching ups.
         // silu(fp16(gate)) rounded to fp16, times fp16(up), rounded (llama_xformer.py:186)
         const int n_limit = p.N / 2;
@@ -352,39 +477,19 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           const int n = nt * (BN / 2) + 8 * j + col_in_pair;
           if (row_ok && n < n_limit) store_pair(out_row + n, __halves2half2(o[0], o[1]), n + 1 < n_limit);
         }
-      } else {
-        const __half* res_row = (p.residual != nullptr && row_ok) ? p.residual + rrow * p.ldr : nullptr;
-        float2 ln_st = make_float2(0.0f, 1.0f);
-        if (p.ln_stats != nullptr && row_ok) ln_st = p.ln_stats[m];
-        float mom_s = 0.0f, mom_q = 0.0f;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int n = nt * BN + 8 * j + col_in_pair;
-          const bool col_ok = row_ok && n < p.N;
-          __half2 o = __float2half2_rn(0.0f);
-          if (col_ok) {
-            o = epilogue_pair(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], n, n + 1 < p.N, ln_st, res_row);
-            store_pair(out_row + n, o, n + 1 < p.N);
-          }
-          if (p.row_moments != nullptr) {
-            const float2 f = __half22float2(o);
-            mom_s += f.x + f.y;
-            mom_q = fmaf(f.x, f.x, mom_q);
-            mom_q = fmaf(f.y, f.y, mom_q);
-            if ((j & 7) == 7) {          // a 64-column group is complete: reduce over the 4 threads of the row
-              mom_s += __shfl_xor_sync(0xffffffffu, mom_s, 1);
-              mom_q += __shfl_xor_sync(0xffffffffu, mom_q, 1);
-              mom_s += __shfl_xor_sync(0xffffffffu, mom_s, 2);
-              mom_q += __shfl_xor_sync(0xffffffffu, mom_q, 2);
-              // a last tile that reaches past N (N % BN != 0) has groups beyond the row: they belong to no one
-              const int groups = p.N >> 6, g = ((nt * BN) >> 6) + (j >> 3);
-              if (row_ok && (lane & 3) == 0 && g < groups)
-                p.row_moments[(long long)m * groups + g] = make_float2(mom_s, mom_q);
-              mom_s = 0.0f; mom_q = 0.0f;
-            }
-          }
-        }
       }
+    } else {
+      // this tile's column vectors: visible to both consumer warpgroups once all 256 threads have stored theirs.
+      // Double-buffered by round: a thread writes buffer (round & 1) only after the previous round's barrier, which
+      // every reader of that buffer two rounds ago passed after its epilogue.
+      float* colv = col_smem + (round & 1) * 2 * BN;
+      if (cols != EPI_NONE) {
+        if (ct < BN) { colv[ct] = col_c; colv[BN + ct] = col_b; }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+      }
+      if (cols == EPI_LN) epilogue_tile<BN, EPI_LN>(p, acc, m0, n0, col_in_pair, lane, colv, colv + BN, ln_st);
+      else if (cols == EPI_BIAS) epilogue_tile<BN, EPI_BIAS>(p, acc, m0, n0, col_in_pair, lane, colv, colv + BN, ln_st);
+      else epilogue_tile<BN, EPI_NONE>(p, acc, m0, n0, col_in_pair, lane, colv, colv + BN, ln_st);
     }
   }
 }
