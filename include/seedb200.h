@@ -37,7 +37,7 @@ enum seedb200_status {
   SEEDB200_ERR_UNSUPPORTED = 3
 };
 
-enum seedb200_dtype { SEEDB200_F16 = 0, SEEDB200_F32 = 1, SEEDB200_I64 = 2, SEEDB200_I32 = 3 };
+enum seedb200_dtype { SEEDB200_F16 = 0, SEEDB200_F32 = 1, SEEDB200_I64 = 2, SEEDB200_I32 = 3, SEEDB200_I8 = 4 };
 
 enum seedb200_act { SEEDB200_ACT_NONE = 0, SEEDB200_ACT_GELU = 1, SEEDB200_ACT_TANH = 2, SEEDB200_ACT_RELU = 3 };
 
@@ -209,6 +209,49 @@ int seedb200_embedding(const void* table, int64_t ld, const int64_t* ids, int n,
 int seedb200_gemv(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w,
                   float eps, int M, int N, int K, int mode, void* stream);
 
+/* ---- LLM.int8() linear layers (transformers load_in_8bit=True: bitsandbytes Linear8bitLt, has_fp16_weights=False) ----
+ * Weights are quantised once:  SCB[n] = max_k |W[n,k]| (fp32),  CB[n,k] = rint(W[n,k] * (127 / SCB[n])) (int8,
+ * half to even; 0 for a row with SCB 0).  Activations per call: element (m,k) is an outlier when !(|A[m,k]| <
+ * threshold) (NaN and inf are outliers); the outlier set O is every column holding an outlier in any row;
+ * SCA[m] = max |A[m,k]| over the row's non-outlier elements; CA[m,k] = rint(A[m,k] * (127 / SCA[m])), 0 for k in O
+ * and when SCA[m] == 0.  Output, with acc = sum_k CA[m,k] CB[n,k] in int32:
+ *   base = fp16(((float)acc * 6.200012e-05f) * SCA[m] * SCB[n])
+ *   y    = O empty ? base : fp16(base + fp16(sum_{j in O ascending} A[m,j] * fp16(CB[n,j] * SCB[n] / 127)))
+ * then mode 0 adds the residual (fp16(y + r)) and mode 1 applies SiLU-gate to the fp16 gate and up values.
+ * The GEMM (any M) and the GEMV (M <= 4) produce the same bits.                                                   */
+/* W fp16 [N,K] (row stride ldw elements) -> CB int8 [N,K] packed, SCB fp32 [N].  One block per row.              */
+int seedb200_int8_quantize_weight(const void* W, int64_t ldw, int N, int K, void* CB, void* SCB, void* stream);
+/* A fp16 [M,K] (row stride lda) -> CA int8 [M,K] packed, SCA fp32 [M], outliers int32 [K] (capacity K: the outlier
+ * columns in ascending order) and *n_outliers (device int32).  No host synchronisation: graph capturable.  K % 8 == 0. */
+int seedb200_int8_quantize_act(const void* A, int64_t lda, int M, int K, float threshold, void* CA, void* SCA,
+                               int32_t* outliers, int32_t* n_outliers, void* stream);
+/* out = epilogue(linear8(A, W)) by the int8 wgmma GEMM: CA / SCA / outliers / n_outliers as quantize_act left them,
+ * A16 the fp16 activations they came from (read at the outlier columns), W = CB and SCB of quantize_weight.
+ * Leading dimensions in elements, 0 = packed.  K % 16 == 0; mode 1 needs N % 256 == 0 (W rows in blocks of
+ * [128 gate | 128 up]) and no residual.  bn: tile width 64, 128 or 256, 0 = auto.  Two launches: the outlier
+ * correction as a dense product over the gathered outlier columns (into workspace), then the GEMM.              */
+typedef struct seedb200_gemm_int8_desc {
+  int32_t M, N, K;
+  const void* A;   int64_t lda;       /* int8 CA [M,K]                             */
+  const void* SCA;                    /* fp32 [M]                                  */
+  const void* A16; int64_t lda16;     /* fp16 [M,K]                                */
+  const int32_t* outliers;            /* ascending outlier columns                 */
+  const int32_t* n_outliers;          /* device int32: how many                    */
+  const void* W;   int64_t ldw;       /* int8 CB [N,K]                             */
+  const void* SCB;                    /* fp32 [N]                                  */
+  void* out;       int64_t ldo;       /* fp16 [M, N] (N/2 columns in mode 1)       */
+  const void* residual; int64_t ldr;  /* fp16 or NULL, mode 0 only                 */
+  int32_t mode;
+  int32_t bn;
+  void* workspace;                    /* fp16 [M,N]: the outlier corrections   */
+} seedb200_gemm_int8_desc;
+int seedb200_gemm_int8(const seedb200_gemm_int8_desc* d, void* stream);
+/* The same for M <= 4 rows from fp16 x [M,K] (packed): the activation quantisation (and, with norm_w, the RMSNorm of
+ * seedb200_gemv) happens while the rows are staged in shared memory; W = CB [N,K] packed, SCB [N]; out [M,N] packed
+ * ([M,N/2] in mode 1), residual [M,N] or NULL.  K % 16 == 0.                                                    */
+int seedb200_gemv_int8(const void* x, const void* norm_w, float eps, float threshold, const void* W, const void* SCB,
+                       void* out, const void* residual, int M, int N, int K, int mode, void* stream);
+
 /* LlamaAttention.forward with q_len == 1 (llama_xformer.py:240-256, attn_bias=None): q [B,H,D] against the first
  * kv_len rows of caches laid out [B,H,max_seq,D]; out [B,H*D] fp16; D must be 128.  workspace: at least
  * seedb200_decode_attention_workspace_bytes(B, H, max_seq) bytes of device memory (split-KV partials).          */
@@ -311,6 +354,20 @@ typedef struct seedb200_llama_config {
 
 int seedb200_llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
                           seedb200_llama** out);
+/* The same model with LLM.int8() decoder linears (transformers LlamaForCausalLM.from_pretrained(load_in_8bit=True)):
+ * q/k/v/o_proj and gate/up/down_proj of every layer come as "<name>.weight" SEEDB200_I8 [N,K] (CB) plus
+ * "<name>.SCB" SEEDB200_F32 [N] (bitsandbytes' state-dict names, seedb200_int8_quantize_weight's output); every other
+ * tensor is fp16 as for seedb200_llama_create.  The int8 weights and scales are copied into the handle (the caller
+ * may free them after this call); the fp16 tensors are borrowed.  threshold: the outlier threshold (6.0).
+ * A linear given with neither tensor is loaded later with seedb200_llama_int8_load_weight.                     */
+int seedb200_llama_create_int8(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
+                               float threshold, seedb200_llama** out);
+/* Quantises the fp16 weight `name` (a decoder linear, e.g. "model.layers.3.mlp.up_proj.weight", [N,K] with row
+ * stride ldw elements, 0 = K) straight into the handle's fused int8 layout.  create_int8 accepts a linear with
+ * neither "<name>.weight" nor "<name>.SCB"; it must then be loaded this way before the first forward / generate
+ * (which refuse otherwise).  Loading one fp16 tensor at a time keeps device memory at the int8 model plus that
+ * tensor.  Enqueued on `stream`; W may be freed once the stream has passed this call.                          */
+int seedb200_llama_int8_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream);
 void seedb200_llama_destroy(seedb200_llama* llm);
 
 /* LlamaForCausalLM.forward (llama_xformer.py:661-743).  input_ids [B,S] int64

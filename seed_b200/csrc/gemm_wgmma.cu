@@ -20,6 +20,8 @@
 #include <stdio.h>
 
 #include "common.cuh"
+#include "int8.cuh"
+#include "ops.h"
 
 namespace sb {
 
@@ -195,6 +197,28 @@ template <> __device__ __forceinline__ void wgmma_f16<256>(float (&d)[128], uint
   asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
                "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n}\n"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+               : "l"(a), "l"(b));
+}
+
+// D[64 x N] += A[64 x 32] . B[N x 32]^T, int8 operands K-major in shared memory, int32 accumulators
+template <int N>
+__device__ __forceinline__ void wgmma_s8(int (&d)[N / 2], uint64_t a, uint64_t b);
+template <> __device__ __forceinline__ void wgmma_s8<64>(int (&d)[32], uint64_t a, uint64_t b) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n}\n"
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+               : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_s8<128>(int (&d)[64], uint64_t a, uint64_t b) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p;\n}\n"
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+               : "l"(a), "l"(b));
+}
+template <> __device__ __forceinline__ void wgmma_s8<256>(int (&d)[128], uint64_t a, uint64_t b) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, 1, 0;\n"
+               "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p;\n}\n"
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]), "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63]), "+r"(d[64]), "+r"(d[65]), "+r"(d[66]), "+r"(d[67]), "+r"(d[68]), "+r"(d[69]), "+r"(d[70]), "+r"(d[71]), "+r"(d[72]), "+r"(d[73]), "+r"(d[74]), "+r"(d[75]), "+r"(d[76]), "+r"(d[77]), "+r"(d[78]), "+r"(d[79]), "+r"(d[80]), "+r"(d[81]), "+r"(d[82]), "+r"(d[83]), "+r"(d[84]), "+r"(d[85]), "+r"(d[86]), "+r"(d[87]), "+r"(d[88]), "+r"(d[89]), "+r"(d[90]), "+r"(d[91]), "+r"(d[92]), "+r"(d[93]), "+r"(d[94]), "+r"(d[95]), "+r"(d[96]), "+r"(d[97]), "+r"(d[98]), "+r"(d[99]), "+r"(d[100]), "+r"(d[101]), "+r"(d[102]), "+r"(d[103]), "+r"(d[104]), "+r"(d[105]), "+r"(d[106]), "+r"(d[107]), "+r"(d[108]), "+r"(d[109]), "+r"(d[110]), "+r"(d[111]), "+r"(d[112]), "+r"(d[113]), "+r"(d[114]), "+r"(d[115]), "+r"(d[116]), "+r"(d[117]), "+r"(d[118]), "+r"(d[119]), "+r"(d[120]), "+r"(d[121]), "+r"(d[122]), "+r"(d[123]), "+r"(d[124]), "+r"(d[125]), "+r"(d[126]), "+r"(d[127])
                : "l"(a), "l"(b));
 }
 
@@ -494,6 +518,170 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   }
 }
 
+// ---- int8 operands (LLM.int8(), seedb200_gemm_int8) ----------------------------------------------------------------
+// The same warp-specialised TMA / mbarrier pipeline over int8 rows: a 128-byte swizzled row holds 128 int8 values,
+// so a stage is BK = 128 deep with the byte layout of the fp16 kernel's 64-deep stage, and its four 32-byte k-steps
+// are wgmma m64nBNk32 s8 x s8 -> s32.  The epilogue dequantises, adds the outlier correction and then applies the
+// residual (mode 0) or SiLU-gate (mode 1), with the rounding points of int8.cuh.  The outlier correction is computed
+// before it by int8_correction (a dense product over the gathered outlier columns) and read from `corr`.
+struct GemmI8Params {
+  int M, N, K;
+  int m_tiles, n_tiles;
+  const float* sca;                    // [M] activation row scales
+  const float* scb;                    // [N] weight row scales
+  const __half* corr; long long ldc;   // [M,N] outlier corrections (int8_correction), read when there are outliers
+  const int* n_outliers;
+  const __half* residual; long long ldr;
+  __half* out; long long ldo;
+};
+
+template <int R>
+__device__ __forceinline__ void acc_fence_i(int (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+template <int BN, int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_i8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+               const GemmI8Params p) {
+  using Cfg = GemmCfg<BN>;             // 128 x 128 int8 = 128 x 64 fp16 bytes: the fp16 kernel's stage sizes
+  constexpr int STAGES = Cfg::STAGES;
+  constexpr int BK = 128;
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t smem_a = smem_base;
+  const uint32_t smem_b = smem_base + STAGES * Cfg::A_BYTES;
+  const uint32_t full_bar = smem_base + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t empty_bar = full_bar + STAGES * 8;
+
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
+  const int lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar + 8 * s, 1);
+      mbar_init(empty_bar + 8 * s, 8);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int num_kb = (p.K + BK - 1) / BK;
+  const int total_tiles = p.m_tiles * p.n_tiles;
+
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      int stage = 0; uint32_t phase = 0;
+      for (int round = 0;; ++round) {
+        const int tile = sched_tile(0, round, blockIdx.x, gridDim.x, p.m_tiles, p.n_tiles, 0);
+        if (tile >= total_tiles) break;
+        const int m_idx = (tile / p.n_tiles) * GEMM_BLOCK_M, n_idx = (tile % p.n_tiles) * BN;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait_relaxed_nocall(empty_bar + 8 * stage, phase ^ 1);
+          mbar_arrive_expect_tx(full_bar + 8 * stage, (uint32_t)Cfg::STAGE_BYTES);
+          tma_load_2d(smem_a + stage * Cfg::A_BYTES, &tmap_a, full_bar + 8 * stage, kb * BK, m_idx);
+          tma_load_2d(smem_b + stage * Cfg::B_BYTES, &tmap_b, full_bar + 8 * stage, kb * BK, n_idx);
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+    return;
+  }
+
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int cw = (threadIdx.x >> 5) & 3;
+  const int row_in_tile = (wg - 1) * 64 + cw * 16 + (lane >> 2);
+  const int col_in_pair = (lane & 3) * 2;
+  const uint32_t a_off = (uint32_t)(wg - 1) * 64 * 128;
+  const int cnt = *p.n_outliers;
+  int stage = 0; uint32_t phase = 0;
+  int acc[BN / 2];
+  for (int round = 0;; ++round) {
+    const int tile = sched_tile(0, round, blockIdx.x, gridDim.x, p.m_tiles, p.n_tiles, 0);
+    if (tile >= total_tiles) break;
+    const int mt = tile / p.n_tiles, nt = tile % p.n_tiles;
+    const int n0 = nt * BN;
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
+    int prev_stage = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait_nocall(full_bar + 8 * stage, phase);
+      wgmma_fence();
+      const uint64_t adesc = wgmma_desc_sw128(smem_a + stage * Cfg::A_BYTES + a_off);
+      const uint64_t bdesc = wgmma_desc_sw128(smem_b + stage * Cfg::B_BYTES);
+#pragma unroll
+      for (int k = 0; k < BK / 32; ++k) wgmma_s8<BN>(acc, adesc + 2 * k, bdesc + 2 * k);   // +32 bytes per k-step
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_stage >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+      }
+      prev_stage = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    acc_fence_i(acc);
+    if (prev_stage >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+    }
+
+    // ---- epilogue: rows m0, m0 + 8; per 8-column group j the columns 8 j + col_in_pair (+1) of the tile ----
+    const int m0 = mt * GEMM_BLOCK_M + row_in_tile;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + 8 * h;
+      if (m >= p.M) continue;
+      const float sa = p.sca[m];
+      const __half* crow = p.corr + (long long)m * p.ldc;
+      __half* orow = p.out + (long long)m * p.ldo;
+      if constexpr (MODE == 1) {
+        // columns [0,128) of the tile are gates, [128,256) the matching ups
+#pragma unroll
+        for (int j = 0; j < BN / 16; ++j) {
+          __half o[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int ng = n0 + 8 * j + col_in_pair + e, nu = ng + 128;
+            const float sg = p.scb[ng], su = p.scb[nu];
+            float g = int8_base(acc[4 * j + 2 * h + e], sa, sg), u = int8_base(acc[4 * (j + BN / 16) + 2 * h + e], sa, su);
+            const __half gh = cnt ? int8_add_corr(g, crow[ng]) : __float2half_rn(g);
+            const __half uh = cnt ? int8_add_corr(u, crow[nu]) : __float2half_rn(u);
+            o[e] = int8_silu_mul(gh, uh);
+          }
+          const int n = nt * (BN / 2) + 8 * j + col_in_pair;
+          store_pair(orow + n, __halves2half2(o[0], o[1]), true);
+        }
+      } else {
+        const __half* rrow = p.residual != nullptr ? p.residual + (long long)m * p.ldr : nullptr;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int n = n0 + 8 * j + col_in_pair;
+          if (n >= p.N) continue;
+          __half o[2] = {__float2half_rn(0.0f), __float2half_rn(0.0f)};
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (n + e < p.N) {
+              const float sb = p.scb[n + e];
+              const float b = int8_base(acc[4 * j + 2 * h + e], sa, sb);
+              __half y = cnt ? int8_add_corr(b, crow[n + e]) : __float2half_rn(b);
+              if (rrow != nullptr) y = __float2half_rn(__half2float(y) + __half2float(rrow[n + e]));
+              o[e] = y;
+            }
+          }
+          store_pair(orow + n, __halves2half2(o[0], o[1]), n + 1 < p.N);
+        }
+      }
+    }
+  }
+}
+
 // ----------------------------------------------------------------------------
 // host side
 // ----------------------------------------------------------------------------
@@ -515,20 +703,23 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// fp16 [rows, cols] row-major with leading dimension ld (elements); box = box_rows x 64 columns, 128B swizzle
-static int make_tmap(CUtensorMap* tm, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows) {
+// [rows, cols] row-major with leading dimension ld (elements of esize bytes: fp16 by default, int8 for the int8 GEMM);
+// box = box_rows x one 128-byte row (64 fp16 or 128 int8 columns), 128B swizzle
+static int make_tmap(CUtensorMap* tm, const void* ptr, int64_t rows, int64_t cols, int64_t ld, int box_rows,
+                     CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16, int esize = 2) {
   EncodeTiledFn fn = get_encode_fn();
   if (fn == nullptr) {
     set_error("cuTensorMapEncodeTiled entry point not available (no CUDA driver?)");
     return SEEDB200_ERR_CUDA;
   }
   SB_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "gemm: operand pointer %p not 16-byte aligned", ptr);
-  SB_REQUIRE((ld * 2) % 16 == 0, "gemm: leading dimension %lld (elements) is not a multiple of 8", (long long)ld);
+  SB_REQUIRE((ld * esize) % 16 == 0, "gemm: leading dimension %lld (elements) is not a multiple of %d", (long long)ld,
+             16 / esize);
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)ld * 2};
-  cuuint32_t box[2] = {(cuuint32_t)GEMM_BLOCK_K, (cuuint32_t)box_rows};
+  cuuint64_t gstr[1] = {(cuuint64_t)ld * esize};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), gdim, gstr, box, estr,
+  CUresult r = fn(tm, dtype, 2, const_cast<void*>(ptr), gdim, gstr, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -712,7 +903,76 @@ int gemm(const seedb200_gemm_desc& desc, cudaStream_t stream) {
   return SEEDB200_ERR_UNSUPPORTED;
 }
 
+// ---- int8 GEMM host side ----
+template <int BN, int MODE>
+static int launch_gemm_i8(const seedb200_gemm_int8_desc& d, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN>;
+  static bool attr_set_dev[SB_MAX_DEVICES] = {};
+  bool& attr_set = attr_set_dev[cur_device()];
+  auto kern = gemm_i8_kernel<BN, MODE>;
+  if (!attr_set) {
+    SB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    attr_set = true;
+  }
+  CUtensorMap ta, tb;
+  SB_PROPAGATE(make_tmap(&ta, d.A, d.M, d.K, d.lda, GEMM_BLOCK_M, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1));
+  SB_PROPAGATE(make_tmap(&tb, d.W, d.N, d.K, d.ldw, BN, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1));
+  const TileSchedule ts = make_schedule(d.M, d.N, BN, 0, num_sms());
+  GemmI8Params p;
+  p.M = d.M; p.N = d.N; p.K = d.K;
+  p.m_tiles = ts.m_tiles; p.n_tiles = ts.n_tiles;
+  p.sca = static_cast<const float*>(d.SCA);
+  p.scb = static_cast<const float*>(d.SCB);
+  p.corr = static_cast<const __half*>(d.workspace); p.ldc = d.N;
+  p.n_outliers = d.n_outliers;
+  p.residual = static_cast<const __half*>(d.residual); p.ldr = d.ldr;
+  p.out = static_cast<__half*>(d.out); p.ldo = d.ldo;
+  kern<<<ts.units, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p);
+  SB_LAUNCH_CHECK();
+  return 0;
+}
+
+int gemm_int8(const seedb200_gemm_int8_desc& desc, cudaStream_t stream) {
+  seedb200_gemm_int8_desc d = desc;
+  SB_REQUIRE(d.M > 0 && d.N > 0 && d.K > 0, "gemm_int8: non-positive shape M=%d N=%d K=%d", d.M, d.N, d.K);
+  SB_REQUIRE(d.mode == 0 || d.mode == 1, "gemm_int8: unknown mode %d", d.mode);
+  SB_REQUIRE(d.K % 16 == 0, "gemm_int8: K=%d must be a multiple of 16 (16-byte TMA rows)", d.K);
+  SB_REQUIRE(d.mode == 0 || (d.N % 256 == 0 && d.residual == nullptr),
+             "gemm_int8: SiLU-gate mode needs N %% 256 == 0 and no residual");
+  const int n_out = d.mode == 1 ? d.N / 2 : d.N;
+  if (d.lda == 0) d.lda = d.K;
+  if (d.ldw == 0) d.ldw = d.K;
+  if (d.lda16 == 0) d.lda16 = d.K;
+  if (d.ldo == 0) d.ldo = n_out;
+  if (d.ldr == 0) d.ldr = n_out;
+  SB_REQUIRE(d.lda >= d.K && d.ldw >= d.K && d.lda16 >= d.K, "gemm_int8: a leading dimension is below K=%d", d.K);
+  SB_REQUIRE(d.ldo >= n_out && (d.residual == nullptr || d.ldr >= n_out),
+             "gemm_int8: ldo / ldr below the %d output columns", n_out);
+  SB_REQUIRE(d.A && d.SCA && d.A16 && d.outliers && d.n_outliers && d.W && d.SCB && d.out && d.workspace,
+             "gemm_int8: null operand");
+  int bn = d.bn;
+  if (bn == 0) bn = d.mode == 1 ? 256 : d.N % 256 == 0 ? 256 : d.N <= 64 ? 64 : 128;
+  SB_REQUIRE(d.mode == 0 || bn == 256, "gemm_int8: SiLU-gate mode needs bn 256");
+  SB_REQUIRE(bn == 256 || bn == 128 || bn == 64, "gemm_int8: unsupported tile width bn=%d (64, 128 or 256)", bn);
+  SB_PROPAGATE(int8_correction(d.A16, d.lda16, d.W, d.ldw, d.SCB, d.outliers, d.n_outliers, d.M, d.N, d.workspace,
+                               stream));
+  if (bn == 256 && d.mode == 1) return launch_gemm_i8<256, 1>(d, stream);
+  if (bn == 256) return launch_gemm_i8<256, 0>(d, stream);
+  if (bn == 128) return launch_gemm_i8<128, 0>(d, stream);
+  if (bn == 64) return launch_gemm_i8<64, 0>(d, stream);
+  set_error("gemm_int8: unsupported tile width bn=%d (64, 128 or 256)", bn);
+  return SEEDB200_ERR_UNSUPPORTED;
+}
+
 }  // namespace sb
+
+extern "C" int seedb200_gemm_int8(const seedb200_gemm_int8_desc* d, void* stream) {
+  if (d == nullptr) {
+    sb::set_error("seedb200_gemm_int8: null descriptor");
+    return SEEDB200_ERR_INVALID;
+  }
+  return sb::gemm_int8(*d, static_cast<cudaStream_t>(stream));
+}
 
 extern "C" int seedb200_gemm_plan(const seedb200_gemm_desc* d, int sms, int32_t* out9) {
   if (d == nullptr || out9 == nullptr || sms <= 0) {

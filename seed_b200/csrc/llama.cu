@@ -12,6 +12,10 @@
 // Weights named like the HF checkpoint (model.layers.N.self_attn.q_proj.weight ...).  o_proj, down_proj,
 // norms, embed_tokens and lm_head are borrowed; q/k/v and gate/up are copied into their fused layouts and
 // the originals are not referenced after create.
+// int8 mode (seedb200_llama_create_int8, LLM.int8()): the seven decoder linears of every layer arrive as int8 CB plus
+// fp32 SCB and are copied into handle-owned fused layouts (q|k|v concatenated, gate|up interleaved in 128-row blocks,
+// the scales the same way); lin8() sends them to the int8 GEMV (<= 4 rows) or quantises the activations and runs the
+// int8 wgmma GEMM.
 #include <string.h>
 
 #include <map>
@@ -25,6 +29,9 @@ namespace sb {
 struct LlamaLayerW {
   const __half *in_ln, *post_ln, *qkv_w, *o_w, *gu_w, *down_w;
   __half *k_cache, *v_cache;
+  // int8 mode: CB [N,K] and SCB [N] of the fused projections
+  const int8_t *qkv8, *o8, *gu8, *down8;
+  const float *qkv_s, *o_s, *gu_s, *down_s;
 };
 }  // namespace sb
 
@@ -56,6 +63,15 @@ struct seedb200_llama {
   int gunit_launches[5];          // kernels inside one captured unit (launch accounting of graph replays)
   int used_graph;
   int gen_cache_len;
+  // ---- int8 mode ----
+  int int8;
+  float threshold;
+  std::vector<uint8_t> i8_loaded; // [layers][7]: the int8 linear holds its weights
+  __half* corr;                   // [max_batch * max_seq, 2 * ffn] outlier correction of the GEMM path
+  int8_t* ca;                     // [max_batch * max_seq, max(hidden, ffn)] quantised activations (GEMM path)
+  float* sca;                     // [max_batch * max_seq]
+  int* olist;                     // [max(hidden, ffn)] outlier columns
+  int* ocount;
 };
 
 namespace sb {
@@ -78,6 +94,59 @@ static int llama_find(const seedb200_llama* m, const std::string& name, const __
   return 0;
 }
 
+// an int8 linear: "<base>.weight" int8 [N,K] and "<base>.SCB" fp32 [N].  Both absent: *cb = *scb = NULL (the slot is
+// filled later by seedb200_llama_int8_load_weight).
+static int llama_find_i8(const seedb200_llama* m, const std::string& base, int64_t N, int64_t K, const int8_t** cb,
+                         const float** scb) {
+  const std::string wn = base + ".weight", sn = base + ".SCB";
+  auto wi = m->w.find(wn), si = m->w.find(sn);
+  *cb = nullptr;
+  *scb = nullptr;
+  if (wi == m->w.end() && si == m->w.end()) return 0;
+  if (wi == m->w.end() || si == m->w.end()) {
+    set_error("llama_create_int8: missing weight '%s'", (wi == m->w.end() ? wn : sn).c_str());
+    return SEEDB200_ERR_INVALID;
+  }
+  const seedb200_tensor &w = wi->second, &s = si->second;
+  int64_t nw = 1, ns = 1;
+  for (int i = 0; i < w.ndim; ++i) nw *= w.shape[i];
+  for (int i = 0; i < s.ndim; ++i) ns *= s.shape[i];
+  if (w.dtype != SEEDB200_I8 || w.ndim != 2 || w.shape[0] != N || w.shape[1] != K || w.data == nullptr) {
+    set_error("llama_create_int8: '%s' must be int8 [%lld, %lld] (dtype %d, %lld elements)", wn.c_str(),
+              (long long)N, (long long)K, w.dtype, (long long)nw);
+    return SEEDB200_ERR_INVALID;
+  }
+  if (s.dtype != SEEDB200_F32 || ns != N || s.data == nullptr) {
+    set_error("llama_create_int8: '%s' must be fp32 [%lld] (dtype %d, %lld elements)", sn.c_str(), (long long)N,
+              s.dtype, (long long)ns);
+    return SEEDB200_ERR_INVALID;
+  }
+  *cb = static_cast<const int8_t*>(w.data);
+  *scb = static_cast<const float*>(s.data);
+  return 0;
+}
+
+static const char* const kI8Lin[7] = {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj",
+                                     "mlp.gate_proj", "mlp.up_proj", "mlp.down_proj"};
+
+// Where int8 linear i of layer L lives in the handle's fused buffers: CB rows r of [N,K] go to row
+// (r / grp) * gstride + r % grp + off of the fused weight, SCB entries likewise (gate|up: blocks of 128 rows).
+struct I8Slot { int8_t* cb; float* scb; int64_t N, K, grp, gstride, off; };
+static I8Slot i8_slot(const seedb200_llama* m, int layer, int i) {
+  const int64_t h = m->cfg.hidden, ffn = m->cfg.ffn;
+  const sb::LlamaLayerW& L = m->layers[layer];
+  I8Slot t;
+  t.K = i == 6 ? ffn : h;
+  t.N = i == 6 ? h : (i >= 4 ? ffn : h);
+  t.grp = t.N; t.gstride = 0; t.off = 0;
+  if (i < 3) { t.cb = const_cast<int8_t*>(L.qkv8); t.scb = const_cast<float*>(L.qkv_s); t.off = i * h; }
+  else if (i == 3) { t.cb = const_cast<int8_t*>(L.o8); t.scb = const_cast<float*>(L.o_s); }
+  else if (i < 6) { t.cb = const_cast<int8_t*>(L.gu8); t.scb = const_cast<float*>(L.gu_s); t.grp = 128; t.gstride = 256;
+                    t.off = i == 5 ? 128 : 0; }
+  else { t.cb = const_cast<int8_t*>(L.down8); t.scb = const_cast<float*>(L.down_s); }
+  return t;
+}
+
 template <typename T>
 static int llama_alloc(seedb200_llama* m, T** p, size_t elems) {
   void* q = nullptr;
@@ -96,6 +165,17 @@ static int llama_build(seedb200_llama* m) {
   SB_PROPAGATE(llama_find(m, "model.embed_tokens.weight", &m->embed, V * h));
   SB_PROPAGATE(llama_find(m, "model.norm.weight", &m->norm_w, h));
   SB_PROPAGATE(llama_find(m, "lm_head.weight", &m->lm_head, V * h));
+  if (m->int8) {    // every int8 tensor is checked before anything is allocated
+    for (int l = 0; l < c.layers; ++l)
+      for (int i = 0; i < 7; ++i) {
+        const int64_t N = i == 6 ? h : (i >= 4 ? ffn : h), K = i == 6 ? ffn : h;
+        const int8_t* cb;
+        const float* scb;
+        snprintf(nm, sizeof(nm), "model.layers.%d.%s", l, kI8Lin[i]);
+        SB_PROPAGATE(llama_find_i8(m, nm, N, K, &cb, &scb));
+      }
+    m->i8_loaded.assign((size_t)c.layers * 7, 0);
+  }
   m->layers.resize(c.layers);
   const size_t cache_elems = (size_t)c.max_batch * c.heads * c.max_seq * c.head_dim;
   for (int l = 0; l < c.layers; ++l) {
@@ -104,6 +184,40 @@ static int llama_build(seedb200_llama* m) {
     const __half *wq, *wk, *wv, *wg, *wu;
     SB_PROPAGATE(llama_find(m, key("input_layernorm.weight"), &L.in_ln, h));
     SB_PROPAGATE(llama_find(m, key("post_attention_layernorm.weight"), &L.post_ln, h));
+    SB_PROPAGATE(llama_alloc(m, &L.k_cache, cache_elems));
+    SB_PROPAGATE(llama_alloc(m, &L.v_cache, cache_elems));
+    L.qkv_w = L.o_w = L.gu_w = L.down_w = nullptr;
+    L.qkv8 = L.o8 = L.gu8 = L.down8 = nullptr;
+    L.qkv_s = L.o_s = L.gu_s = L.down_s = nullptr;
+    if (m->int8) {
+      // handle-owned fused buffers: q|k|v, o, [ffn/128] blocks of [128 gate | 128 up], down; scales alike
+      int8_t *q8, *o8, *g8, *d8;
+      float *qs, *os, *gs, *ds;
+      SB_PROPAGATE(llama_alloc(m, &q8, (size_t)3 * h * h));
+      SB_PROPAGATE(llama_alloc(m, &qs, (size_t)3 * h));
+      SB_PROPAGATE(llama_alloc(m, &o8, (size_t)h * h));
+      SB_PROPAGATE(llama_alloc(m, &os, (size_t)h));
+      SB_PROPAGATE(llama_alloc(m, &g8, (size_t)2 * ffn * h));
+      SB_PROPAGATE(llama_alloc(m, &gs, (size_t)2 * ffn));
+      SB_PROPAGATE(llama_alloc(m, &d8, (size_t)h * ffn));
+      SB_PROPAGATE(llama_alloc(m, &ds, (size_t)h));
+      L.qkv8 = q8; L.o8 = o8; L.gu8 = g8; L.down8 = d8;
+      L.qkv_s = qs; L.o_s = os; L.gu_s = gs; L.down_s = ds;
+      for (int i = 0; i < 7; ++i) {
+        const I8Slot t = i8_slot(m, l, i);
+        const int8_t* cb;
+        const float* scb;
+        SB_PROPAGATE(llama_find_i8(m, key(kI8Lin[i]), t.N, t.K, &cb, &scb));
+        if (cb == nullptr) continue;     // quantised into its slot later
+        const int64_t blocks = t.N / t.grp, dst_rows = t.grp == t.N ? t.N : t.gstride;
+        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.cb + t.off * t.K, (size_t)(dst_rows * t.K), cb, (size_t)(t.grp * t.K),
+                                        (size_t)(t.grp * t.K), (size_t)blocks, cudaMemcpyDeviceToDevice, st));
+        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.scb + t.off, (size_t)(dst_rows * 4), scb, (size_t)(t.grp * 4),
+                                        (size_t)(t.grp * 4), (size_t)blocks, cudaMemcpyDeviceToDevice, st));
+        m->i8_loaded[(size_t)l * 7 + i] = 1;
+      }
+      continue;
+    }
     SB_PROPAGATE(llama_find(m, key("self_attn.q_proj.weight"), &wq, h * h));
     SB_PROPAGATE(llama_find(m, key("self_attn.k_proj.weight"), &wk, h * h));
     SB_PROPAGATE(llama_find(m, key("self_attn.v_proj.weight"), &wv, h * h));
@@ -124,8 +238,6 @@ static int llama_build(seedb200_llama* m) {
     SB_CHECK_CUDA(cudaMemcpy2DAsync(reinterpret_cast<uint8_t*>(fg) + blk, 2 * blk, wu, blk, blk, ffn / 128,
                                     cudaMemcpyDeviceToDevice, st));
     L.gu_w = fg;
-    SB_PROPAGATE(llama_alloc(m, &L.k_cache, cache_elems));
-    SB_PROPAGATE(llama_alloc(m, &L.v_cache, cache_elems));
   }
   SB_PROPAGATE(get_rope_tables(c.head_dim, c.rope_base, c.max_seq, &m->cos_t, &m->sin_t, &m->max_pos, st));
   const size_t T = (size_t)c.max_batch * c.max_seq;
@@ -137,6 +249,15 @@ static int llama_build(seedb200_llama* m) {
   SB_PROPAGATE(llama_alloc(m, &m->gu, T * ffn));
   SB_PROPAGATE(llama_alloc(m, &m->hn, T * h));
   SB_PROPAGATE(llama_alloc(m, &m->last, (size_t)c.max_batch * h));
+  m->ca = nullptr; m->sca = nullptr; m->olist = nullptr; m->ocount = nullptr; m->corr = nullptr;
+  if (m->int8) {
+    SB_PROPAGATE(llama_alloc(m, &m->corr, T * (size_t)(2 * ffn > 3 * h ? 2 * ffn : 3 * h)));
+    const size_t kmax = (size_t)(ffn > h ? ffn : h);
+    SB_PROPAGATE(llama_alloc(m, &m->ca, T * kmax));
+    SB_PROPAGATE(llama_alloc(m, &m->sca, T));
+    SB_PROPAGATE(llama_alloc(m, &m->olist, kmax));
+    SB_PROPAGATE(llama_alloc(m, &m->ocount, 1));
+  }
   SB_PROPAGATE(llama_alloc(m, &m->da_ws, (size_t)c.max_batch * c.heads * decode_attention_max_splits(c.max_seq) * (128 + 2)));
   SB_PROPAGATE(llama_alloc(m, &m->da_tickets, (size_t)c.max_batch * c.heads));   // zero now, left zero by every launch
   SB_CHECK_CUDA(cudaMemsetAsync(m->da_tickets, 0, (size_t)c.max_batch * c.heads * sizeof(int), st));
@@ -166,6 +287,21 @@ static int lin(cudaStream_t st, int ctas, int M, int N, int K, const void* A, co
   return gemm(d, st);
 }
 
+// int8 decoder linear: GEMV for M <= 4 (with the RMSNorm folded in when norm_w is given), otherwise activation
+// quantisation + int8 wgmma GEMM.  Outputs are dense rows of N (N/2 in mode 1) columns.
+static int lin8(seedb200_llama* m, cudaStream_t st, int M, int N, int K, const void* A, const int8_t* W,
+                const float* scb, void* out, const void* residual, int mode, const void* norm_w = nullptr,
+                float eps = 0.0f) {
+  if (M <= 4) return gemv_int8(A, norm_w, eps, m->threshold, W, scb, out, residual, M, N, K, mode, st);
+  SB_PROPAGATE(int8_quantize_act(A, K, M, K, m->threshold, m->ca, m->sca, m->olist, m->ocount, st));
+  seedb200_gemm_int8_desc d;
+  memset(&d, 0, sizeof(d));
+  d.M = M; d.N = N; d.K = K;
+  d.A = m->ca; d.SCA = m->sca; d.A16 = A; d.outliers = m->olist; d.n_outliers = m->ocount;
+  d.W = W; d.SCB = scb; d.out = out; d.residual = residual; d.mode = mode; d.workspace = m->corr;
+  return gemm_int8(d, st);
+}
+
 // dyn (device, optional): {cache length, ...} read by the RoPE/append and decode-attention kernels instead of the
 // host value `past_len` -- what makes a captured decode step position independent (S must be 1).
 static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void* inputs_embeds,
@@ -185,7 +321,14 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
   const bool fused_attn = S == 1 && get_option("decode_fused_attention") != 0 && decode_attention_rope_supported(D, c.max_seq);
   for (int l = 0; l < c.layers; ++l) {
     const LlamaLayerW& L = m->layers[l];
-    if (fuse_norm) {
+    if (m->int8) {
+      if (fuse_norm) {
+        SB_PROPAGATE(lin8(m, st, T, 3 * h, h, m->x, L.qkv8, L.qkv_s, m->qkv, nullptr, 0, L.in_ln, c.rms_eps));
+      } else {
+        SB_PROPAGATE(rmsnorm(m->x, h, L.in_ln, m->nb, h, T, h, c.rms_eps, st));
+        SB_PROPAGATE(lin8(m, st, T, 3 * h, h, m->nb, L.qkv8, L.qkv_s, m->qkv, nullptr, 0));
+      }
+    } else if (fuse_norm) {
       SB_PROPAGATE(lin(st, ct, T, 3 * h, h, m->x, L.qkv_w, m->qkv, 3 * h, nullptr, 0, L.in_ln, c.rms_eps));
     } else {
       SB_PROPAGATE(rmsnorm(m->x, h, L.in_ln, m->nb, h, T, h, c.rms_eps, st));
@@ -213,6 +356,17 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
       a.batch = B; a.heads = H; a.nq = S; a.nk = kv_len; a.head_dim = D; a.causal = 1; a.scale = scale;
       SB_PROPAGATE(attention(a, st));
     }
+    }
+    if (m->int8) {
+      SB_PROPAGATE(lin8(m, st, T, h, h, m->att, L.o8, L.o_s, m->x, m->x, 0));
+      if (fuse_norm) {
+        SB_PROPAGATE(lin8(m, st, T, 2 * ffn, h, m->x, L.gu8, L.gu_s, m->gu, nullptr, 1, L.post_ln, c.rms_eps));
+      } else {
+        SB_PROPAGATE(rmsnorm(m->x, h, L.post_ln, m->nb, h, T, h, c.rms_eps, st));
+        SB_PROPAGATE(lin8(m, st, T, 2 * ffn, h, m->nb, L.gu8, L.gu_s, m->gu, nullptr, 1));
+      }
+      SB_PROPAGATE(lin8(m, st, T, h, ffn, m->gu, L.down8, L.down_s, m->x, m->x, 0));
+      continue;
     }
     SB_PROPAGATE(lin(st, ct, T, h, h, m->att, L.o_w, m->x, h, m->x, 0));
     if (fuse_norm) {
@@ -359,12 +513,23 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
   return 0;
 }
 
+// every int8 linear must hold its weights before the model runs
+static int llama_int8_ready(const seedb200_llama* m) {
+  for (size_t i = 0; i < m->i8_loaded.size(); ++i)
+    if (!m->i8_loaded[i]) {
+      set_error("llama: int8 weight 'model.layers.%d.%s.weight' was neither given to create_int8 nor loaded",
+                (int)(i / 7), kI8Lin[i % 7]);
+      return SEEDB200_ERR_INVALID;
+    }
+  return 0;
+}
+
 }  // namespace sb
 
 extern "C" {
 
-int seedb200_llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
-                          seedb200_llama** out) {
+static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights, int int8,
+                        float threshold, seedb200_llama** out) {
   if (!cfg || !weights || !out) {
     sb::set_error("llama_create: null argument");
     return SEEDB200_ERR_INVALID;
@@ -385,6 +550,8 @@ int seedb200_llama_create(const seedb200_llama_config* cfg, const seedb200_tenso
   m->used_graph = -1;
   m->gen_cache_len = 0;
   for (int i = 0; i < 5; ++i) { m->gexec[i] = nullptr; m->gunit_launches[i] = 0; }
+  m->int8 = int8;
+  m->threshold = threshold;
   for (int i = 0; i < n_weights; ++i) m->w[std::string(weights[i].name)] = weights[i];
   int s = sb::llama_build(m);
   if (s != 0) {
@@ -393,6 +560,40 @@ int seedb200_llama_create(const seedb200_llama_config* cfg, const seedb200_tenso
   }
   m->w.clear();
   *out = m;
+  return 0;
+}
+
+int seedb200_llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
+                          seedb200_llama** out) {
+  return llama_create(cfg, weights, n_weights, 0, 0.0f, out);
+}
+
+int seedb200_llama_create_int8(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
+                               float threshold, seedb200_llama** out) {
+  SB_REQUIRE(threshold > 0.0f, "llama_create_int8: threshold must be > 0 (got %g)", (double)threshold);
+  SB_REQUIRE(cfg == nullptr || cfg->hidden % 16 == 0, "llama_create_int8: hidden must be a multiple of 16");
+  return llama_create(cfg, weights, n_weights, 1, threshold, out);
+}
+
+int seedb200_llama_int8_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream) {
+  SB_REQUIRE(llm && name && W, "llama_int8_load_weight: null argument");
+  SB_REQUIRE(llm->int8, "llama_int8_load_weight: the handle was not made by seedb200_llama_create_int8");
+  int layer = -1, i = -1;
+  for (int k = 0; k < 7 && i < 0; ++k) {
+    char tail[64];
+    snprintf(tail, sizeof(tail), ".%s.weight", sb::kI8Lin[k]);
+    int l = -1, n = 0;
+    if (sscanf(name, "model.layers.%d%n", &l, &n) == 1 && strcmp(name + n, tail) == 0) { layer = l; i = k; }
+  }
+  SB_REQUIRE(i >= 0 && layer >= 0 && layer < (int)llm->layers.size(),
+             "llama_int8_load_weight: '%s' is not a decoder linear of this model", name);
+  const sb::I8Slot t = sb::i8_slot(llm, layer, i);
+  if (ldw == 0) ldw = t.K;
+  SB_REQUIRE(ldw >= t.K, "llama_int8_load_weight: ldw %lld below K %lld", (long long)ldw, (long long)t.K);
+  sb::DeviceGuard guard(llm->device);
+  SB_PROPAGATE(sb::int8_quantize_weight_rows(W, ldw, (int)t.N, (int)t.K, t.cb, t.scb, (int)t.grp, (int)t.gstride,
+                                             (int)t.off, static_cast<cudaStream_t>(stream)));
+  llm->i8_loaded[(size_t)layer * 7 + i] = 1;
   return 0;
 }
 
@@ -418,6 +619,7 @@ int seedb200_llama_forward_ld(seedb200_llama* llm, const int64_t* input_ids, con
   SB_REQUIRE(logits_mode == 0 || logits_mode == 1, "llama_forward: logits_mode must be 0 or 1");
   SB_REQUIRE(logits_out == nullptr || logits_ld >= llm->cfg.vocab, "llama_forward: logits_ld %lld < vocab %d",
              (long long)logits_ld, llm->cfg.vocab);
+  SB_PROPAGATE(sb::llama_int8_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_forward(llm, input_ids, inputs_embeds, position_ids, B, S, past_len, logits_mode, logits_out,
                            logits_ld, static_cast<cudaStream_t>(stream));
@@ -439,6 +641,7 @@ int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int 
   SB_REQUIRE(S >= 1 && max_new_tokens >= 1 && S + max_new_tokens <= llm->cfg.max_seq,
              "llama_generate: prompt %d + %d new tokens exceeds max_seq %d", S, max_new_tokens, llm->cfg.max_seq);
   SB_REQUIRE(!sp->do_sample || (sp->temperature > 0.0f && sp->top_p > 0.0f), "llama_generate: temperature and top_p must be > 0");
+  SB_PROPAGATE(sb::llama_int8_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_generate(llm, prompt_ids, B, S, max_new_tokens, sp, eos_id, pad_id, use_graph, tokens_out,
                             n_generated_host, static_cast<cudaStream_t>(stream));

@@ -57,5 +57,18 @@ int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, co
 int image_ids_to_tokens(const int64_t* ids, int n, int64_t shift, int64_t boi, int64_t eoi, int64_t* out,
                         int64_t out_stride, cudaStream_t stream);
 int cur_device();
+// LLM.int8() (int8.cu, gemm_wgmma.cu)
+int int8_quantize_weight(const void* W, int64_t ldw, int N, int K, void* CB, void* SCB, cudaStream_t stream);
+// the same into a fused layout: row n -> (n / grp) * gstride + n % grp + off
+int int8_quantize_weight_rows(const void* W, int64_t ldw, int N, int K, void* CB, void* SCB, int grp, int gstride,
+                              int off, cudaStream_t stream);
+int int8_quantize_act(const void* A, int64_t lda, int M, int K, float threshold, void* CA, void* SCA, int* outliers,
+                      int* n_outliers, cudaStream_t stream);
+int gemm_int8(const seedb200_gemm_int8_desc& d, cudaStream_t stream);
+// corr [M,N] fp16 = the outlier correction of every output (written only when *n_outliers > 0)
+int int8_correction(const void* A16, int64_t lda, const void* W, int64_t ldw, const void* SCB, const int* outliers,
+                    const int* n_outliers, int M, int N, void* corr, cudaStream_t stream);
+int gemv_int8(const void* x, const void* norm_w, float eps, float threshold, const void* W, const void* SCB, void* out,
+              const void* residual, int M, int N, int K, int mode, cudaStream_t stream);
 
 }  // namespace sb

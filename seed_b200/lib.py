@@ -35,7 +35,12 @@ EXPORTS = [
     "seedb200_llama_forward_ld", "seedb200_llama_generate", "seedb200_llama_generate_used_graph",
     "seedb200_row_stats", "seedb200_row_stats_from_moments", "seedb200_ln_fold_weights",
     "seedb200_gemm_plan", "seedb200_gemm_schedule_tile", "seedb200_decode_attention_rope",
+    "seedb200_int8_quantize_weight", "seedb200_int8_quantize_act", "seedb200_gemm_int8", "seedb200_gemv_int8",
+    "seedb200_llama_create_int8", "seedb200_llama_int8_load_weight",
 ]
+
+DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
+_DTYPE_CODE = {torch.float16: DTYPE_F16, torch.float32: DTYPE_F32, torch.int8: DTYPE_I8}
 
 
 class Tensor(C.Structure):
@@ -56,6 +61,17 @@ class GemmDesc(C.Structure):
                 ("bn", C.c_int32), ("ctas", C.c_int32),
                 ("ln_stats", C.c_void_p), ("ln_c", C.c_void_p), ("ln_b", C.c_void_p),
                 ("row_moments", C.c_void_p)]
+
+
+class GemmInt8Desc(C.Structure):
+    _fields_ = [("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32),
+                ("A", C.c_void_p), ("lda", C.c_int64), ("SCA", C.c_void_p),
+                ("A16", C.c_void_p), ("lda16", C.c_int64),
+                ("outliers", C.c_void_p), ("n_outliers", C.c_void_p),
+                ("W", C.c_void_p), ("ldw", C.c_int64), ("SCB", C.c_void_p),
+                ("out", C.c_void_p), ("ldo", C.c_int64),
+                ("residual", C.c_void_p), ("ldr", C.c_int64),
+                ("mode", C.c_int32), ("bn", C.c_int32), ("workspace", C.c_void_p)]
 
 
 class AttnDesc(C.Structure):
@@ -165,6 +181,16 @@ def load() -> C.CDLL:
     lib.seedb200_llama_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(SampleParams),
                                             C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
     lib.seedb200_llama_generate_used_graph.argtypes = [C.c_void_p]
+    lib.seedb200_int8_quantize_weight.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p]
+    lib.seedb200_int8_quantize_act.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_float, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.seedb200_gemm_int8.argtypes = [C.POINTER(GemmInt8Desc), C.c_void_p]
+    lib.seedb200_gemv_int8.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    lib.seedb200_llama_create_int8.argtypes = [C.POINTER(LlamaConfig), C.POINTER(Tensor), C.c_int, C.c_float,
+                                               C.POINTER(C.c_void_p)]
+    lib.seedb200_llama_int8_load_weight.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p]
     _lib = lib
     return lib
 
@@ -454,6 +480,82 @@ def gemv(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = No
     return out
 
 
+def int8_quantize_weight(w: torch.Tensor):
+    """LLM.int8() weight quantisation: fp16 [N,K] -> (CB int8 [N,K], SCB fp32 [N])."""
+    _need_cuda_f16(w, "int8_quantize_weight.w")
+    N, K = w.shape
+    if w.stride(1) != 1:
+        w = w.contiguous()
+    cb = torch.empty((N, K), dtype=torch.int8, device=w.device)
+    scb = torch.empty((N,), dtype=torch.float32, device=w.device)
+    with on(w.device):
+        check(load().seedb200_int8_quantize_weight(w.data_ptr(), w.stride(0), N, K, cb.data_ptr(), scb.data_ptr(),
+                                                   stream_ptr(w.device)), "seedb200_int8_quantize_weight")
+    return cb, scb
+
+
+def int8_quantize_act(a: torch.Tensor, threshold: float = 6.0):
+    """LLM.int8() activation quantisation: fp16 [M,K] -> (CA int8 [M,K], SCA fp32 [M], outliers int32 [K] (the
+    first n entries are the outlier columns in ascending order), n int32 [1]) -- all on the device."""
+    _need_cuda_f16(a, "int8_quantize_act.a")
+    M, K = a.shape
+    if a.stride(1) != 1:
+        a = a.contiguous()
+    ca = torch.empty((M, K), dtype=torch.int8, device=a.device)
+    sca = torch.empty((M,), dtype=torch.float32, device=a.device)
+    ol = torch.empty((K,), dtype=torch.int32, device=a.device)
+    n = torch.empty((1,), dtype=torch.int32, device=a.device)
+    with on(a.device):
+        check(load().seedb200_int8_quantize_act(a.data_ptr(), a.stride(0), M, K, float(threshold), ca.data_ptr(),
+                                                sca.data_ptr(), ol.data_ptr(), n.data_ptr(), stream_ptr(a.device)),
+              "seedb200_int8_quantize_act")
+    return ca, sca, ol, n
+
+
+def gemm_int8(a: torch.Tensor, cb: torch.Tensor, scb: torch.Tensor, threshold: float = 6.0,
+              residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, mode: int = 0,
+              bn: int = 0) -> torch.Tensor:
+    """linear8(a, (cb, scb)) by activation quantisation + the int8 wgmma GEMM; a fp16 [M,K], cb int8 [N,K]."""
+    _need_cuda_f16(a, "gemm_int8.a")
+    a = a.contiguous()
+    M, K = a.shape
+    N = cb.shape[0]
+    ca, sca, ol, n = int8_quantize_act(a, threshold)
+    if out is None:
+        out = torch.empty((M, N // 2 if mode == 1 else N), dtype=torch.float16, device=a.device)
+    d = GemmInt8Desc()
+    d.M, d.N, d.K = M, N, K
+    d.A, d.lda, d.SCA = ca.data_ptr(), K, sca.data_ptr()
+    d.A16, d.lda16 = a.data_ptr(), K
+    d.outliers, d.n_outliers = ol.data_ptr(), n.data_ptr()
+    d.W, d.ldw, d.SCB = cb.data_ptr(), cb.stride(0), scb.data_ptr()
+    d.out, d.ldo = out.data_ptr(), out.stride(0)
+    d.residual, d.ldr = _p(residual), (residual.stride(0) if residual is not None else 0)
+    d.mode, d.bn = mode, bn
+    ws = torch.empty((M, N), dtype=torch.float16, device=a.device)
+    d.workspace = ws.data_ptr()
+    with on(a.device):
+        check(load().seedb200_gemm_int8(C.byref(d), stream_ptr(a.device)), "seedb200_gemm_int8")
+    return out
+
+
+def gemv_int8(x: torch.Tensor, cb: torch.Tensor, scb: torch.Tensor, threshold: float = 6.0,
+              residual: Optional[torch.Tensor] = None, norm_w: Optional[torch.Tensor] = None, eps: float = 1e-6,
+              mode: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """linear8 for M <= 4 rows by the int8 GEMV (quantisation, and RMSNorm with norm_w, inside the kernel)."""
+    _need_cuda_f16(x, "gemv_int8.x")
+    x = x.contiguous()
+    M, K = x.shape
+    N = cb.shape[0]
+    if out is None:
+        out = torch.empty((M, N // 2 if mode == 1 else N), dtype=torch.float16, device=x.device)
+    with on(x.device):
+        check(load().seedb200_gemv_int8(x.data_ptr(), _p(norm_w), eps, float(threshold), cb.data_ptr(), scb.data_ptr(),
+                                        out.data_ptr(), _p(residual), M, N, K, mode, stream_ptr(x.device)),
+              "seedb200_gemv_int8")
+    return out
+
+
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, kv_len: int,
                      scale: float) -> torch.Tensor:
     """q [B,H,D] against the first kv_len rows of caches [B,H,max_seq,D] -> [B, H*D]."""
@@ -536,8 +638,9 @@ def _tensor_array(weights: Dict[str, torch.Tensor]):
     keep = []
     dev = None
     for i, (name, t) in enumerate(weights.items()):
-        if not t.is_cuda or t.dtype != torch.float16 or not t.is_contiguous():
-            raise RuntimeError(f"weight {name}: expected contiguous CUDA float16, got {t.dtype} on {t.device}")
+        if not t.is_cuda or t.dtype not in _DTYPE_CODE or not t.is_contiguous():
+            raise RuntimeError(f"weight {name}: expected a contiguous CUDA float16, float32 or int8 tensor, got {t.dtype} "
+                               f"on {t.device}")
         if dev is None:
             dev = t.device
         elif t.device != dev:
@@ -546,7 +649,7 @@ def _tensor_array(weights: Dict[str, torch.Tensor]):
         keep.append(b)
         arr[i].name = b
         arr[i].data = t.data_ptr()
-        arr[i].dtype = 0
+        arr[i].dtype = _DTYPE_CODE[t.dtype]
         arr[i].ndim = min(t.dim(), 4)
         shp = list(t.shape)
         if len(shp) > 4:   # fold leading dims (conv weight [1408,3,14,14] has exactly 4)
@@ -659,7 +762,10 @@ class Llama:
 
     def __init__(self, weights: Dict[str, torch.Tensor], hidden: int, layers: int, heads: int, ffn: int, vocab: int,
                  max_batch: int = 1, max_seq: int = 4096, rms_eps: float = 1e-6, rope_base: float = 10000.0,
-                 gemm_ctas: int = 0):
+                 gemm_ctas: int = 0, int8_threshold: Optional[float] = None):
+        """int8_threshold: None = fp16 weights (seedb200_llama_create); a float = LLM.int8() decoder linears given as
+        int8 "<name>.weight" + fp32 "<name>.SCB" (seedb200_llama_create_int8), which the handle copies: only the
+        fp16 tensors stay referenced after construction."""
         lib = load()
         self._weights = dict(weights)
         arr, keep = _tensor_array(self._weights)
@@ -668,7 +774,14 @@ class Llama:
                           rope_base, gemm_ctas)
         h = C.c_void_p()
         with on(self.device):
-            check(lib.seedb200_llama_create(C.byref(cfg), arr, len(self._weights), C.byref(h)), "seedb200_llama_create")
+            if int8_threshold is None:
+                check(lib.seedb200_llama_create(C.byref(cfg), arr, len(self._weights), C.byref(h)),
+                      "seedb200_llama_create")
+            else:
+                check(lib.seedb200_llama_create_int8(C.byref(cfg), arr, len(self._weights), float(int8_threshold),
+                                                     C.byref(h)), "seedb200_llama_create_int8")
+        if int8_threshold is not None:
+            self._weights = {k: v for k, v in self._weights.items() if v.dtype == torch.float16}
         self._h = h
         self.hidden, self.layers, self.heads, self.head_dim = hidden, layers, heads, hidden // heads
         self.ffn, self.vocab, self.max_batch, self.max_seq = ffn, vocab, max_batch, max_seq
@@ -730,6 +843,15 @@ class Llama:
                                                  out.data_ptr(), C.byref(n), stream_ptr(self.device)),
                   "seedb200_llama_generate")
         return out[:, :n.value]
+
+    def int8_load_weight(self, name: str, w: torch.Tensor) -> None:
+        """quantise the fp16 decoder linear `name` straight into the int8 handle's fused layout"""
+        _need_cuda_f16(w, name)
+        if w.stride(1) != 1 or w.device != self.device:
+            raise RuntimeError(f"{name}: expected rows with contiguous columns on {self.device}")
+        with on(self.device):
+            check(load().seedb200_llama_int8_load_weight(self._h, name.encode(), w.data_ptr(), w.stride(0),
+                                                         stream_ptr(self.device)), "seedb200_llama_int8_load_weight")
 
     @property
     def used_graph(self) -> int:

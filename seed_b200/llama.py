@@ -9,6 +9,9 @@ Reference behaviours kept on purpose (SURVEY.md section 7 "quirks"):
     to choose between a causal and an unmasked xformers call (llama_xformer.py:240-256);
   * q_len == 1 attends to the whole cache without a mask; q_len > 1 is causal;
   * logits are returned for every position in fp16.
+`load_in_8bit=True` runs the seven linear layers of every decoder layer as LLM.int8() (transformers' bitsandbytes
+path, threshold `llm_int8_threshold`): int8 weights with per-row scales, per-call activation quantisation with fp16
+outlier columns; embed_tokens, lm_head and the norms stay fp16 (include/seedb200.h states the arithmetic).
 Differences: `past_key_values` are views of the handle's preallocated cache (no torch.cat per step);
 `output_attentions` / `output_hidden_states` are not available (the reference's xformers path never computed
 attention weights either).
@@ -34,9 +37,49 @@ class _CudaView:
                                          "strides": tuple(s * 2 for s in strides_elems)}
 
 
+_INT8_LINEARS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
+
+
+def _is_int8_linear(name: str) -> bool:
+    """the decoder-layer nn.Linear weights transformers' load_in_8bit replaces (lm_head is kept in fp16)"""
+    parts = name.split(".")
+    return ".layers." in name and len(parts) >= 2 and parts[-1] == "weight" and parts[-2] in _INT8_LINEARS
+
+
+def _one_device(device_map) -> torch.device:
+    """device_map of HF from_pretrained -> the single device it names; no model parallelism here."""
+    def dev(v):
+        return torch.device(f"cuda:{v}") if isinstance(v, int) else torch.device(v)
+
+    if isinstance(device_map, dict):
+        devs = {dev(v) for v in device_map.values()}
+        if len(devs) != 1:
+            raise ValueError(f"device_map spans {len(devs)} devices; seed_b200 runs the model on one device")
+        return devs.pop()
+    if device_map == "auto":
+        if torch.cuda.device_count() > 1:
+            raise ValueError("device_map='auto' would span several GPUs; pass one device (e.g. 'cuda:0')")
+        return torch.device("cuda:0")
+    return dev(device_map)
+
+
+def _linear_items(state_dict, names):
+    """(name, tensor) of the int8 linears; a state dict that makes its tensors on demand (its items() is a generator)
+    is walked again rather than indexed, so nothing is made twice at once"""
+    wanted = set(names)
+    if isinstance(state_dict, dict) and type(state_dict).items is dict.items:
+        for k in names:
+            yield k, state_dict[k]
+        return
+    for k, v in state_dict.items():
+        if k in wanted:
+            yield k, v
+
+
 class LlamaForCausalLM(nn.Module):
     def __init__(self, config: LlamaConfig, state_dict, device="cuda", max_batch: int = 1,
-                 max_seq: Optional[int] = None, gemm_ctas: int = 0):
+                 max_seq: Optional[int] = None, gemm_ctas: int = 0, load_in_8bit: bool = False,
+                 llm_int8_threshold: float = 6.0):
         super().__init__()
         dev = torch.device(device)
         if dev.type != "cuda" or not torch.cuda.is_available():
@@ -48,11 +91,41 @@ class LlamaForCausalLM(nn.Module):
             raise ValueError("grouped-query attention is not part of models/llama_xformer.py")
         self.max_batch = max_batch
         self.max_seq = max_seq or config.max_position_embeddings
-        weights = {k: v.detach().to(device=dev, dtype=torch.float16).contiguous() for k, v in state_dict.items()
-                   if "rotary_emb" not in k}
-        self._llm = L.Llama(weights, hidden=h, layers=nl, heads=nh, ffn=config.intermediate_size,
-                            vocab=config.vocab_size, max_batch=max_batch, max_seq=self.max_seq,
-                            rms_eps=config.rms_norm_eps, gemm_ctas=gemm_ctas)
+        self.is_loaded_in_8bit = bool(load_in_8bit)
+        if load_in_8bit:
+            # the handle is made with the fp16 tensors only; then each linear goes to the device in fp16, is quantised
+            # straight into the handle's int8 buffers, and is dropped before the next: device memory stays at the
+            # int8 model plus one fp16 tensor
+            weights, linears = {}, []
+            items = iter(state_dict.items())
+            for k, v in items:
+                if "rotary_emb" in k:
+                    continue
+                if _is_int8_linear(k):
+                    linears.append(k)
+                    continue
+                weights[k] = v.detach().to(device=dev, dtype=torch.float16).contiguous()
+            self._weight_bytes = sum(t.numel() * t.element_size() for t in weights.values())
+            self._llm = L.Llama(weights, hidden=h, layers=nl, heads=nh, ffn=config.intermediate_size,
+                                vocab=config.vocab_size, max_batch=max_batch, max_seq=self.max_seq,
+                                rms_eps=config.rms_norm_eps, gemm_ctas=gemm_ctas,
+                                int8_threshold=float(llm_int8_threshold))
+            for k, v in _linear_items(state_dict, linears):
+                w16 = v.detach().to(device=dev, dtype=torch.float16)
+                if w16.stride(-1) != 1:
+                    w16 = w16.contiguous()
+                self._llm.int8_load_weight(k, w16)
+                # int8 values plus one fp32 scale per row
+                self._weight_bytes += w16.shape[0] * w16.shape[1] + 4 * w16.shape[0]
+                del w16, v     # stream-ordered: the allocator reuses this block only after the kernel has read it
+        else:
+            weights = {k: v.detach().to(device=dev, dtype=torch.float16).contiguous() for k, v in state_dict.items()
+                       if "rotary_emb" not in k}
+            # device bytes of the weights the handle owns or borrows (HF get_memory_footprint: no KV cache / workspace)
+            self._weight_bytes = sum(t.numel() * t.element_size() for t in weights.values())
+            self._llm = L.Llama(weights, hidden=h, layers=nl, heads=nh, ffn=config.intermediate_size,
+                                vocab=config.vocab_size, max_batch=max_batch, max_seq=self.max_seq,
+                                rms_eps=config.rms_norm_eps, gemm_ctas=gemm_ctas)
         # q/k/v and gate/up were copied into fused layouts by the handle: drop our references to the originals
         for k in [k for k in self._llm._weights if any(s in k for s in ("q_proj", "k_proj", "v_proj", "gate_proj", "up_proj"))]:
             del self._llm._weights[k]
@@ -63,8 +136,12 @@ class LlamaForCausalLM(nn.Module):
 
     # ---- construction --------------------------------------------------------------------------
     @classmethod
-    def from_pretrained(cls, pretrained_model_name_or_path, torch_dtype=torch.float16, device="cuda", **kwargs):
-        """HF checkpoint directory (config.json + *.safetensors or pytorch_model*.bin)."""
+    def from_pretrained(cls, pretrained_model_name_or_path, torch_dtype=torch.float16, device="cuda", device_map=None,
+                        **kwargs):
+        """HF checkpoint directory (config.json + *.safetensors or pytorch_model*.bin).  `load_in_8bit`,
+        `llm_int8_threshold` and a single-device `device_map` are honoured as transformers does."""
+        if device_map is not None:
+            device = _one_device(device_map)
         path = str(pretrained_model_name_or_path)
         if not os.path.isdir(path):
             raise RuntimeError(f"{path} is not a local checkpoint directory (no network access)")
@@ -84,7 +161,8 @@ class LlamaForCausalLM(nn.Module):
                 sd.update(torch.load(fn, map_location="cpu"))
         if not sd:
             raise RuntimeError(f"no weight files found under {path}")
-        kwargs = {k: v for k, v in kwargs.items() if k in ("max_batch", "max_seq", "gemm_ctas")}
+        kwargs = {k: v for k, v in kwargs.items()
+                  if k in ("max_batch", "max_seq", "gemm_ctas", "load_in_8bit", "llm_int8_threshold")}
         return cls(config, sd, device=device, **kwargs)
 
     # ---- nn.Module conveniences ------------------------------------------------------------------
@@ -94,6 +172,11 @@ class LlamaForCausalLM(nn.Module):
 
     def eval(self):
         return self
+
+    def get_memory_footprint(self) -> int:
+        """device bytes of the model's weights (int8 linears count their int8 values and fp32 scales); the KV cache
+        and workspaces are excluded, as in transformers."""
+        return int(self._weight_bytes)
 
     def half(self):
         return self
