@@ -289,6 +289,46 @@ int seedb200_sample(const void* logits, int64_t ld, int B, int V, const seedb200
 /* the uniform in (0,1] the sampler draws for (seed, offset + step, row) -- host function, for tests */
 float seedb200_philox_uniform(uint64_t seed, uint64_t offset, uint32_t row);
 
+/* Beam search and beam sampling (num_beams > 1), transformers 4.30.2 GenerationMixin.beam_search / beam_sample with
+ * BeamSearchScorer(num_beam_hyps_to_keep = 1), the arithmetic the reference pins (requirements.txt:8):
+ *   init       beam_scores fp32 = 0 for beam 0 and -1e9 for beams 1..k-1 of every sequence (the prompt is expanded k
+ *              times, so all beams see the same first logits)
+ *   step       lp = log_softmax(logits) rounded to fp16 (the logits' dtype); s = float(lp) + beam_score in fp32
+ *   greedy     the top 2k of s over the sequence's [k * V] flat entries, descending, ties to the lowest flat index;
+ *              beam = j / V, token = j % V
+ *   sampling   w = s / temperature (fp32); TopP on each beam row of w with min_tokens_to_keep = 2 in threshold form
+ *              (every token tied with the least kept one stays, as seedb200_sample); 2k draws without replacement
+ *              from softmax(w) over [k * V] by Gumbel-top-k: key_j = w_j + (-log(-log u_j)) in fp32, filtered
+ *              entries -inf, the top 2k keys (ties to the lowest j; non-finite keys fill the last ranks by index).
+ *              u_j = ((x >> 9) + 0.5) * 2^-23 with x the first word of Philox4x32-10, key = seed, counter =
+ *              (offset + step lo, hi, sequence, 1 + j): strictly inside (0, 1), and word 3 != 0 keeps this stream
+ *              apart from seedb200_sample's.  The draws are sorted by w descending (ties to the lowest index) and
+ *              the scorer receives w, so running beam scores accumulate temperature-scaled sums (4.30.2's quirk).
+ *   scorer     candidates in rank order: an eos candidate at rank < k adds the hypothesis "parent's sequence" with
+ *              score = (double)s / len ** length_penalty, len = prompt + generated tokens before the append; at rank
+ *              >= k it is skipped; other candidates become the next beams until k are chosen.  At most k hypotheses
+ *              are kept: on overflow the lowest score goes (ties: the earliest added), worst_score as BeamHypotheses.
+ *              Done (early_stopping 0 = False: k hypotheses and worst >= best / cur_len ** lp; 1 = True: k
+ *              hypotheses; 2 = "never": worst >= best / max_length ** lp when lp > 0, else as False).  A finished
+ *              sequence emits pad.  The loop ends when every sequence is done or after max_new_tokens steps.
+ *   finalize   unfinished sequences add their k running beams; the best hypothesis is the last of a stable ascending
+ *              sort by score (ties to the latest added); output width = min(longest + 1, S + max_new_tokens),
+ *              eos_id right after every shorter hypothesis and pad after that.                                   */
+typedef struct seedb200_beam_params {
+  int32_t num_beams;          /* k, 1..8 */
+  int32_t do_sample;          /* 0 = beam_search, 1 = beam_sample */
+  float temperature, top_p;
+  double length_penalty;
+  int32_t early_stopping;     /* 0 = False, 1 = True, 2 = "never" */
+  uint64_t seed, offset;
+} seedb200_beam_params;
+/* logits row of (sequence i, beam j) = logits + i * seq_ld + j * beam_ld (fp16, V valid columns; beam_ld = 0 reads
+ * one row for every beam, as after the prefill); beam_scores [B * k] fp32 -> cand_score [B, 2k] fp32 (s or w) and
+ * cand_idx [B, 2k] int32 flat indices (beam * V + token), in the scorer's order.  step: the Philox step.          */
+int seedb200_beam_select(const void* logits, int64_t seq_ld, int64_t beam_ld, int B, int V, const float* beam_scores,
+                         const seedb200_beam_params* bp, uint64_t step, float* cand_score, int32_t* cand_idx,
+                         void* stream);
+
 /* Codebook ids -> LLaMA token ids without the '<img_%05d>' string round trip of
  * scripts/seed_llama_inference_8B.py:16-23,60,98-100 and gradio_demo/seed_llama_flask.py:144-150:
  * ids [n,32] int64 -> tokens_out[i*out_stride + 0..33] = boi, image_id_shift + id (x32), eoi.  out_stride >= 34
@@ -401,6 +441,31 @@ int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int 
                             int64_t* tokens_out, int* n_generated_host, void* stream);
 /* 1 when the last generate() replayed a captured graph, 0 when it ran eagerly, -1 before any call */
 int seedb200_llama_generate_used_graph(seedb200_llama* llm);
+/* Beam search / beam sampling (see seedb200_beam_params) of prompt_ids [B,S] (device int64): prefill at B cache rows,
+ * then per step candidates -> scorer -> one cached forward of B * k rows whose attention reads each beam's past
+ * through a lineage table (no cache copies).  The decode step is captured once per (B, k) into a CUDA graph when
+ * use_graph != 0.  eos_id < 0: no eos (fixed length).  B * k <= max_batch (see seedb200_llama_reserve_rows).
+ * tokens_out [B, max_new_tokens] int64 (device): the generated part of the output; *n_out_host receives its valid
+ * width (output width - S); best_scores_out [B] fp32 (device, may be NULL): the chosen hypotheses' scores.
+ * Synchronises the stream (every 32 steps with an eos id, and once at the end).                                  */
+int seedb200_llama_beam_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                                 const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id, int use_graph,
+                                 int64_t* tokens_out, int* n_out_host, float* best_scores_out, void* stream);
+/* Grows every buffer sized by max_batch (KV caches, activations, int8 workspaces, generation state) to `rows`
+ * rows; no-op when rows <= max_batch.  The cache contents and the captured graphs are dropped.  Synchronises the
+ * device.  Bytes added per row: see INTEGRATION.md "C4. Beam search".                                           */
+int seedb200_llama_reserve_rows(seedb200_llama* llm, int rows);
+/* Decode attention through a lineage table: cached key / value p of row b is read from cache row
+ * slot[b * max_seq + p] (slot [B, max_seq] int32, device); otherwise seedb200_decode_attention. */
+int seedb200_decode_attention_lineage(const void* q, const void* k_cache, const void* v_cache, const int32_t* slot,
+                                      void* out, int B, int H, int D, int kv_len, int max_seq, float scale,
+                                      void* workspace, void* stream);
+/* seedb200_decode_attention_rope through a lineage table (max_seq <= 2048): the new K/V are appended at row b,
+ * position past_len, which slot[b * max_seq + past_len] must name (= b); earlier positions are read from
+ * slot[b * max_seq + p].                                                                                         */
+int seedb200_decode_attention_rope_lineage(const void* qkv, const int64_t* positions, const int32_t* slot, int B, int H,
+                                           int D, int past_len, int max_seq, void* k_cache, void* v_cache, void* out,
+                                           float scale, void* stream);
 
 /* Views of the KV cache of one layer: [max_batch, heads, max_seq, head_dim]
  * fp16; the first past_len+S rows per (batch, head) are valid.  Used to build

@@ -17,7 +17,7 @@ LIB = os.path.join(ROOT, "libseedb200.so")
 ORACLE_DIR = os.path.join(REPO, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "libvq_oracle.so")
 
-SOURCES = ["capi.cu", "gemm_wgmma.cu", "attention.cu", "rowwise.cu", "vq.cu", "misc.cu", "sampler.cu", "encoder.cu", "llama.cu", "preprocess.cu", "int8.cu"]
+SOURCES = ["capi.cu", "gemm_wgmma.cu", "attention.cu", "rowwise.cu", "vq.cu", "misc.cu", "sampler.cu", "encoder.cu", "llama.cu", "preprocess.cu", "int8.cu", "beam.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "int8.cuh"), os.path.join(CSRC, "ops.h"), os.path.join(REPO, "include", "seedb200.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -199,4 +199,16 @@ int seedb200_decode_attention_rope(const void* qkv, const int64_t* positions, in
                                    out, scale, st);
 }
 
+int seedb200_decode_attention_rope_lineage(const void* qkv, const int64_t* positions, const int32_t* slot, int B, int H,
+                                           int D, int past_len, int max_seq, void* k_cache, void* v_cache, void* out,
+                                           float scale, void* stream) {
+  SB_REQUIRE(slot != nullptr, "seedb200_decode_attention_rope_lineage: null slot table");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const void *cos_t, *sin_t;
+  int max_pos;
+  SB_PROPAGATE(sb::get_rope_tables(D, 10000.0f, max_seq, &cos_t, &sin_t, &max_pos, st));
+  return sb::decode_attention_rope(qkv, positions, B, H, D, past_len, max_seq, max_pos, cos_t, sin_t, k_cache, v_cache,
+                                   out, scale, st, nullptr, slot);
+}
+
 }  // extern "C"

@@ -20,6 +20,7 @@
 
 #include <map>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -39,6 +40,7 @@ struct seedb200_llama {
   seedb200_llama_config cfg;
   std::map<std::string, seedb200_tensor> w;
   std::vector<void*> owned;
+  std::vector<void*> row_owned;   // buffers sized by max_batch (seedb200_llama_reserve_rows reallocates them)
   const __half *embed, *norm_w, *lm_head;
   std::vector<sb::LlamaLayerW> layers;
   const void *cos_t, *sin_t;
@@ -59,8 +61,9 @@ struct seedb200_llama {
   int* gstate_host;               // pinned mirror of gstate (early-stop polling)
   cudaStream_t gstream;           // private stream the decode step is captured on (the caller's may be the legacy
                                   // default stream, which cannot be captured); replays go to the caller's stream
-  cudaGraphExec_t gexec[5];       // decode-step graph per batch size (1..4)
-  int gunit_launches[5];          // kernels inside one captured unit (launch accounting of graph replays)
+  // captured decode units per (batch, beams): beams 0 = the sampler loop; value = (graph, kernels inside one unit)
+  std::map<std::pair<int, int>, std::pair<cudaGraphExec_t, int>> graphs;
+  sb::BeamState beam;             // beam-search state (rows = batch * beams <= max_batch)
   int used_graph;
   int gen_cache_len;
   // ---- int8 mode ----
@@ -157,6 +160,75 @@ static int llama_alloc(seedb200_llama* m, T** p, size_t elems) {
   return 0;
 }
 
+template <typename T>
+static int llama_alloc_row(seedb200_llama* m, T** p, size_t elems) {
+  void* q = nullptr;
+  size_t bytes = elems * sizeof(T);
+  SB_CHECK_CUDA(cudaMalloc(&q, bytes < 256 ? 256 : bytes));
+  m->row_owned.push_back(q);
+  *p = static_cast<T*>(q);
+  return 0;
+}
+
+// every buffer whose size follows max_batch: KV caches, activations, int8 workspaces, generation and beam state
+static int llama_alloc_rows(seedb200_llama* m, cudaStream_t st) {
+  const seedb200_llama_config& c = m->cfg;
+  const int64_t h = c.hidden, ffn = c.ffn;
+  const size_t cache_elems = (size_t)c.max_batch * c.heads * c.max_seq * c.head_dim;
+  for (LlamaLayerW& L : m->layers) {
+    SB_PROPAGATE(llama_alloc_row(m, &L.k_cache, cache_elems));
+    SB_PROPAGATE(llama_alloc_row(m, &L.v_cache, cache_elems));
+  }
+  const size_t T = (size_t)c.max_batch * c.max_seq;
+  SB_PROPAGATE(llama_alloc_row(m, &m->x, T * h));
+  SB_PROPAGATE(llama_alloc_row(m, &m->nb, T * h));
+  SB_PROPAGATE(llama_alloc_row(m, &m->qkv, T * 3 * h));
+  SB_PROPAGATE(llama_alloc_row(m, &m->q, T * h));
+  SB_PROPAGATE(llama_alloc_row(m, &m->att, T * h));
+  SB_PROPAGATE(llama_alloc_row(m, &m->gu, T * ffn));
+  SB_PROPAGATE(llama_alloc_row(m, &m->hn, T * h));
+  SB_PROPAGATE(llama_alloc_row(m, &m->last, (size_t)c.max_batch * h));
+  m->ca = nullptr; m->sca = nullptr; m->corr = nullptr;
+  if (m->int8) {
+    SB_PROPAGATE(llama_alloc_row(m, &m->corr, T * (size_t)(2 * ffn > 3 * h ? 2 * ffn : 3 * h)));
+    SB_PROPAGATE(llama_alloc_row(m, &m->ca, T * (size_t)(ffn > h ? ffn : h)));
+    SB_PROPAGATE(llama_alloc_row(m, &m->sca, T));
+  }
+  SB_PROPAGATE(llama_alloc_row(m, &m->da_ws, (size_t)c.max_batch * c.heads * decode_attention_max_splits(c.max_seq) * (128 + 2)));
+  SB_PROPAGATE(llama_alloc_row(m, &m->da_tickets, (size_t)c.max_batch * c.heads));   // zero now, left zero by every launch
+  SB_CHECK_CUDA(cudaMemsetAsync(m->da_tickets, 0, (size_t)c.max_batch * c.heads * sizeof(int), st));
+  SB_PROPAGATE(llama_alloc_row(m, &m->gfinished, (size_t)c.max_batch));
+  SB_PROPAGATE(llama_alloc_row(m, &m->gtok, (size_t)c.max_batch));
+  SB_PROPAGATE(llama_alloc_row(m, &m->gout, (size_t)c.max_batch * c.max_seq));
+  SB_PROPAGATE(llama_alloc_row(m, &m->glogits, (size_t)c.max_batch * m->vpad));
+  BeamState& b = m->beam;
+  const size_t R = (size_t)c.max_batch;
+  b.tokens = reinterpret_cast<long long*>(m->gtok);
+  b.state = m->gstate;
+  SB_PROPAGATE(llama_alloc_row(m, &b.beam_scores, R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.row_stats, 5 * R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.cand_score, 2 * R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.cand_idx, 2 * R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.slot, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc_row(m, &b.slot_tmp, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc_row(m, &b.hist_tok, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc_row(m, &b.hist_par, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_score, R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_len, R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_beam, R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_step, R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_n, R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.worst, R));
+  SB_PROPAGATE(llama_alloc_row(m, &b.done, R));
+  b.max_seq = c.max_seq;
+  return 0;
+}
+
+static void llama_free_rows(seedb200_llama* m) {
+  for (void* p : m->row_owned) cudaFree(p);
+  m->row_owned.clear();
+}
+
 static int llama_build(seedb200_llama* m) {
   const seedb200_llama_config& c = m->cfg;
   const int64_t h = c.hidden, ffn = c.ffn, V = c.vocab;
@@ -177,15 +249,12 @@ static int llama_build(seedb200_llama* m) {
     m->i8_loaded.assign((size_t)c.layers * 7, 0);
   }
   m->layers.resize(c.layers);
-  const size_t cache_elems = (size_t)c.max_batch * c.heads * c.max_seq * c.head_dim;
   for (int l = 0; l < c.layers; ++l) {
     LlamaLayerW& L = m->layers[l];
     auto key = [&](const char* s) { snprintf(nm, sizeof(nm), "model.layers.%d.%s", l, s); return std::string(nm); };
     const __half *wq, *wk, *wv, *wg, *wu;
     SB_PROPAGATE(llama_find(m, key("input_layernorm.weight"), &L.in_ln, h));
     SB_PROPAGATE(llama_find(m, key("post_attention_layernorm.weight"), &L.post_ln, h));
-    SB_PROPAGATE(llama_alloc(m, &L.k_cache, cache_elems));
-    SB_PROPAGATE(llama_alloc(m, &L.v_cache, cache_elems));
     L.qkv_w = L.o_w = L.gu_w = L.down_w = nullptr;
     L.qkv8 = L.o8 = L.gu8 = L.down8 = nullptr;
     L.qkv_s = L.o_s = L.gu_s = L.down_s = nullptr;
@@ -240,34 +309,17 @@ static int llama_build(seedb200_llama* m) {
     L.gu_w = fg;
   }
   SB_PROPAGATE(get_rope_tables(c.head_dim, c.rope_base, c.max_seq, &m->cos_t, &m->sin_t, &m->max_pos, st));
-  const size_t T = (size_t)c.max_batch * c.max_seq;
-  SB_PROPAGATE(llama_alloc(m, &m->x, T * h));
-  SB_PROPAGATE(llama_alloc(m, &m->nb, T * h));
-  SB_PROPAGATE(llama_alloc(m, &m->qkv, T * 3 * h));
-  SB_PROPAGATE(llama_alloc(m, &m->q, T * h));
-  SB_PROPAGATE(llama_alloc(m, &m->att, T * h));
-  SB_PROPAGATE(llama_alloc(m, &m->gu, T * ffn));
-  SB_PROPAGATE(llama_alloc(m, &m->hn, T * h));
-  SB_PROPAGATE(llama_alloc(m, &m->last, (size_t)c.max_batch * h));
-  m->ca = nullptr; m->sca = nullptr; m->olist = nullptr; m->ocount = nullptr; m->corr = nullptr;
+  m->olist = nullptr; m->ocount = nullptr;
   if (m->int8) {
-    SB_PROPAGATE(llama_alloc(m, &m->corr, T * (size_t)(2 * ffn > 3 * h ? 2 * ffn : 3 * h)));
-    const size_t kmax = (size_t)(ffn > h ? ffn : h);
-    SB_PROPAGATE(llama_alloc(m, &m->ca, T * kmax));
-    SB_PROPAGATE(llama_alloc(m, &m->sca, T));
-    SB_PROPAGATE(llama_alloc(m, &m->olist, kmax));
+    SB_PROPAGATE(llama_alloc(m, &m->olist, (size_t)(ffn > h ? ffn : h)));
     SB_PROPAGATE(llama_alloc(m, &m->ocount, 1));
   }
-  SB_PROPAGATE(llama_alloc(m, &m->da_ws, (size_t)c.max_batch * c.heads * decode_attention_max_splits(c.max_seq) * (128 + 2)));
-  SB_PROPAGATE(llama_alloc(m, &m->da_tickets, (size_t)c.max_batch * c.heads));   // zero now, left zero by every launch
-  SB_CHECK_CUDA(cudaMemsetAsync(m->da_tickets, 0, (size_t)c.max_batch * c.heads * sizeof(int), st));
   m->vpad = (c.vocab + 7) / 8 * 8;
   SB_PROPAGATE(llama_alloc(m, &m->gstate, 8));
-  SB_PROPAGATE(llama_alloc(m, &m->gfinished, (size_t)c.max_batch));
-  SB_PROPAGATE(llama_alloc(m, &m->gtok, (size_t)c.max_batch));
-  SB_PROPAGATE(llama_alloc(m, &m->gout, (size_t)c.max_batch * c.max_seq));
-  SB_PROPAGATE(llama_alloc(m, &m->glogits, (size_t)c.max_batch * m->vpad));
   SB_PROPAGATE(llama_alloc(m, &m->gparams, 1));
+  SB_PROPAGATE(llama_alloc(m, &m->beam.params, 1));
+  SB_PROPAGATE(llama_alloc(m, &m->beam.n_out, 1));
+  SB_PROPAGATE(llama_alloc_rows(m, st));
   SB_CHECK_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->gstate_host), 8 * sizeof(int)));
   SB_CHECK_CUDA(cudaStreamCreateWithFlags(&m->gstream, cudaStreamNonBlocking));
   SB_CHECK_CUDA(cudaStreamSynchronize(st));
@@ -306,7 +358,7 @@ static int lin8(seedb200_llama* m, cudaStream_t st, int M, int N, int K, const v
 // host value `past_len` -- what makes a captured decode step position independent (S must be 1).
 static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void* inputs_embeds,
                          const int64_t* position_ids, int B, int S, int past_len, int logits_mode, void* logits,
-                         int64_t logits_ld, cudaStream_t st, const int* dyn = nullptr) {
+                         int64_t logits_ld, cudaStream_t st, const int* dyn = nullptr, const int* slot = nullptr) {
   const seedb200_llama_config& c = m->cfg;
   const int h = c.hidden, H = c.heads, D = c.head_dim, ffn = c.ffn, V = c.vocab, ct = c.gemm_ctas;
   const int T = B * S;
@@ -338,13 +390,13 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
     if (fused_attn) {
       // cached decode step: RoPE + append + attention in one launch (bit-identical to the pair below up to 512 keys)
       SB_PROPAGATE(decode_attention_rope(m->qkv, position_ids, B, H, D, past_len, c.max_seq, m->max_pos, m->cos_t,
-                                         m->sin_t, L.k_cache, L.v_cache, m->att, scale, st, dyn));
+                                         m->sin_t, L.k_cache, L.v_cache, m->att, scale, st, dyn, slot));
     } else {
     SB_PROPAGATE(rope_kv_append_tables(m->qkv, position_ids, B, S, H, D, past_len, c.max_seq, m->max_pos, m->cos_t,
                                        m->sin_t, m->q, L.k_cache, L.v_cache, st, dyn));
     if (S == 1) {
       SB_PROPAGATE(decode_attention(m->q, L.k_cache, L.v_cache, m->att, B, H, D, kv_len, c.max_seq, scale, m->da_ws, st, dyn,
-                                    m->da_tickets));
+                                    m->da_tickets, slot));
     } else {
       seedb200_attn_desc a;
       memset(&a, 0, sizeof(a));
@@ -406,22 +458,33 @@ __global__ void gen_reset_kernel(GenParams gp, GenParams* dst, int* state, int* 
   if (threadIdx.x < B) finished[threadIdx.x] = 0;
 }
 
-// one unit of the loop: cached forward of the tokens in m->gtok, then the sampler (which also advances the device
-// counters).  Every launch argument is a handle-owned pointer or a constant: the unit can be captured once.
-static int gen_unit(seedb200_llama* m, int B, cudaStream_t st) {
+// one unit of the loop: cached forward of the tokens in m->gtok, then the sampler (beams == 0) or the beam candidates
+// and scorer (which also advance the device counters).  Every launch argument is a handle-owned pointer or a
+// constant: the unit can be captured once per (B, beams).
+static int gen_unit(seedb200_llama* m, int B, int beams, cudaStream_t st) {
   PdlScope pdl(get_option("decode_pdl") != 0);
-  SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B, 1, 0, 1, m->glogits, m->vpad, st, m->gstate));
-  SB_PROPAGATE(sample(m->glogits, m->vpad, B, m->cfg.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/1,
-                      m->gtok, m->gout, m->cfg.max_seq, m->gfinished, st));
+  if (beams == 0) {
+    SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B, 1, 0, 1, m->glogits, m->vpad, st, m->gstate));
+    SB_PROPAGATE(sample(m->glogits, m->vpad, B, m->cfg.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/1,
+                        m->gtok, m->gout, m->cfg.max_seq, m->gfinished, st));
+    return 0;
+  }
+  const int rows = B * beams;
+  SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, rows, 1, 0, 1, m->glogits, m->vpad, st, m->gstate,
+                             m->beam.slot));
+  SB_PROPAGATE(beam_select(m->glogits, (int64_t)beams * m->vpad, m->vpad, B, beams, m->cfg.vocab, m->beam.beam_scores,
+                           nullptr, m->beam.params, 0, m->gstate, m->beam.row_stats, m->beam.cand_score,
+                           m->beam.cand_idx, st));
+  SB_PROPAGATE(beam_score(m->beam, B, beams, m->cfg.vocab, /*advance_cache=*/1, st));
   return 0;
 }
 
-static int gen_capture(seedb200_llama* m, int B) {
+static int gen_capture(seedb200_llama* m, int B, int beams) {
   cudaGraph_t graph = nullptr;
   cudaStream_t st = m->gstream;
   SB_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   const int64_t before = seedb200_launch_count();
-  const int s = gen_unit(m, B, st);
+  const int s = gen_unit(m, B, beams, st);
   const int unit = (int)(seedb200_launch_count() - before);
   count_launch(-unit);                        // captured, not executed
   const cudaError_t e = cudaStreamEndCapture(st, &graph);
@@ -443,8 +506,54 @@ static int gen_capture(seedb200_llama* m, int B) {
     cudaGetLastError();
     return SEEDB200_ERR_CUDA;
   }
-  m->gexec[B] = exec;
-  m->gunit_launches[B] = unit;
+  m->graphs[std::make_pair(B, beams)] = std::make_pair(exec, unit);
+  return 0;
+}
+
+// run `units` decode units (the first eagerly, the rest replayed from the (B, beams) graph when use_graph); with
+// `poll`, the device flag state[poll] is read every 32 units and the loop stops once it is set.  Returns units run.
+static int gen_run_units(seedb200_llama* m, int B, int beams, int units, int use_graph, int poll, cudaStream_t st,
+                         int* done_out) {
+  int done = 0;
+  m->used_graph = 0;
+  if (units > 0) {   // first unit eagerly (also resolves every lazily-set function attribute before a capture)
+    SB_PROPAGATE(gen_unit(m, B, beams, st));
+    done = 1;
+  }
+  const auto key = std::make_pair(B, beams);
+  if (units > done && use_graph) {
+    if (m->graphs.find(key) == m->graphs.end()) {
+      int s = gen_capture(m, B, beams);
+      if (s != 0 && get_option("decode_pdl") != 0) {   // retry without programmatic launches inside the graph
+        seedb200_set_option("decode_pdl", 0);
+        s = gen_capture(m, B, beams);
+        seedb200_set_option("decode_pdl", 1);
+      }
+      if (s != 0) return s;
+    }
+    m->used_graph = 1;
+  }
+  bool stop = false;
+  while (done < units && !stop) {
+    int chunk = units - done;
+    if (poll >= 0 && chunk > 32) chunk = 32;
+    for (int i = 0; i < chunk; ++i) {
+      if (m->used_graph) {
+        const auto& g = m->graphs[key];
+        SB_CHECK_CUDA(cudaGraphLaunch(g.first, st));
+        count_launch(g.second);
+      } else {
+        SB_PROPAGATE(gen_unit(m, B, beams, st));
+      }
+    }
+    done += chunk;
+    if (poll >= 0 && done < units) {
+      SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
+      SB_CHECK_CUDA(cudaStreamSynchronize(st));
+      stop = poll == 3 ? m->gstate_host[3] < m->gstate_host[1] : m->gstate_host[poll] != 0;
+    }
+  }
+  *done_out = done;
   return 0;
 }
 
@@ -461,48 +570,13 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
   // token 0 comes from the prefill logits: the step counter advances, the cache length does not
   SB_PROPAGATE(sample(m->glogits, m->vpad, B, c.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/0, m->gtok,
                       m->gout, c.max_seq, m->gfinished, st));
-  int units = max_new - 1, done = 0;
-  m->used_graph = 0;
-  auto all_finished = [&](bool* stop) -> int {   // early stop: poll the device counters (only with an eos id)
-    SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 5 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    SB_CHECK_CUDA(cudaStreamSynchronize(st));
-    *stop = m->gstate_host[3] < m->gstate_host[1];      // a step ran with every sequence already finished
-    return 0;
-  };
-  if (units > 0) {   // first unit eagerly (also resolves every lazily-set function attribute before a capture)
-    SB_PROPAGATE(gen_unit(m, B, st));
-    done = 1;
-  }
-  if (units > done && use_graph) {
-    if (m->gexec[B] == nullptr) {
-      int s = gen_capture(m, B);
-      if (s != 0 && get_option("decode_pdl") != 0) {   // retry without programmatic launches inside the graph
-        seedb200_set_option("decode_pdl", 0);
-        s = gen_capture(m, B);
-        seedb200_set_option("decode_pdl", 1);
-      }
-      if (s != 0) return s;
-    }
-    m->used_graph = 1;
-  }
-  bool stop = false;
-  while (done < units && !stop) {
-    int chunk = units - done;
-    if (eos >= 0 && chunk > 32) chunk = 32;
-    for (int i = 0; i < chunk; ++i) {
-      if (m->used_graph) {
-        SB_CHECK_CUDA(cudaGraphLaunch(m->gexec[B], st));
-        count_launch(m->gunit_launches[B]);
-      } else {
-        SB_PROPAGATE(gen_unit(m, B, st));
-      }
-    }
-    done += chunk;
-    if (eos >= 0 && done < units) SB_PROPAGATE(all_finished(&stop));
-  }
+  int done = 0;
+  // early stop (only with an eos id): a step ran with every sequence already finished (state[3] < state[1])
+  SB_PROPAGATE(gen_run_units(m, B, 0, max_new - 1, use_graph, eos >= 0 ? 3 : -1, st, &done));
   int n_valid = done + 1;
   if (eos >= 0) {
-    SB_PROPAGATE(all_finished(&stop));
+    SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    SB_CHECK_CUDA(cudaStreamSynchronize(st));
     n_valid = m->gstate_host[3];
   }
   if (tokens_out != nullptr)
@@ -511,6 +585,36 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
   if (n_generated_host != nullptr) *n_generated_host = n_valid;
   m->gen_cache_len = S + done;     // tokens whose K/V are in the cache
   return 0;
+}
+
+// beam search: prefill at B rows, candidates + scorer from the prefill logits (every beam reads its sequence's row),
+// then max_new - 1 units of (forward of B * k rows through the lineage table -> candidates -> scorer), then finalize
+static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, int max_new,
+                               const seedb200_beam_params* p, int64_t eos, int64_t pad, int use_graph,
+                               int64_t* tokens_out, int* n_out_host, float* best_scores, cudaStream_t st) {
+  const seedb200_llama_config& c = m->cfg;
+  const int k = p->num_beams;
+  const BeamParams bp = beam_params(*p, eos, pad, S, max_new, B);
+  SB_PROPAGATE(beam_init(m->beam, bp, st));
+  SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, m->vpad, st));
+  SB_PROPAGATE(beam_select(m->glogits, m->vpad, 0, B, k, c.vocab, m->beam.beam_scores, nullptr, m->beam.params, 0,
+                           m->gstate, m->beam.row_stats, m->beam.cand_score,
+                           m->beam.cand_idx, st));
+  SB_PROPAGATE(beam_score(m->beam, B, k, c.vocab, /*advance_cache=*/0, st));
+  int done = 0;
+  SB_PROPAGATE(gen_run_units(m, B, k, max_new - 1, use_graph, eos >= 0 ? 5 : -1, st, &done));
+  SB_PROPAGATE(beam_finalize(m->beam, B, tokens_out, max_new, best_scores, st));
+  int n_out = 0;
+  SB_CHECK_CUDA(cudaMemcpyAsync(&n_out, m->beam.n_out, sizeof(int), cudaMemcpyDeviceToHost, st));
+  SB_CHECK_CUDA(cudaStreamSynchronize(st));
+  if (n_out_host != nullptr) *n_out_host = n_out;
+  m->gen_cache_len = 0;            // the cache rows now hold beam lineages, not B plain sequences
+  return 0;
+}
+
+static void llama_drop_graphs(seedb200_llama* m) {
+  for (auto& g : m->graphs) cudaGraphExecDestroy(g.second.first);
+  m->graphs.clear();
 }
 
 // every int8 linear must hold its weights before the model runs
@@ -549,7 +653,7 @@ static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor*
   m->gstream = nullptr;
   m->used_graph = -1;
   m->gen_cache_len = 0;
-  for (int i = 0; i < 5; ++i) { m->gexec[i] = nullptr; m->gunit_launches[i] = 0; }
+  memset(&m->beam, 0, sizeof(m->beam));
   m->int8 = int8;
   m->threshold = threshold;
   for (int i = 0; i < n_weights; ++i) m->w[std::string(weights[i].name)] = weights[i];
@@ -599,10 +703,10 @@ int seedb200_llama_int8_load_weight(seedb200_llama* llm, const char* name, const
 
 void seedb200_llama_destroy(seedb200_llama* llm) {
   if (!llm) return;
-  for (int i = 0; i < 5; ++i)
-    if (llm->gexec[i]) cudaGraphExecDestroy(llm->gexec[i]);
+  sb::llama_drop_graphs(llm);
   if (llm->gstate_host) cudaFreeHost(llm->gstate_host);
   if (llm->gstream) cudaStreamDestroy(llm->gstream);
+  sb::llama_free_rows(llm);
   for (void* p : llm->owned) cudaFree(p);
   delete llm;
 }
@@ -648,6 +752,53 @@ int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int 
 }
 
 int seedb200_llama_generate_used_graph(seedb200_llama* llm) { return llm ? llm->used_graph : -1; }
+
+int seedb200_llama_beam_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                                 const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id, int use_graph,
+                                 int64_t* tokens_out, int* n_out_host, float* best_scores_out, void* stream) {
+  SB_REQUIRE(llm && prompt_ids && bp && tokens_out, "llama_beam_generate: null argument");
+  SB_REQUIRE(bp->num_beams >= 1 && bp->num_beams <= sb::BEAM_MAX, "llama_beam_generate: num_beams %d outside [1,%d]",
+             bp->num_beams, sb::BEAM_MAX);
+  SB_REQUIRE(B >= 1 && (int64_t)B * bp->num_beams <= llm->cfg.max_batch,
+             "llama_beam_generate: batch %d x %d beams exceeds max_batch %d (seedb200_llama_reserve_rows)", B,
+             bp->num_beams, llm->cfg.max_batch);
+  SB_REQUIRE(S >= 1 && max_new_tokens >= 1 && S + max_new_tokens <= llm->cfg.max_seq,
+             "llama_beam_generate: prompt %d + %d new tokens exceeds max_seq %d", S, max_new_tokens, llm->cfg.max_seq);
+  SB_REQUIRE(!bp->do_sample || (bp->temperature > 0.0f && bp->top_p > 0.0f),
+             "llama_beam_generate: temperature and top_p must be > 0 when sampling");
+  SB_REQUIRE(bp->early_stopping >= 0 && bp->early_stopping <= 2, "llama_beam_generate: early_stopping %d not in {0,1,2}",
+             bp->early_stopping);
+  SB_REQUIRE(eos_id < llm->cfg.vocab, "llama_beam_generate: eos_id %lld outside the vocabulary", (long long)eos_id);
+  SB_PROPAGATE(sb::llama_int8_ready(llm));
+  sb::DeviceGuard guard(llm->device);
+  return sb::llama_beam_generate(llm, prompt_ids, B, S, max_new_tokens, bp, eos_id, pad_id, use_graph, tokens_out,
+                                 n_out_host, best_scores_out, static_cast<cudaStream_t>(stream));
+}
+
+int seedb200_llama_reserve_rows(seedb200_llama* llm, int rows) {
+  SB_REQUIRE(llm != nullptr, "llama_reserve_rows: null handle");
+  SB_REQUIRE(rows >= 1, "llama_reserve_rows: rows %d < 1", rows);
+  if (rows <= llm->cfg.max_batch) return 0;
+  sb::DeviceGuard guard(llm->device);
+  SB_CHECK_CUDA(cudaDeviceSynchronize());
+  sb::llama_drop_graphs(llm);
+  sb::llama_free_rows(llm);
+  const int old = llm->cfg.max_batch;
+  llm->cfg.max_batch = rows;
+  int s = sb::llama_alloc_rows(llm, 0);
+  if (s != 0) {                      // keep the handle usable at its old size
+    std::string err = seedb200_last_error();
+    sb::llama_free_rows(llm);
+    llm->cfg.max_batch = old;
+    if (sb::llama_alloc_rows(llm, 0) != 0) llm->cfg.max_batch = 0;
+    sb::set_error("llama_reserve_rows: %s", err.c_str());
+    return s;
+  }
+  SB_CHECK_CUDA(cudaStreamSynchronize(0));
+  llm->last_T = 0;
+  llm->gen_cache_len = 0;
+  return 0;
+}
 
 int seedb200_llama_kv_ptrs(seedb200_llama* llm, int layer, void** k, void** v) {
   SB_REQUIRE(llm && k && v && layer >= 0 && layer < (int)llm->layers.size(), "llama_kv_ptrs: bad arguments");

@@ -327,10 +327,22 @@ __host__ __device__ inline void da_split(int kv_len, int& nsplit, int& chunk) {
   nsplit = (kv_len + chunk - 1) / chunk;
 }
 
+// Lineage (LIN): cached key / value p of row b is read from row slot[b * max_seq + p] of the caches instead of row b
+// (beam search: beams share the prefix they inherited without copying it).  Only the addresses change.
+template <bool LIN>
+__device__ __forceinline__ long long da_row(const int* __restrict__ slot, long long base, int b, int H, int h,
+                                            int max_seq, int p) {
+  if (!LIN) return base + (long long)p * DA_D;
+  const long long r = slot[(long long)b * max_seq + p];
+  return ((r * H + h) * max_seq + p) * DA_D;
+}
+
+template <bool LIN>
 __global__ void __launch_bounds__(128)
 decode_attn_partial(const __half* __restrict__ q, const __half* __restrict__ kc, const __half* __restrict__ vc,
                     float* __restrict__ ws, int H, int kv_len, int max_seq, int chunk, float scale_log2,
-                    const int* __restrict__ dyn, int* __restrict__ tickets, __half* __restrict__ out) {
+                    const int* __restrict__ dyn, int* __restrict__ tickets, __half* __restrict__ out,
+                    const int* __restrict__ slot) {
   const int split = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   int nsplit = gridDim.x;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -360,12 +372,12 @@ decode_attn_partial(const __half* __restrict__ q, const __half* __restrict__ kc,
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       const int t = g + 8 * i;
-      vv[i] = t < cnt ? __ldg(reinterpret_cast<const uint4*>(vc + base + (long long)(kb + t) * DA_D) + c)
+      vv[i] = t < cnt ? __ldg(reinterpret_cast<const uint4*>(vc + da_row<LIN>(slot, base, b, H, h, max_seq, kb + t)) + c)
                       : make_uint4(0, 0, 0, 0);
     }
     float s = -INFINITY;
     if (tid < cnt) {
-      const uint4* kr = reinterpret_cast<const uint4*>(kc + base + (long long)(kb + tid) * DA_D);
+      const uint4* kr = reinterpret_cast<const uint4*>(kc + da_row<LIN>(slot, base, b, H, h, max_seq, kb + tid));
       uint4 kk[16];
 #pragma unroll
       for (int i = 0; i < 16; ++i) kk[i] = __ldg(kr + i);
@@ -480,11 +492,13 @@ decode_attn_merge(const float* __restrict__ ws, __half* __restrict__ out, int ns
 // ----------------------------------------------------------------------------
 constexpr int DAF_MAX_GROUPS = 4;
 
+template <bool LIN>
 __global__ void __launch_bounds__(DAF_MAX_GROUPS * 128)
 decode_attn_rope_kernel(const __half* __restrict__ qkv, const long long* __restrict__ positions,
                         const __half* __restrict__ cos_t, const __half* __restrict__ sin_t, int max_pos,
                         __half* __restrict__ kc, __half* __restrict__ vc, int H, int past_len, int max_seq,
-                        float scale_log2, const int* __restrict__ dyn, __half* __restrict__ out) {
+                        float scale_log2, const int* __restrict__ dyn, __half* __restrict__ out,
+                        const int* __restrict__ slot) {
   const int h = blockIdx.x, b = blockIdx.y;
   const int tid = threadIdx.x, grp = tid >> 7, gt = tid & 127, ng = blockDim.x >> 7;
   const int warp = gt >> 5, lane = tid & 31;
@@ -545,13 +559,13 @@ decode_attn_rope_kernel(const __half* __restrict__ qkv, const long long* __restr
       const int t = g + 8 * i;
       if (t >= cnt) vv[i] = make_uint4(0, 0, 0, 0);
       else if (kb + t == crow) vv[i] = *(reinterpret_cast<const uint4*>(s_vn) + c);
-      else vv[i] = __ldg(reinterpret_cast<const uint4*>(vc + base + (long long)(kb + t) * DA_D) + c);
+      else vv[i] = __ldg(reinterpret_cast<const uint4*>(vc + da_row<LIN>(slot, base, b, H, h, max_seq, kb + t)) + c);
     }
     float s = -INFINITY;
     if (gt < cnt) {
       const bool fresh = (kb + gt == crow);
       const uint4* kr = fresh ? reinterpret_cast<const uint4*>(s_kn)
-                              : reinterpret_cast<const uint4*>(kc + base + (long long)(kb + gt) * DA_D);
+                              : reinterpret_cast<const uint4*>(kc + da_row<LIN>(slot, base, b, H, h, max_seq, kb + gt));
       uint4 kk[16];
       if (fresh) {
 #pragma unroll
@@ -636,7 +650,7 @@ bool decode_attention_rope_supported(int D, int max_seq) {
 // The thread-group count depends on max_seq only, so eager launches and the captured decode step run the same code.
 int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int H, int D, int past_len, int max_seq,
                           int max_pos, const void* cos_t, const void* sin_t, void* k_cache, void* v_cache, void* out,
-                          float scale, cudaStream_t stream, const int* dyn) {
+                          float scale, cudaStream_t stream, const int* dyn, const int* slot) {
   SB_REQUIRE(qkv && k_cache && v_cache && out && cos_t && sin_t, "decode_attention_rope: null operand");
   SB_REQUIRE(decode_attention_rope_supported(D, max_seq),
              "decode_attention_rope: head_dim %d / max_seq %d unsupported (head_dim 128, max_seq <= %d)", D, max_seq,
@@ -645,11 +659,12 @@ int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int 
              past_len, max_seq);
   int ng = (max_seq + DA_BLK - 1) / DA_BLK;
   if (ng > DAF_MAX_GROUPS) ng = DAF_MAX_GROUPS;
-  SB_CHECK_CUDA(launch_chain(decode_attn_rope_kernel, dim3(H, B), dim3(ng * 128), 0, stream,
+  SB_CHECK_CUDA(launch_chain(slot ? decode_attn_rope_kernel<true> : decode_attn_rope_kernel<false>, dim3(H, B),
+                             dim3(ng * 128), 0, stream,
                              static_cast<const __half*>(qkv), reinterpret_cast<const long long*>(positions),
                              static_cast<const __half*>(cos_t), static_cast<const __half*>(sin_t), max_pos,
                              static_cast<__half*>(k_cache), static_cast<__half*>(v_cache), H, past_len, max_seq,
-                             scale * 1.4426950408889634f, dyn, static_cast<__half*>(out)));
+                             scale * 1.4426950408889634f, dyn, static_cast<__half*>(out), slot));
   SB_LAUNCH_CHECK();
   return 0;
 }
@@ -665,7 +680,7 @@ int decode_attention_max_splits(int max_seq) {
 // so a handle zeroes it once at create and never again.
 int decode_attention(const void* q, const void* k_cache, const void* v_cache, void* out, int B, int H, int D,
                      int kv_len, int max_seq, float scale, void* workspace, cudaStream_t stream, const int* dyn,
-                     int* tickets) {
+                     int* tickets, const int* slot) {
   SB_REQUIRE(D == DA_D, "decode_attention: head_dim %d unsupported (LLaMA uses 128)", D);
   SB_REQUIRE(dyn != nullptr || (kv_len >= 1 && kv_len <= max_seq), "decode_attention: kv_len %d outside [1,%d]", kv_len, max_seq);
   int nsplit, chunk;
@@ -676,10 +691,11 @@ int decode_attention(const void* q, const void* k_cache, const void* v_cache, vo
     SB_CHECK_CUDA(cudaMemsetAsync(tickets, 0, (size_t)B * H * sizeof(int), stream));
   }
   dim3 grid(nsplit, H, B);
-  SB_CHECK_CUDA(launch_chain(decode_attn_partial, grid, dim3(128), 0, stream, static_cast<const __half*>(q),
+  SB_CHECK_CUDA(launch_chain(slot ? decode_attn_partial<true> : decode_attn_partial<false>, grid, dim3(128), 0, stream,
+                             static_cast<const __half*>(q),
                              static_cast<const __half*>(k_cache), static_cast<const __half*>(v_cache),
                              static_cast<float*>(workspace), H, kv_len, max_seq, chunk, scale * 1.4426950408889634f, dyn,
-                             tickets, static_cast<__half*>(out)));
+                             tickets, static_cast<__half*>(out), slot));
   SB_LAUNCH_CHECK();
   return 0;
 }
@@ -705,6 +721,14 @@ int seedb200_decode_attention(const void* q, const void* k_cache, const void* v_
   SB_REQUIRE(q && k_cache && v_cache && out && workspace, "seedb200_decode_attention: null operand");
   return sb::decode_attention(q, k_cache, v_cache, out, B, H, D, kv_len, max_seq, scale, workspace,
                               static_cast<cudaStream_t>(stream));
+}
+
+int seedb200_decode_attention_lineage(const void* q, const void* k_cache, const void* v_cache, const int32_t* slot,
+                                      void* out, int B, int H, int D, int kv_len, int max_seq, float scale,
+                                      void* workspace, void* stream) {
+  SB_REQUIRE(q && k_cache && v_cache && slot && out && workspace, "seedb200_decode_attention_lineage: null operand");
+  return sb::decode_attention(q, k_cache, v_cache, out, B, H, D, kv_len, max_seq, scale, workspace,
+                              static_cast<cudaStream_t>(stream), nullptr, nullptr, slot);
 }
 
 }  // extern "C"

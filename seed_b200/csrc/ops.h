@@ -40,13 +40,15 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
 // dyn (optional, device): kv_len = dyn[0] + 1 at run time; the grid is then sized for max_seq keys
 int decode_attention(const void* q, const void* k_cache, const void* v_cache, void* out, int B, int H, int D,
                      int kv_len, int max_seq, float scale, void* workspace, cudaStream_t stream,
-                     const int* dyn = nullptr, int* tickets = nullptr);
+                     const int* dyn = nullptr, int* tickets = nullptr, const int* slot = nullptr);
 int decode_attention_max_splits(int max_seq);
 // RoPE of the new token's q / k + KV append + attention in one launch (max_seq <= 2048); dyn as above (past_len = dyn[0])
 bool decode_attention_rope_supported(int D, int max_seq);
 int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int H, int D, int past_len, int max_seq,
                           int max_pos, const void* cos_t, const void* sin_t, void* k_cache, void* v_cache, void* out,
-                          float scale, cudaStream_t stream, const int* dyn = nullptr);
+                          float scale, cudaStream_t stream, const int* dyn = nullptr, const int* slot = nullptr);
+// slot (optional, device) [B, max_seq] int32: cached key / value p of row b lives in cache row slot[b*max_seq + p]
+// (beam lineage); NULL = row b.  The new token is still appended at row b.
 // sampler.cu
 struct GenParams { seedb200_sample_params sp; long long eos, pad; };
 // gp (host, by value) or gp_dev (device, read at run time); state (device, optional) = {cache length, step, arrive,
@@ -54,6 +56,52 @@ struct GenParams { seedb200_sample_params sp; long long eos, pad; };
 int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, const GenParams* gp_dev, uint64_t step,
            int* state, int advance_cache, int64_t* tokens, int64_t* out, int64_t out_ld, int* finished,
            cudaStream_t stream);
+// beam search (sampler.cu: candidates; beam.cu: scorer, bookkeeping, finalize)
+constexpr int BEAM_MAX = 8;
+struct BeamParams {                    // read by the beam kernels at run time (graph replay)
+  int k, do_sample, early_stopping, S, max_new, B;
+  float temperature, top_p;
+  double length_penalty;
+  unsigned long long seed, offset;
+  long long eos, pad;
+};
+inline BeamParams beam_params(const seedb200_beam_params& p, long long eos, long long pad, int S, int max_new, int B) {
+  BeamParams b;
+  b.k = p.num_beams; b.do_sample = p.do_sample; b.early_stopping = p.early_stopping; b.S = S; b.max_new = max_new;
+  b.B = B; b.temperature = p.temperature; b.top_p = p.top_p; b.length_penalty = p.length_penalty;
+  b.seed = p.seed; b.offset = p.offset; b.eos = eos; b.pad = pad;
+  return b;
+}
+// logits row of (sequence i, beam j) = logits + i * seq_ld + j * beam_ld; -> cand_score / cand_idx [B, 2k]
+int beam_select(const void* logits, int64_t seq_ld, int64_t beam_ld, int B, int k, int V, const float* beam_scores,
+                const BeamParams* bp, const BeamParams* bp_dev, uint64_t step, const int* state, float* row_stats,
+                float* cand_score, int* cand_idx, cudaStream_t stream);   // row_stats: [B*k, 5] scratch
+// the device state of one beam-search run (rows = B * k <= max_batch; hyps: k per sequence)
+struct BeamState {
+  BeamParams* params;
+  int* state;            // {cache length, step, arrive counter, -, -, all sequences done}
+  float* beam_scores;    // [rows]
+  float* row_stats;      // [rows, 5] per-row statistics of the candidate kernel
+  float* cand_score;     // [rows * 2]
+  int* cand_idx;         // [rows * 2]
+  long long* tokens;     // [rows] next decode input
+  int* slot;             // [rows, max_seq] lineage table
+  int* slot_tmp;         // [rows, max_seq]
+  long long* hist_tok;   // [max_seq, rows] token chosen at step t by beam b
+  int* hist_par;         // [max_seq, rows] its parent beam (within the sequence)
+  double* hyp_score;     // [rows]: k finished hypotheses per sequence, in insertion order
+  int* hyp_len;          // [rows] length including the prompt
+  int* hyp_beam;         // [rows] beam whose sequence after step hyp_step it is
+  int* hyp_step;         // [rows]
+  int* hyp_n;            // [rows] (first B used)
+  double* worst;         // [rows]
+  int* done;             // [rows]
+  int* n_out;            // [1]
+  int max_seq;
+};
+int beam_init(const BeamState& st, const BeamParams& bp, cudaStream_t stream);
+int beam_score(const BeamState& st, int B, int k, int V, int advance_cache, cudaStream_t stream);
+int beam_finalize(const BeamState& st, int B, int64_t* tokens_out, int64_t ld, float* best_scores, cudaStream_t stream);
 int image_ids_to_tokens(const int64_t* ids, int n, int64_t shift, int64_t boi, int64_t eoi, int64_t* out,
                         int64_t out_stride, cudaStream_t stream);
 int cur_device();

@@ -37,6 +37,8 @@ EXPORTS = [
     "seedb200_gemm_plan", "seedb200_gemm_schedule_tile", "seedb200_decode_attention_rope",
     "seedb200_int8_quantize_weight", "seedb200_int8_quantize_act", "seedb200_gemm_int8", "seedb200_gemv_int8",
     "seedb200_llama_create_int8", "seedb200_llama_int8_load_weight",
+    "seedb200_beam_select", "seedb200_llama_beam_generate", "seedb200_llama_reserve_rows",
+    "seedb200_decode_attention_lineage", "seedb200_decode_attention_rope_lineage",
 ]
 
 DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
@@ -99,6 +101,24 @@ class LlamaConfig(C.Structure):
 class SampleParams(C.Structure):
     _fields_ = [("do_sample", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float), ("seed", C.c_uint64),
                 ("offset", C.c_uint64)]
+
+
+class BeamParams(C.Structure):
+    _fields_ = [("num_beams", C.c_int32), ("do_sample", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float),
+                ("length_penalty", C.c_double), ("early_stopping", C.c_int32), ("seed", C.c_uint64),
+                ("offset", C.c_uint64)]
+
+
+# early_stopping of transformers' GenerationConfig -> seedb200_beam_params.early_stopping
+EARLY_STOPPING = {False: 0, True: 1, "never": 2}
+
+
+def beam_params(num_beams: int, do_sample: bool = False, temperature: float = 1.0, top_p: float = 1.0,
+                length_penalty: float = 1.0, early_stopping=False, seed: int = 0, offset: int = 0) -> BeamParams:
+    if early_stopping not in EARLY_STOPPING:
+        raise ValueError(f"early_stopping must be False, True or 'never' (got {early_stopping!r})")
+    return BeamParams(int(num_beams), int(bool(do_sample)), float(temperature), float(top_p), float(length_penalty),
+                      EARLY_STOPPING[early_stopping], int(seed), int(offset))
 
 
 _lib: Optional[C.CDLL] = None
@@ -191,6 +211,15 @@ def load() -> C.CDLL:
     lib.seedb200_llama_create_int8.argtypes = [C.POINTER(LlamaConfig), C.POINTER(Tensor), C.c_int, C.c_float,
                                                C.POINTER(C.c_void_p)]
     lib.seedb200_llama_int8_load_weight.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.seedb200_beam_select.argtypes = [C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                         C.POINTER(BeamParams), C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.seedb200_llama_beam_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                 C.POINTER(BeamParams), C.c_int64, C.c_int64, C.c_int, C.c_void_p,
+                                                 C.POINTER(C.c_int), C.c_void_p, C.c_void_p]
+    lib.seedb200_llama_reserve_rows.argtypes = [C.c_void_p, C.c_int]
+    lib.seedb200_decode_attention_lineage.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                      C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                                      C.c_void_p, C.c_void_p]
     _lib = lib
     return lib
 
@@ -574,6 +603,76 @@ def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tens
     return out
 
 
+def decode_attention_lineage(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, slot: torch.Tensor,
+                             kv_len: int, scale: float) -> torch.Tensor:
+    """decode_attention where row b reads cached key / value p from cache row slot[b, p] (slot [B, max_seq] int32)."""
+    _need_cuda_f16(q, "decode_attention_lineage.q")
+    B, H, D = q.shape
+    max_seq = k_cache.shape[2]
+    if not (k_cache.is_contiguous() and v_cache.is_contiguous() and q.is_contiguous()):
+        raise RuntimeError("decode_attention_lineage: q and the caches must be contiguous")
+    if slot.dtype != torch.int32 or tuple(slot.shape) != (B, max_seq) or not slot.is_contiguous():
+        raise RuntimeError("decode_attention_lineage: slot must be contiguous int32 [B, max_seq]")
+    out = torch.empty((B, H * D), dtype=torch.float16, device=q.device)
+    nbytes = int(load().seedb200_decode_attention_workspace_bytes(B, H, max_seq))
+    ws = torch.empty((nbytes,), dtype=torch.uint8, device=q.device)
+    with on(q.device):
+        check(load().seedb200_decode_attention_lineage(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                       slot.data_ptr(), out.data_ptr(), B, H, D, kv_len, max_seq, scale,
+                                                       ws.data_ptr(), stream_ptr(q.device)),
+              "seedb200_decode_attention_lineage")
+    return out
+
+
+def decode_attention_rope_lineage(qkv: torch.Tensor, slot: torch.Tensor, H: int, past_len: int, k_cache: torch.Tensor,
+                                  v_cache: torch.Tensor, scale: float) -> torch.Tensor:
+    """decode_attention_rope where row b reads cached position p < past_len from cache row slot[b, p]"""
+    _need_cuda_f16(qkv, "decode_attention_rope_lineage.qkv")
+    B = qkv.shape[0]
+    D = qkv.shape[1] // (3 * H)
+    max_seq = k_cache.shape[2]
+    if not (k_cache.is_contiguous() and v_cache.is_contiguous() and qkv.is_contiguous()):
+        raise RuntimeError("decode_attention_rope_lineage: qkv and the caches must be contiguous")
+    if slot.dtype != torch.int32 or tuple(slot.shape) != (B, max_seq) or not slot.is_contiguous():
+        raise RuntimeError("decode_attention_rope_lineage: slot must be contiguous int32 [B, max_seq]")
+    out = torch.empty((B, H * D), dtype=torch.float16, device=qkv.device)
+    lib = load()
+    lib.seedb200_decode_attention_rope_lineage.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                           C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                           C.c_float, C.c_void_p]
+    with on(qkv.device):
+        check(lib.seedb200_decode_attention_rope_lineage(qkv.data_ptr(), None, slot.data_ptr(), B, H, D, past_len,
+                                                         max_seq, k_cache.data_ptr(), v_cache.data_ptr(),
+                                                         out.data_ptr(), scale, stream_ptr(qkv.device)),
+              "seedb200_decode_attention_rope_lineage")
+    return out
+
+
+def beam_select(logits: torch.Tensor, beam_scores: torch.Tensor, B: int, num_beams: int, first_step: bool = False,
+                step: int = 0, **params):
+    """Beam-search candidates of B sequences: logits [B*k, V] fp16 rows (or [B, V] with first_step: every beam reads
+    its sequence's row), beam_scores [B*k] fp32 -> (scores [B, 2k] fp32, flat indices [B, 2k] int64)."""
+    _need_cuda_f16(logits, "beam_select.logits")
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise RuntimeError("beam_select: logits must be 2-D with contiguous rows")
+    V = logits.shape[1]
+    k = int(num_beams)
+    if logits.shape[0] != (B if first_step else B * k):
+        raise RuntimeError(f"beam_select: logits have {logits.shape[0]} rows")
+    if beam_scores.dtype != torch.float32 or beam_scores.numel() != B * k or not beam_scores.is_contiguous():
+        raise RuntimeError("beam_select: beam_scores must be contiguous fp32 [B*k]")
+    ld = logits.stride(0)
+    seq_ld, beam_ld = (ld, 0) if first_step else (k * ld, ld)
+    bp = beam_params(k, **params)
+    sc = torch.empty((B, 2 * k), dtype=torch.float32, device=logits.device)
+    ix = torch.empty((B, 2 * k), dtype=torch.int32, device=logits.device)
+    with on(logits.device):
+        check(load().seedb200_beam_select(logits.data_ptr(), seq_ld, beam_ld, B, V, beam_scores.data_ptr(), C.byref(bp),
+                                          int(step), sc.data_ptr(), ix.data_ptr(), stream_ptr(logits.device)),
+              "seedb200_beam_select")
+    return sc, ix.long()
+
+
 def decode_attention_rope(qkv: torch.Tensor, positions: Optional[torch.Tensor], H: int, past_len: int,
                           k_cache: torch.Tensor, v_cache: torch.Tensor, scale: float) -> torch.Tensor:
     """RoPE + KV append + attention of one new token per sequence: qkv [B, 3*H*D] -> [B, H*D] (caches updated)."""
@@ -843,6 +942,33 @@ class Llama:
                                                  out.data_ptr(), C.byref(n), stream_ptr(self.device)),
                   "seedb200_llama_generate")
         return out[:, :n.value]
+
+    def beam_generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, num_beams: int, do_sample: bool = False,
+                      temperature: float = 1.0, top_p: float = 1.0, length_penalty: float = 1.0, early_stopping=False,
+                      seed: int = 0, offset: int = 0, eos_token_id: int = -1, pad_token_id: int = 0,
+                      use_graph: bool = True):
+        """prompt [B,S] int64 (device) -> (generated tokens [B, n] of the best hypothesis per sequence, fp32 scores [B]);
+        see seedb200_llama_beam_generate.  Needs B * num_beams <= max_batch (reserve_rows)."""
+        if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
+            raise RuntimeError(f"beam_generate: prompt_ids must be int64 on {self.device}")
+        prompt_ids = prompt_ids.contiguous()
+        B, S = prompt_ids.shape
+        out = torch.empty((B, max_new_tokens), dtype=torch.int64, device=self.device)
+        scores = torch.empty((B,), dtype=torch.float32, device=self.device)
+        bp = beam_params(num_beams, do_sample, temperature, top_p, length_penalty, early_stopping, seed, offset)
+        n = C.c_int(0)
+        with on(self.device):
+            check(load().seedb200_llama_beam_generate(self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(bp),
+                                                      int(eos_token_id), int(pad_token_id), int(bool(use_graph)),
+                                                      out.data_ptr(), C.byref(n), scores.data_ptr(),
+                                                      stream_ptr(self.device)), "seedb200_llama_beam_generate")
+        return out[:, :n.value], scores
+
+    def reserve_rows(self, rows: int) -> None:
+        """grow every max_batch-sized buffer to `rows` rows (drops the cache contents and the captured graphs)"""
+        with on(self.device):
+            check(load().seedb200_llama_reserve_rows(self._h, int(rows)), "seedb200_llama_reserve_rows")
+        self.max_batch = max(self.max_batch, int(rows))
 
     def int8_load_weight(self, name: str, w: torch.Tensor) -> None:
         """quantise the fp16 decoder linear `name` straight into the int8 handle's fused layout"""

@@ -287,11 +287,17 @@ class LlamaForCausalLM(nn.Module):
             return int(generator.initial_seed())
         return int(torch.initial_seed())
 
+    # GenerationConfig fields generate() honours, with the defaults used when neither it nor a kwarg sets them
+    _GEN_DEFAULTS = {"max_new_tokens": 20, "do_sample": False, "temperature": 1.0, "top_p": 1.0, "num_beams": 1,
+                     "length_penalty": 1.0, "early_stopping": False, "num_return_sequences": 1}
+
     @torch.no_grad()
-    def generate(self, input_ids=None, inputs=None, max_new_tokens: int = 20, do_sample: bool = False,
-                 temperature: float = 1.0, top_p: float = 1.0, num_beams: int = 1, eos_token_id=None,
-                 pad_token_id=None, attention_mask=None, generator: Optional[torch.Generator] = None,
-                 seed: Optional[int] = None, use_graph: bool = True, device_loop: Optional[bool] = None, **_):
+    def generate(self, input_ids=None, inputs=None, max_new_tokens: Optional[int] = None,
+                 do_sample: Optional[bool] = None, temperature: Optional[float] = None, top_p: Optional[float] = None,
+                 num_beams: Optional[int] = None, eos_token_id=None, pad_token_id=None, attention_mask=None,
+                 generator: Optional[torch.Generator] = None, seed: Optional[int] = None, use_graph: bool = True,
+                 device_loop: Optional[bool] = None, generation_config=None, length_penalty: Optional[float] = None,
+                 early_stopping=None, num_return_sequences: Optional[int] = None, **_):
         """Call pattern of scripts/seed_llama_inference_8B.py:33 (temperature=1.0, num_beams=1, max_new_tokens=512,
         top_p=0.5, do_sample=True); returns [B, S + n_new] like HF generate.
 
@@ -300,9 +306,36 @@ class LlamaForCausalLM(nn.Module):
         not past + arange) or more than one eos id, the loop runs from Python through
         `prepare_inputs_for_generation` exactly as HF drives the reference, still sampling with the device kernel.
         Sampled ids depend on the RNG (Philox keyed by `seed`, counter = draws made so far), not on torch's stream;
-        logits are the parity contract."""
-        if num_beams != 1:
-            raise NotImplementedError("beam search is not used by the SEED scripts")
+        logits are the parity contract.
+
+        `num_beams` > 1 runs transformers 4.30.2's beam search (`do_sample=False`) or beam sampling (`do_sample=True`)
+        on the device (seedb200_llama_beam_generate), with `length_penalty` and `early_stopping` (False / True /
+        "never"); only `num_return_sequences=1`, an unpadded batch and one eos id.  B * num_beams rows must fit the
+        handle: a model built with a smaller `max_batch` grows to it first, which drops the KV cache, so
+        `past_key_values` returned by earlier forward() calls are no longer valid.
+        `generation_config` (a transformers GenerationConfig) supplies these fields and its eos / pad ids, and
+        explicit keyword arguments override it, as in transformers."""
+        given = {"max_new_tokens": max_new_tokens, "do_sample": do_sample, "temperature": temperature, "top_p": top_p,
+                 "num_beams": num_beams, "length_penalty": length_penalty, "early_stopping": early_stopping,
+                 "num_return_sequences": num_return_sequences}
+        opts = dict(self._GEN_DEFAULTS)
+        if generation_config is not None:
+            for name in opts:
+                v = getattr(generation_config, name, None)
+                if v is not None:
+                    opts[name] = v
+            if eos_token_id is None:       # the config's own ids replace the model's, as in transformers
+                eos_token_id = generation_config.eos_token_id if generation_config.eos_token_id is not None else -1
+            if pad_token_id is None:
+                pad_token_id = generation_config.pad_token_id
+        opts.update({k: v for k, v in given.items() if v is not None})
+        max_new_tokens, do_sample, temperature, top_p = (int(opts["max_new_tokens"]), bool(opts["do_sample"]),
+                                                         float(opts["temperature"]), float(opts["top_p"]))
+        num_beams = int(opts["num_beams"])
+        if int(opts["num_return_sequences"]) != 1:
+            raise NotImplementedError("num_return_sequences > 1 is not supported")
+        if num_beams < 1:
+            raise ValueError(f"num_beams must be >= 1 (got {num_beams})")
         if input_ids is None:
             input_ids = inputs
         input_ids = input_ids.to(self._device, torch.int64)
@@ -318,6 +351,10 @@ class LlamaForCausalLM(nn.Module):
         rng_seed = self._next_seed(generator, seed)
         offset = self._draws
         padded = attention_mask is not None and not bool(attention_mask.to(torch.bool).all())
+        if num_beams > 1:
+            return self._beam_generate(input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p,
+                                       float(opts["length_penalty"]), opts["early_stopping"], eos_list, pad, padded,
+                                       rng_seed, offset, use_graph)
         if device_loop is None:
             device_loop = (not padded) and len(eos_list) <= 1 and B <= 4
         if device_loop:
@@ -351,6 +388,31 @@ class LlamaForCausalLM(nn.Module):
                 break
         self._draws += max_new_tokens
         return seq
+
+    def _beam_generate(self, input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p, length_penalty,
+                       early_stopping, eos_list, pad, padded, rng_seed, offset, use_graph):
+        if num_beams > 8:
+            raise ValueError(f"num_beams={num_beams}: at most 8 beams (the scorer runs one CTA per sequence)")
+        if padded:
+            raise NotImplementedError("a padding attention_mask is not supported with num_beams > 1")
+        if len(eos_list) > 1:
+            raise NotImplementedError("several eos_token_id values are not supported with num_beams > 1")
+        if early_stopping not in (False, True, "never"):
+            raise ValueError(f"early_stopping must be False, True or 'never' (got {early_stopping!r})")
+        if do_sample and temperature <= 0.0:
+            raise ValueError(f"temperature must be > 0 when sampling (got {temperature})")
+        B = input_ids.shape[0]
+        if B * num_beams > self.max_batch:
+            self._llm.reserve_rows(B * num_beams)       # the cache is reallocated: earlier past_key_values are void
+            self.max_batch = B * num_beams
+        new, _ = self._llm.beam_generate(input_ids, max_new_tokens, num_beams, do_sample=do_sample,
+                                         temperature=temperature if do_sample else 1.0, top_p=top_p,
+                                         length_penalty=length_penalty, early_stopping=early_stopping, seed=rng_seed,
+                                         offset=offset, eos_token_id=eos_list[0] if eos_list else -1,
+                                         pad_token_id=pad, use_graph=use_graph)
+        self._draws += max_new_tokens
+        self._cache_len, self._cache_batch = 0, 0
+        return torch.cat([input_ids, new], dim=1)
 
 
 def get_pretrained_llama_causal_model(pretrained_model_name_or_path=None, torch_dtype="fp16", **kwargs):
