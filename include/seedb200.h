@@ -467,6 +467,59 @@ int seedb200_decode_attention_rope_lineage(const void* qkv, const int64_t* posit
                                            int D, int past_len, int max_seq, void* k_cache, void* v_cache, void* out,
                                            float scale, void* stream);
 
+/* ---- unmerged LoRA adapters (PEFT lora.Linear, eval mode, fp16 module) -------------------------------------------
+ * For a decoder linear with weight W [N,K], lora_A [r,K], lora_B [N,r] (all fp16) and s = lora_alpha / r:
+ *   base = fp16(W x)                      the linear's kernel, unchanged
+ *   t    = fp16(A x)                      fp32 accumulation over K, [r]
+ *   u    = fp16(B t)                      fp32 accumulation over r
+ *   c    = fp16(float(u) * float32(s))
+ *   y    = fp16(base + c)
+ * and y takes the linear's epilogue step in place of fp16(acc): o_proj / down_proj fp16(residual + y); gate / up
+ * silu(y_gate) * y_up at the SiLU-gate epilogue's rounding points; q / k / v: y is what RoPE and the KV append read.
+ * (Dropout is the identity, fan_in_fan_out = False, bias = "none".)  c is added before the residual, as PEFT does.
+ * Merging adds fp16(fp16(B A) * s) to W (fp32 accumulation over r) and rounds to fp16.
+ * t of the <= 4-row (decode) shrink sums K in a tree over 256 threads; the prefill shrink sums K in ascending order.
+ * Rows n of a fused weight read t columns ((n / grp) % nsub) * r + [0, r): q|k|v grp = hidden, nsub 3; gate|up in
+ * 128-row blocks grp = 128, nsub 2; o / down grp = N, nsub 1.  A sub-block whose bit in `mask` is clear has no
+ * adapter there: y = base.  1 <= r <= 64.                                                                           */
+typedef struct seedb200_lora_operand {
+  const void* T;          /* [M, r * nsub] fp16: the shrink output t of every row                                  */
+  int64_t ldt;
+  const void* B;          /* [N, r] fp16 in the weight's fused row layout                                           */
+  int32_t r, grp, nsub;
+  uint32_t mask;
+  float scale;            /* s = lora_alpha / r                                                                     */
+  void* workspace;        /* [M, N] fp16 for the base product; may be NULL for mode 0 without residual (in place)   */
+} seedb200_lora_operand;
+typedef struct seedb200_gemm_lora_desc {
+  seedb200_gemm_desc gemm;          /* mode 0 (optionally with residual) or 1; no bias, act, LN fold or row remap */
+  seedb200_lora_operand lora;
+} seedb200_gemm_lora_desc;
+/* T [M, r_tot] (row stride ldt) = fp16(x . A^T), A [r_tot, K] fp16 dense, r_tot <= 192.  norm_w (M <= 4 only, x dense):
+ * x is RMS-normalised while staged with seedb200_gemv's arithmetic, so T matches what the fused-norm GEMV multiplies. */
+int seedb200_lora_shrink(const void* x, int64_t ldx, const void* norm_w, float eps, const void* A, int M, int K,
+                         int r_tot, void* T, int64_t ldt, void* stream);
+/* seedb200_gemm / seedb200_gemv with the LoRA branch.  GEMV (M <= 4): the expand runs in the GEMV's epilogue (no
+ * workspace).  GEMM: the base product (unchanged kernel, mode 0 into the workspace), then an expand kernel (residual
+ * add, or the SiLU gate with the GEMM epilogue's SiLU).                                                           */
+int seedb200_gemm_lora(const seedb200_gemm_lora_desc* d, void* stream);
+int seedb200_gemv_lora(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w,
+                       float eps, int M, int N, int K, int mode, const seedb200_lora_operand* lora, void* stream);
+/* Loads a PEFT LoRA adapter into an fp16 handle: "model.layers.N.<self_attn|mlp>.<proj>.lora_A.weight" [r,K] and
+ * ".lora_B.weight" [N,r], fp16.  Every layer must carry the same target set; one r and alpha for all (s = alpha / r).
+ * Every tensor is validated before anything is allocated, then copied into handle-owned fused layouts (the caller
+ * may free them).  A second load replaces the first.  Captured decode graphs are dropped.  int8 handles refuse.  */
+int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors, int n, int r, float alpha);
+/* Adds the loaded adapter into the fused weights (W = fp16(W + fp16(fp16(B A) * s))) and frees it; the model then
+ * runs exactly the base kernels.  o_proj and down_proj are borrowed, so the caller's tensors change in place, as
+ * PEFT's merge changes the base model's.  Fails when no adapter is loaded.                                        */
+int seedb200_llama_lora_merge(seedb200_llama* llm);
+/* Re-points borrowed fp16 tensors: "model.embed_tokens.weight" and "lm_head.weight" ([V', hidden]; a vocabulary
+ * change needs both, with one V'), "model.norm.weight", "model.layers.N.input_layernorm.weight",
+ * "model.layers.N.post_attention_layernorm.weight".  All are validated first.  A vocabulary change reallocates the
+ * max_batch-sized buffers (the KV cache contents are dropped); captured graphs are always dropped.                  */
+int seedb200_llama_replace_weights(seedb200_llama* llm, const seedb200_tensor* tensors, int n);
+
 /* Views of the KV cache of one layer: [max_batch, heads, max_seq, head_dim]
  * fp16; the first past_len+S rows per (batch, head) are valid.  Used to build
  * the past_key_values tuple the reference returns (llama_xformer.py:239).      */

@@ -34,6 +34,11 @@ struct LlamaLayerW {
   const int8_t *qkv8, *o8, *gu8, *down8;
   const float *qkv_s, *o_s, *gu_s, *down_s;
 };
+// LoRA adapter of one layer, per fused linear g (0 q|k|v, 1 o, 2 gate|up, 3 down): A_cat [nsub r, K], B [N, r]
+struct LoraLayer {
+  const __half* A[4];
+  const __half* B[4];
+};
 }  // namespace sb
 
 struct seedb200_llama {
@@ -75,6 +80,14 @@ struct seedb200_llama {
   float* sca;                     // [max_batch * max_seq]
   int* olist;                     // [max(hidden, ffn)] outlier columns
   int* ocount;
+  // ---- LoRA adapter (seedb200_llama_lora_load) ----
+  int lora_r;                     // 0: no adapter
+  float lora_s;                   // lora_alpha / r
+  unsigned lora_mask[4];          // per fused linear: the sub-blocks (q, k, v / gate, up) that carry an adapter
+  std::vector<sb::LoraLayer> lora;
+  void* lora_mem;                 // every layer's A and B
+  __half* lora_t;                 // [max_batch * max_seq, 3 * r] shrink output (row buffer)
+  __half* lora_base;              // [max_batch * max_seq, max(2 ffn, hidden)] base product (row buffer)
 };
 
 namespace sb {
@@ -193,6 +206,11 @@ static int llama_alloc_rows(seedb200_llama* m, cudaStream_t st) {
     SB_PROPAGATE(llama_alloc_row(m, &m->corr, T * (size_t)(2 * ffn > 3 * h ? 2 * ffn : 3 * h)));
     SB_PROPAGATE(llama_alloc_row(m, &m->ca, T * (size_t)(ffn > h ? ffn : h)));
     SB_PROPAGATE(llama_alloc_row(m, &m->sca, T));
+  }
+  m->lora_t = nullptr; m->lora_base = nullptr;
+  if (m->lora_r > 0) {
+    SB_PROPAGATE(llama_alloc_row(m, &m->lora_t, T * 3 * (size_t)m->lora_r));
+    SB_PROPAGATE(llama_alloc_row(m, &m->lora_base, T * (size_t)(2 * ffn > h ? 2 * ffn : h)));
   }
   SB_PROPAGATE(llama_alloc_row(m, &m->da_ws, (size_t)c.max_batch * c.heads * decode_attention_max_splits(c.max_seq) * (128 + 2)));
   SB_PROPAGATE(llama_alloc_row(m, &m->da_tickets, (size_t)c.max_batch * c.heads));   // zero now, left zero by every launch
@@ -339,6 +357,45 @@ static int lin(cudaStream_t st, int ctas, int M, int N, int K, const void* A, co
   return gemm(d, st);
 }
 
+// shape of fused linear g of a layer in the LoRA adapter: N x K, sub-blocks of grp rows cycling over nsub adapters
+struct LoraGeom { int N, K, grp, nsub; };
+static LoraGeom lora_geom(const seedb200_llama* m, int g) {
+  const int h = m->cfg.hidden, ffn = m->cfg.ffn;
+  if (g == 0) return {3 * h, h, h, 3};
+  if (g == 1) return {h, h, h, 1};
+  if (g == 2) return {2 * ffn, h, 128, 2};
+  return {h, ffn, h, 1};
+}
+// decoder linear i (kI8Lin order) -> (fused linear, sub-block)
+static const int kLoraGroup[7] = {0, 0, 0, 1, 2, 2, 3}, kLoraSub[7] = {0, 1, 2, 0, 0, 1, 0};
+
+static seedb200_lora_operand lora_operand(const seedb200_llama* m, int l, int g, void* workspace) {
+  const LoraGeom G = lora_geom(m, g);
+  seedb200_lora_operand lo;
+  memset(&lo, 0, sizeof(lo));
+  lo.T = m->lora_t; lo.ldt = (int64_t)G.nsub * m->lora_r; lo.B = m->lora[l].B[g];
+  lo.r = m->lora_r; lo.grp = G.grp; lo.nsub = G.nsub; lo.mask = m->lora_mask[g]; lo.scale = m->lora_s;
+  lo.workspace = workspace;
+  return lo;
+}
+
+// fp16 decoder linear g of layer l: lin(), plus the adapter's LoRA branch when one covers this linear
+static int lin_lora(seedb200_llama* m, cudaStream_t st, int l, int g, int M, int N, int K, const void* A,
+                    const void* W, void* out, int64_t ldo, const void* residual, int mode,
+                    const void* norm_w = nullptr, float eps = 0.0f) {
+  if (m->lora_r == 0 || m->lora_mask[g] == 0)
+    return lin(st, m->cfg.gemm_ctas, M, N, K, A, W, out, ldo, residual, mode, norm_w, eps);
+  const seedb200_lora_operand lo =
+      lora_operand(m, l, g, mode == 0 && residual == nullptr ? nullptr : static_cast<void*>(m->lora_base));
+  SB_PROPAGATE(lora_shrink(A, K, norm_w, eps, m->lora[l].A[g], M, K, (int)lo.ldt, m->lora_t, lo.ldt, st));
+  if (M <= 4) return gemv_lora(A, W, K, out, residual, norm_w, eps, M, N, K, mode, lo, st, ldo);
+  seedb200_gemm_desc d;
+  memset(&d, 0, sizeof(d));
+  d.M = M; d.N = N; d.K = K; d.A = A; d.lda = K; d.W = W; d.ldw = K;
+  d.out = out; d.ldo = ldo; d.residual = residual; d.ldr = ldo; d.mode = mode; d.ctas = m->cfg.gemm_ctas;
+  return gemm_lora(d, lo, st);
+}
+
 // int8 decoder linear: GEMV for M <= 4 (with the RMSNorm folded in when norm_w is given), otherwise activation
 // quantisation + int8 wgmma GEMM.  Outputs are dense rows of N (N/2 in mode 1) columns.
 static int lin8(seedb200_llama* m, cudaStream_t st, int M, int N, int K, const void* A, const int8_t* W,
@@ -381,10 +438,10 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
         SB_PROPAGATE(lin8(m, st, T, 3 * h, h, m->nb, L.qkv8, L.qkv_s, m->qkv, nullptr, 0));
       }
     } else if (fuse_norm) {
-      SB_PROPAGATE(lin(st, ct, T, 3 * h, h, m->x, L.qkv_w, m->qkv, 3 * h, nullptr, 0, L.in_ln, c.rms_eps));
+      SB_PROPAGATE(lin_lora(m, st, l, 0, T, 3 * h, h, m->x, L.qkv_w, m->qkv, 3 * h, nullptr, 0, L.in_ln, c.rms_eps));
     } else {
       SB_PROPAGATE(rmsnorm(m->x, h, L.in_ln, m->nb, h, T, h, c.rms_eps, st));
-      SB_PROPAGATE(lin(st, ct, T, 3 * h, h, m->nb, L.qkv_w, m->qkv, 3 * h, nullptr, 0));
+      SB_PROPAGATE(lin_lora(m, st, l, 0, T, 3 * h, h, m->nb, L.qkv_w, m->qkv, 3 * h, nullptr, 0));
     }
     // qkv rows are [q | k | v] per token, each [H, D]
     if (fused_attn) {
@@ -420,14 +477,14 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
       SB_PROPAGATE(lin8(m, st, T, h, ffn, m->gu, L.down8, L.down_s, m->x, m->x, 0));
       continue;
     }
-    SB_PROPAGATE(lin(st, ct, T, h, h, m->att, L.o_w, m->x, h, m->x, 0));
+    SB_PROPAGATE(lin_lora(m, st, l, 1, T, h, h, m->att, L.o_w, m->x, h, m->x, 0));
     if (fuse_norm) {
-      SB_PROPAGATE(lin(st, ct, T, 2 * ffn, h, m->x, L.gu_w, m->gu, ffn, nullptr, 1, L.post_ln, c.rms_eps));
+      SB_PROPAGATE(lin_lora(m, st, l, 2, T, 2 * ffn, h, m->x, L.gu_w, m->gu, ffn, nullptr, 1, L.post_ln, c.rms_eps));
     } else {
       SB_PROPAGATE(rmsnorm(m->x, h, L.post_ln, m->nb, h, T, h, c.rms_eps, st));
-      SB_PROPAGATE(lin(st, ct, T, 2 * ffn, h, m->nb, L.gu_w, m->gu, ffn, nullptr, 1));
+      SB_PROPAGATE(lin_lora(m, st, l, 2, T, 2 * ffn, h, m->nb, L.gu_w, m->gu, ffn, nullptr, 1));
     }
-    SB_PROPAGATE(lin(st, ct, T, h, ffn, m->gu, L.down_w, m->x, h, m->x, 0));
+    SB_PROPAGATE(lin_lora(m, st, l, 3, T, h, ffn, m->gu, L.down_w, m->x, h, m->x, 0));
   }
   SB_PROPAGATE(rmsnorm(m->x, h, m->norm_w, m->hn, h, T, h, c.rms_eps, st));
   m->last_T = T;
@@ -656,6 +713,10 @@ static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor*
   memset(&m->beam, 0, sizeof(m->beam));
   m->int8 = int8;
   m->threshold = threshold;
+  m->lora_r = 0;
+  m->lora_s = 0.0f;
+  memset(m->lora_mask, 0, sizeof(m->lora_mask));
+  m->lora_mem = nullptr;
   for (int i = 0; i < n_weights; ++i) m->w[std::string(weights[i].name)] = weights[i];
   int s = sb::llama_build(m);
   if (s != 0) {
@@ -707,6 +768,7 @@ void seedb200_llama_destroy(seedb200_llama* llm) {
   if (llm->gstate_host) cudaFreeHost(llm->gstate_host);
   if (llm->gstream) cudaStreamDestroy(llm->gstream);
   sb::llama_free_rows(llm);
+  if (llm->lora_mem) cudaFree(llm->lora_mem);
   for (void* p : llm->owned) cudaFree(p);
   delete llm;
 }
@@ -797,6 +859,216 @@ int seedb200_llama_reserve_rows(seedb200_llama* llm, int rows) {
   SB_CHECK_CUDA(cudaStreamSynchronize(0));
   llm->last_T = 0;
   llm->gen_cache_len = 0;
+  return 0;
+}
+
+}  // extern "C"
+
+namespace sb {
+
+static void lora_free(seedb200_llama* m) {
+  if (m->lora_mem) cudaFree(m->lora_mem);
+  m->lora_mem = nullptr;
+  m->lora.clear();
+  m->lora_r = 0;
+  memset(m->lora_mask, 0, sizeof(m->lora_mask));
+  for (__half** p : {&m->lora_t, &m->lora_base}) {
+    for (size_t i = 0; i < m->row_owned.size(); ++i)
+      if (m->row_owned[i] == *p) { m->row_owned.erase(m->row_owned.begin() + i); break; }
+    if (*p) cudaFree(*p);
+    *p = nullptr;
+  }
+}
+
+static int tensor_is(const seedb200_tensor& t, int64_t d0, int64_t d1) {
+  return t.dtype == SEEDB200_F16 && t.ndim == 2 && t.shape[0] == d0 && t.shape[1] == d1 && t.data != nullptr &&
+         (reinterpret_cast<uintptr_t>(t.data) & 15) == 0;
+}
+
+}  // namespace sb
+
+extern "C" {
+
+int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors, int n, int r, float alpha) {
+  SB_REQUIRE(llm && (tensors || n == 0), "llama_lora_load: null argument");
+  SB_REQUIRE(!llm->int8, "llama_lora_load: LoRA on an int8 (load_in_8bit) model is not supported");
+  SB_REQUIRE(r >= 1 && r <= sb::LORA_MAX_R, "llama_lora_load: r %d outside [1,%d]", r, sb::LORA_MAX_R);
+  SB_REQUIRE(alpha == alpha && alpha > -1e30f && alpha < 1e30f, "llama_lora_load: lora_alpha must be finite");
+  const int nl = (int)llm->layers.size();
+  std::vector<const seedb200_tensor*> found((size_t)nl * 7 * 2, nullptr);   // [layer][linear][A, B]
+  for (int t = 0; t < n; ++t) {
+    const seedb200_tensor& x = tensors[t];
+    SB_REQUIRE(x.name != nullptr, "llama_lora_load: tensor %d has no name", t);
+    int layer = -1, lin = -1, ab = -1;
+    for (int i = 0; i < 7 && lin < 0; ++i)
+      for (int k = 0; k < 2 && lin < 0; ++k) {
+        char tail[96];
+        snprintf(tail, sizeof(tail), ".%s.lora_%c.weight", sb::kI8Lin[i], k ? 'B' : 'A');
+        int l = -1, c = 0;
+        if (sscanf(x.name, "model.layers.%d%n", &l, &c) == 1 && strcmp(x.name + c, tail) == 0) { layer = l; lin = i; ab = k; }
+      }
+    SB_REQUIRE(lin >= 0, "llama_lora_load: '%s' is not a lora_A / lora_B of a decoder linear", x.name);
+    SB_REQUIRE(layer >= 0 && layer < nl, "llama_lora_load: '%s': the model has %d layers", x.name, nl);
+    const sb::LoraGeom G = sb::lora_geom(llm, sb::kLoraGroup[lin]);
+    const int64_t N = G.N / G.nsub, K = G.K;
+    const bool ok = ab == 0 ? sb::tensor_is(x, r, K) : sb::tensor_is(x, N, r);
+    SB_REQUIRE(ok, "llama_lora_load: '%s' must be fp16, 16-byte aligned, [%lld, %lld] (dtype %d, ndim %d)", x.name,
+               (long long)(ab == 0 ? r : N), (long long)(ab == 0 ? K : r), x.dtype, x.ndim);
+    const seedb200_tensor*& slot = found[((size_t)layer * 7 + lin) * 2 + ab];
+    SB_REQUIRE(slot == nullptr, "llama_lora_load: '%s' given twice", x.name);
+    slot = &x;
+  }
+  int targets = -1;   // bit i: linear i carries an adapter (the same in every layer)
+  for (int l = 0; l < nl; ++l) {
+    int here = 0;
+    for (int i = 0; i < 7; ++i) {
+      const bool a = found[((size_t)l * 7 + i) * 2] != nullptr, b = found[((size_t)l * 7 + i) * 2 + 1] != nullptr;
+      SB_REQUIRE(a == b, "llama_lora_load: model.layers.%d.%s has lora_%c without lora_%c", l, sb::kI8Lin[i],
+                 a ? 'A' : 'B', a ? 'B' : 'A');
+      if (a) here |= 1 << i;
+    }
+    SB_REQUIRE(targets < 0 || here == targets, "llama_lora_load: layer %d has a different set of target modules", l);
+    targets = here;
+  }
+  SB_REQUIRE(targets > 0, "llama_lora_load: no lora_A / lora_B tensors");
+  sb::DeviceGuard guard(llm->device);
+  SB_CHECK_CUDA(cudaDeviceSynchronize());
+  sb::llama_drop_graphs(llm);
+  sb::lora_free(llm);
+  size_t per_layer = 0;
+  for (int g = 0; g < 4; ++g) {
+    const sb::LoraGeom G = sb::lora_geom(llm, g);
+    per_layer += (size_t)G.nsub * r * G.K + (size_t)G.N * r;
+  }
+  SB_CHECK_CUDA(cudaMalloc(&llm->lora_mem, per_layer * nl * 2 + 256));
+  cudaStream_t st = 0;
+  SB_CHECK_CUDA(cudaMemsetAsync(llm->lora_mem, 0, per_layer * nl * 2, st));
+  llm->lora.resize(nl);
+  __half* p = static_cast<__half*>(llm->lora_mem);
+  for (int l = 0; l < nl; ++l)
+    for (int g = 0; g < 4; ++g) {
+      const sb::LoraGeom G = sb::lora_geom(llm, g);
+      llm->lora[l].A[g] = p; p += (size_t)G.nsub * r * G.K;
+      llm->lora[l].B[g] = p; p += (size_t)G.N * r;
+    }
+  for (int l = 0; l < nl; ++l)
+    for (int i = 0; i < 7; ++i) {
+      if (!((targets >> i) & 1)) continue;
+      const int g = sb::kLoraGroup[i], sub = sb::kLoraSub[i];
+      const sb::LoraGeom G = sb::lora_geom(llm, g);
+      const seedb200_tensor* A = found[((size_t)l * 7 + i) * 2];
+      const seedb200_tensor* B = found[((size_t)l * 7 + i) * 2 + 1];
+      __half* a_dst = const_cast<__half*>(llm->lora[l].A[g]) + (size_t)sub * r * G.K;
+      __half* b_dst = const_cast<__half*>(llm->lora[l].B[g]);
+      SB_CHECK_CUDA(cudaMemcpyAsync(a_dst, A->data, (size_t)r * G.K * 2, cudaMemcpyDeviceToDevice, st));
+      const int64_t rows = G.N / G.nsub;
+      if (g == 2) {   // gate|up: [ffn/128] blocks of [128 gate rows | 128 up rows]
+        const size_t blk = (size_t)128 * r * 2;
+        SB_CHECK_CUDA(cudaMemcpy2DAsync(reinterpret_cast<uint8_t*>(b_dst) + sub * blk, 2 * blk, B->data, blk, blk,
+                                        (size_t)rows / 128, cudaMemcpyDeviceToDevice, st));
+      } else {
+        SB_CHECK_CUDA(cudaMemcpyAsync(b_dst + (size_t)sub * rows * r, B->data, (size_t)rows * r * 2,
+                                      cudaMemcpyDeviceToDevice, st));
+      }
+      llm->lora_mask[g] |= 1u << sub;
+    }
+  llm->lora_r = r;
+  llm->lora_s = alpha / (float)r;
+  const size_t T = (size_t)llm->cfg.max_batch * llm->cfg.max_seq;
+  const size_t wide = (size_t)(2 * llm->cfg.ffn > llm->cfg.hidden ? 2 * llm->cfg.ffn : llm->cfg.hidden);
+  int s = sb::llama_alloc_row(llm, &llm->lora_t, T * 3 * (size_t)r);
+  if (s == 0) s = sb::llama_alloc_row(llm, &llm->lora_base, T * wide);
+  if (s != 0) {
+    sb::lora_free(llm);
+    return s;
+  }
+  SB_CHECK_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int seedb200_llama_lora_merge(seedb200_llama* llm) {
+  SB_REQUIRE(llm != nullptr, "llama_lora_merge: null handle");
+  SB_REQUIRE(llm->lora_r > 0, "llama_lora_merge: no adapter is loaded");
+  sb::DeviceGuard guard(llm->device);
+  cudaStream_t st = 0;
+  SB_CHECK_CUDA(cudaDeviceSynchronize());
+  for (int l = 0; l < (int)llm->layers.size(); ++l) {
+    const sb::LlamaLayerW& L = llm->layers[l];
+    const __half* W[4] = {L.qkv_w, L.o_w, L.gu_w, L.down_w};
+    for (int g = 0; g < 4; ++g) {
+      if (llm->lora_mask[g] == 0) continue;
+      const sb::LoraGeom G = sb::lora_geom(llm, g);
+      const seedb200_lora_operand lo = sb::lora_operand(llm, l, g, nullptr);
+      SB_PROPAGATE(sb::lora_merge(const_cast<__half*>(W[g]), llm->lora[l].A[g], lo, G.N, G.K, st));
+    }
+  }
+  SB_CHECK_CUDA(cudaStreamSynchronize(st));
+  sb::llama_drop_graphs(llm);
+  sb::lora_free(llm);
+  return 0;
+}
+
+int seedb200_llama_replace_weights(seedb200_llama* llm, const seedb200_tensor* tensors, int n) {
+  SB_REQUIRE(llm && (tensors || n == 0), "llama_replace_weights: null argument");
+  const int64_t h = llm->cfg.hidden;
+  const int nl = (int)llm->layers.size();
+  const seedb200_tensor *embed = nullptr, *head = nullptr, *norm = nullptr;
+  std::vector<const seedb200_tensor*> ln((size_t)nl * 2, nullptr);
+  for (int t = 0; t < n; ++t) {
+    const seedb200_tensor& x = tensors[t];
+    SB_REQUIRE(x.name != nullptr, "llama_replace_weights: tensor %d has no name", t);
+    int l = -1, c = 0;
+    const seedb200_tensor** slot = nullptr;
+    if (strcmp(x.name, "model.embed_tokens.weight") == 0) slot = &embed;
+    else if (strcmp(x.name, "lm_head.weight") == 0) slot = &head;
+    else if (strcmp(x.name, "model.norm.weight") == 0) slot = &norm;
+    else if (sscanf(x.name, "model.layers.%d%n", &l, &c) == 1 && l >= 0 && l < nl) {
+      if (strcmp(x.name + c, ".input_layernorm.weight") == 0) slot = &ln[(size_t)l * 2];
+      else if (strcmp(x.name + c, ".post_attention_layernorm.weight") == 0) slot = &ln[(size_t)l * 2 + 1];
+    }
+    SB_REQUIRE(slot != nullptr, "llama_replace_weights: '%s' is not embed_tokens, lm_head or a norm of this model",
+               x.name);
+    const bool vec = slot != &embed && slot != &head;
+    const bool ok = vec ? (x.dtype == SEEDB200_F16 && x.ndim == 1 && x.shape[0] == h && x.data &&
+                           (reinterpret_cast<uintptr_t>(x.data) & 15) == 0)
+                        : (x.ndim == 2 && sb::tensor_is(x, x.shape[0], h) && x.shape[0] >= 1 && x.shape[0] < (1LL << 31));
+    SB_REQUIRE(ok, "llama_replace_weights: '%s' must be fp16, 16-byte aligned, %s", x.name,
+               vec ? "[hidden]" : "[vocab, hidden]");
+    *slot = &x;
+  }
+  const int64_t V = llm->cfg.vocab;
+  const int64_t ve = embed ? embed->shape[0] : V, vh = head ? head->shape[0] : V;
+  SB_REQUIRE(ve == vh, "llama_replace_weights: embed_tokens has %lld rows and lm_head %lld: a vocabulary change "
+             "needs both, with the same size", (long long)ve, (long long)vh);
+  sb::DeviceGuard guard(llm->device);
+  SB_CHECK_CUDA(cudaDeviceSynchronize());
+  sb::llama_drop_graphs(llm);
+  if (ve != V) {
+    sb::llama_free_rows(llm);
+    const int old = llm->cfg.vocab;
+    llm->cfg.vocab = (int)ve;
+    llm->vpad = (llm->cfg.vocab + 7) / 8 * 8;
+    int s = sb::llama_alloc_rows(llm, 0);
+    if (s != 0) {                      // keep the handle usable with its old tensors
+      std::string err = seedb200_last_error();
+      sb::llama_free_rows(llm);
+      llm->cfg.vocab = old;
+      llm->vpad = (old + 7) / 8 * 8;
+      if (sb::llama_alloc_rows(llm, 0) != 0) llm->cfg.max_batch = 0;
+      sb::set_error("llama_replace_weights: %s", err.c_str());
+      return s;
+    }
+    SB_CHECK_CUDA(cudaStreamSynchronize(0));
+    llm->last_T = 0;
+    llm->gen_cache_len = 0;
+  }
+  if (embed) llm->embed = static_cast<const __half*>(embed->data);
+  if (head) llm->lm_head = static_cast<const __half*>(head->data);
+  if (norm) llm->norm_w = static_cast<const __half*>(norm->data);
+  for (int l = 0; l < nl; ++l) {
+    if (ln[(size_t)l * 2]) llm->layers[l].in_ln = static_cast<const __half*>(ln[(size_t)l * 2]->data);
+    if (ln[(size_t)l * 2 + 1]) llm->layers[l].post_ln = static_cast<const __half*>(ln[(size_t)l * 2 + 1]->data);
+  }
   return 0;
 }
 

@@ -73,12 +73,17 @@ __device__ __forceinline__ uint4 gemv_ldw(const uint4* p) {
   }
 }
 
-template <int M, int MODE, bool NORM, int U, bool NA>
+// LORA: the LoRA expand of include/seedb200.h in the epilogue (lo.T staged in shared memory; ksplit must be 1).  Lane
+// 2 m + i of the warp that owns a row pair finishes output row r_i of activation row m: y = fp16(fp16(acc) + c), then
+// the residual add or (mode 1, gate and up exchanged between the two lanes) the SiLU gate.  Without LORA the code is
+// the plain GEMV.
+template <int M, int MODE, bool NORM, int U, bool NA, bool LORA>
 __global__ void __launch_bounds__(256)
 gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long long ldw, __half* __restrict__ out,
             const __half* __restrict__ residual, const __half* __restrict__ norm_w, float eps, int N, int K,
-            int ksplit, int iters, long long ldo, int pf_lines) {
+            int ksplit, int iters, long long ldo, int pf_lines, seedb200_lora_operand lo) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
+  __shared__ float lts[LORA ? M * LORA_MAX_RTOT : 1];
   uint4* xs = reinterpret_cast<uint4*>(smem_raw);     // [M][K/8]
   __shared__ float red[8];
   __shared__ float part[2][8][M][2];                  // [iteration parity][warp][row m][row of the pair]
@@ -156,6 +161,11 @@ gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long lon
   } else {
     for (int i = threadIdx.x; i < M * nvec; i += nthr) xs[i] = reinterpret_cast<const uint4*>(x)[i];
   }
+  if constexpr (LORA) {
+    const int rt = lo.r * lo.nsub;
+    for (int i = threadIdx.x; i < M * rt; i += nthr)
+      lts[(i / rt) * LORA_MAX_RTOT + i % rt] = __half2float(static_cast<const __half*>(lo.T)[(long long)(i / rt) * lo.ldt + i % rt]);
+  }
   __syncthreads();
 
   for (int it = 0; it < iters; ++it) {                // trip count is uniform over the CTA (barriers inside)
@@ -212,7 +222,36 @@ gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long lon
         }
       }
     }
-    if (valid && slice == 0 && lane == 0) {
+    if constexpr (LORA) {
+      if (valid) {                                     // warp-uniform; every lane holds the warp sums (ksplit == 1)
+        const int m = lane < 2 * M ? lane >> 1 : 0, which = lane & 1;
+        float acc = 0.0f;
+#pragma unroll
+        for (int mm = 0; mm < M; ++mm)
+          if (mm == m) acc = which ? a1[mm] : a0[mm];
+        const long long rr = which ? r1 : r0;
+        __half y = __float2half_rn(acc);
+        const int sub = (int)((rr / lo.grp) % lo.nsub);
+        if ((lo.mask >> sub) & 1u) {
+          const __half* brow = static_cast<const __half*>(lo.B) + rr * lo.r;
+          const float* tr = lts + m * LORA_MAX_RTOT + sub * lo.r;
+          float ua = 0.0f;
+          for (int j = 0; j < lo.r; ++j) ua = fmaf(__half2float(brow[j]), tr[j], ua);
+          const __half c = __float2half_rn(__half2float(__float2half_rn(ua)) * lo.scale);
+          y = __float2half_rn(__half2float(y) + __half2float(c));
+        }
+        if (MODE == 1) {
+          const float yf = __half2float(y), other = __shfl_xor_sync(0xffffffffu, yf, 1);
+          if (lane < 2 * M && which == 0) {
+            const float sg = __half2float(__float2half_rn(yf / (1.0f + __expf(-yf))));
+            out[(long long)m * ldo + t] = __float2half_rn(sg * other);
+          }
+        } else if (lane < 2 * M && (which == 0 || r1 != r0)) {
+          if (residual != nullptr) y = __float2half_rn(__half2float(y) + __half2float(residual[(long long)m * n_out + rr]));
+          out[(long long)m * ldo + rr] = y;
+        }
+      }
+    } else if (valid && slice == 0 && lane == 0) {
 #pragma unroll
       for (int m = 0; m < M; ++m) {
         if (MODE == 1) {
@@ -235,8 +274,16 @@ gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long lon
 }
 
 int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w, float eps,
-         int M, int N, int K, int mode, cudaStream_t stream, int64_t ldo) {
+         int M, int N, int K, int mode, cudaStream_t stream, int64_t ldo, const seedb200_lora_operand* lora) {
   if (ldo <= 0) ldo = mode == 1 ? N / 2 : N;
+  seedb200_lora_operand lo;
+  memset(&lo, 0, sizeof(lo));
+  if (lora != nullptr) {
+    lo = *lora;
+    SB_REQUIRE(lo.T && lo.B && lo.r >= 1 && lo.r <= LORA_MAX_R && lo.nsub >= 1 && lo.nsub <= 3 && lo.grp >= 1 &&
+                   lo.ldt >= (int64_t)lo.r * lo.nsub,
+               "gemv: bad LoRA operand (r %d, nsub %d, grp %d, ldt %lld)", lo.r, lo.nsub, lo.grp, (long long)lo.ldt);
+  }
   SB_REQUIRE(M >= 1 && M <= GEMV_MAXM, "gemv: M=%d outside [1,%d]", M, GEMV_MAXM);
   SB_REQUIRE(K % 8 == 0 && ldw % 8 == 0, "gemv: K and ldw must be multiples of 8");
   SB_REQUIRE(mode == 0 || (mode == 1 && N % 256 == 0 && residual == nullptr), "gemv: bad mode/shape");
@@ -250,9 +297,9 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
   const __half* rp = static_cast<const __half*>(residual);
   const __half* np = static_cast<const __half*>(norm_w);
   __half* op = static_cast<__half*>(out);
-#define SB_GEMV_LAUNCH(M_, MD_, NM_, U_, NA_)                                                              \
+#define SB_GEMV_LAUNCH(M_, MD_, NM_, U_, NA_, LO_)                                                         \
   {                                                                                                        \
-    auto kern = gemv_kernel<M_, MD_, NM_, U_, NA_>;                                                        \
+    auto kern = gemv_kernel<M_, MD_, NM_, U_, NA_, LO_>;                                                        \
     const int threads = 256;                                                                               \
     static size_t attr_smem_dev[SB_MAX_DEVICES] = {};   /* per device: cudaFuncSetAttribute is */          \
     const int dev_ = cur_device();                                                                         \
@@ -275,7 +322,7 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
     /* K can be split over 2 or 4 warps per row pair (option gemv_ksplit); measured on the 13B decode step it  */ \
     /* loses (5.19 ms/token unsplit, 5.44 / 5.62 with 2 / 4 slices), so the default stays one warp per pair */ \
     int ksplit = 1;                                                                                        \
-    if (force_split == 1 || force_split == 2 || force_split == 4) ksplit = force_split;                    \
+    if (!(LO_) && (force_split == 1 || force_split == 2 || force_split == 4)) ksplit = force_split;        \
     const int tpi = (threads / 32) / ksplit;                                                               \
     int blocks = (n_tasks + tpi - 1) / tpi;                                                                \
     if (blocks > resident) blocks = resident;                                                              \
@@ -285,18 +332,22 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
                        ? (int)(((long long)get_option("gemv_prefetch_mb") << 20) / (2LL * n_tasks * 128)) : 0; \
     if (pf_lines > (K * 2 / ksplit) / 128) pf_lines = (K * 2 / ksplit) / 128;                               \
     SB_CHECK_CUDA(launch_chain(kern, dim3(blocks), dim3(threads), smem, stream, xp, wp, (long long)ldw, op, rp, np, eps, N, K, \
-                               ksplit, iters, (long long)ldo, pf_lines));                                  \
+                               ksplit, iters, (long long)ldo, pf_lines, lo));                              \
     SB_LAUNCH_CHECK();                                                                                     \
     return 0;                                                                                              \
   }
 #define SB_GEMV(M_, MD_)                                                                                   \
   if (M == M_ && mode == MD_) {                                                                            \
-    if (no_alloc) {                                                                                        \
-      if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, true)                                        \
-      SB_GEMV_LAUNCH(M_, MD_, false, 4, true)                                                              \
+    if (lora != nullptr) {                                                                                 \
+      if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, true, true)                                  \
+      SB_GEMV_LAUNCH(M_, MD_, false, 4, true, true)                                                        \
     }                                                                                                      \
-    if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, false)                                         \
-    SB_GEMV_LAUNCH(M_, MD_, false, 4, false)                                                               \
+    if (no_alloc) {                                                                                        \
+      if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, true, false)                                 \
+      SB_GEMV_LAUNCH(M_, MD_, false, 4, true, false)                                                       \
+    }                                                                                                      \
+    if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, false, false)                                  \
+    SB_GEMV_LAUNCH(M_, MD_, false, 4, false, false)                                                        \
   }
   SB_GEMV(1, 0) SB_GEMV(2, 0) SB_GEMV(3, 0) SB_GEMV(4, 0)
   SB_GEMV(1, 1) SB_GEMV(2, 1) SB_GEMV(3, 1) SB_GEMV(4, 1)

@@ -35,8 +35,10 @@ int get_rope_tables(int D, float base, int min_pos, const void** cos_t, const vo
                     cudaStream_t stream);
 // elementwise helpers (misc.cu)
 int add_rows(const void* a, const void* b, void* out, int rows, int cols, int b_rows, cudaStream_t stream);
+// ldo 0 = dense output rows; lora (optional): the LoRA expand fused into the epilogue (include/seedb200.h)
 int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w, float eps,
-         int M, int N, int K, int mode, cudaStream_t stream, int64_t ldo = 0);   // ldo 0 = dense output rows
+         int M, int N, int K, int mode, cudaStream_t stream, int64_t ldo = 0,
+         const seedb200_lora_operand* lora = nullptr);
 // dyn (optional, device): kv_len = dyn[0] + 1 at run time; the grid is then sized for max_seq keys
 int decode_attention(const void* q, const void* k_cache, const void* v_cache, void* out, int B, int H, int D,
                      int kv_len, int max_seq, float scale, void* workspace, cudaStream_t stream,
@@ -118,5 +120,16 @@ int int8_correction(const void* A16, int64_t lda, const void* W, int64_t ldw, co
                     const int* n_outliers, int M, int N, void* corr, cudaStream_t stream);
 int gemv_int8(const void* x, const void* norm_w, float eps, float threshold, const void* W, const void* SCB, void* out,
               const void* residual, int M, int N, int K, int mode, cudaStream_t stream);
+// LoRA (lora.cu)
+constexpr int LORA_MAX_R = 64, LORA_MAX_RTOT = 3 * LORA_MAX_R;
+int lora_shrink(const void* x, int64_t ldx, const void* norm_w, float eps, const void* A, int M, int K, int rtot,
+                void* T, int64_t ldt, cudaStream_t stream);
+// gemv_silu: the SiLU of the GEMV (base made by gemv) instead of the GEMM epilogue's
+int lora_expand(const void* base, int64_t ldb, const seedb200_lora_operand& lo, int M, int N, int mode,
+                bool gemv_silu, const void* residual, int64_t ldr, void* out, int64_t ldo, cudaStream_t stream);
+int gemm_lora(const seedb200_gemm_desc& d, const seedb200_lora_operand& lo, cudaStream_t stream);
+int gemv_lora(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w, float eps,
+              int M, int N, int K, int mode, const seedb200_lora_operand& lo, cudaStream_t stream, int64_t ldo = 0);
+int lora_merge(void* W, const void* A, const seedb200_lora_operand& lo, int N, int K, cudaStream_t stream);
 
 }  // namespace sb

@@ -39,6 +39,8 @@ EXPORTS = [
     "seedb200_llama_create_int8", "seedb200_llama_int8_load_weight",
     "seedb200_beam_select", "seedb200_llama_beam_generate", "seedb200_llama_reserve_rows",
     "seedb200_decode_attention_lineage", "seedb200_decode_attention_rope_lineage",
+    "seedb200_lora_shrink", "seedb200_gemm_lora", "seedb200_gemv_lora", "seedb200_llama_lora_load",
+    "seedb200_llama_lora_merge", "seedb200_llama_replace_weights",
 ]
 
 DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
@@ -74,6 +76,15 @@ class GemmInt8Desc(C.Structure):
                 ("out", C.c_void_p), ("ldo", C.c_int64),
                 ("residual", C.c_void_p), ("ldr", C.c_int64),
                 ("mode", C.c_int32), ("bn", C.c_int32), ("workspace", C.c_void_p)]
+
+
+class LoraOperand(C.Structure):
+    _fields_ = [("T", C.c_void_p), ("ldt", C.c_int64), ("B", C.c_void_p), ("r", C.c_int32), ("grp", C.c_int32),
+                ("nsub", C.c_int32), ("mask", C.c_uint32), ("scale", C.c_float), ("workspace", C.c_void_p)]
+
+
+class GemmLoraDesc(C.Structure):
+    _fields_ = [("gemm", GemmDesc), ("lora", LoraOperand)]
 
 
 class AttnDesc(C.Structure):
@@ -220,6 +231,15 @@ def load() -> C.CDLL:
     lib.seedb200_decode_attention_lineage.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                       C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                                       C.c_void_p, C.c_void_p]
+    lib.seedb200_lora_shrink.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_int,
+                                         C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.seedb200_gemm_lora.argtypes = [C.POINTER(GemmLoraDesc), C.c_void_p]
+    lib.seedb200_gemv_lora.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_float, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(LoraOperand),
+                                       C.c_void_p]
+    lib.seedb200_llama_lora_load.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int, C.c_int, C.c_float]
+    lib.seedb200_llama_lora_merge.argtypes = [C.c_void_p]
+    lib.seedb200_llama_replace_weights.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int]
     _lib = lib
     return lib
 
@@ -506,6 +526,82 @@ def gemv(x: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = No
     with on(x.device):
         check(load().seedb200_gemv(x.data_ptr(), w.data_ptr(), w.stride(0), out.data_ptr(), _p(residual), _p(norm_w),
                                    eps, M, N, K, mode, stream_ptr(x.device)), "seedb200_gemv")
+    return out
+
+
+def lora_shrink(x: torch.Tensor, a: torch.Tensor, norm_w: Optional[torch.Tensor] = None,
+                eps: float = 1e-6) -> torch.Tensor:
+    """LoRA shrink: x [M, K], a [r_tot, K] -> t = fp16(x . a^T) [M, r_tot].  norm_w (M <= 4): x is RMS-normalised on
+    the way in, as the fused-norm GEMV does."""
+    _need_cuda_f16(x, "lora_shrink.x"); _need_cuda_f16(a, "lora_shrink.a")
+    M, K = x.shape
+    rtot = a.shape[0]
+    a = a.contiguous()
+    if M <= 4:
+        x = x.contiguous()
+    t = torch.empty((M, rtot), dtype=torch.float16, device=x.device)
+    with on(x.device):
+        check(load().seedb200_lora_shrink(x.data_ptr(), x.stride(0), _p(norm_w), eps, a.data_ptr(), M, K, rtot,
+                                          t.data_ptr(), rtot, stream_ptr(x.device)), "seedb200_lora_shrink")
+    return t
+
+
+def lora_operand(t: torch.Tensor, b: torch.Tensor, r: int, grp: int, nsub: int, scale: float, mask: Optional[int] = None,
+                 workspace: Optional[torch.Tensor] = None) -> LoraOperand:
+    """t [M, r * nsub] (lora_shrink output), b [N, r] in the weight's fused row layout; output row n reads the t columns
+    ((n // grp) % nsub) * r + [0, r).  The caller keeps t, b and workspace alive across the call."""
+    for x, nm in ((t, "t"), (b, "b")):
+        _need_cuda_f16(x, f"lora.{nm}")
+    if not b.is_contiguous() or t.stride(1) != 1:
+        raise RuntimeError("lora: b must be contiguous and t must have contiguous columns")
+    return LoraOperand(t.data_ptr(), t.stride(0), b.data_ptr(), int(r), int(grp), int(nsub),
+                       (1 << nsub) - 1 if mask is None else int(mask), float(scale), _p(workspace))
+
+
+def gemm_lora(a: torch.Tensor, w: torch.Tensor, lora: LoraOperand, residual: Optional[torch.Tensor] = None,
+              out: Optional[torch.Tensor] = None, mode: int = 0, bn: int = 0,
+              workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gemm() (mode 0 with optional residual, or mode 1) with the LoRA branch of `lora` (see include/seedb200.h)."""
+    _need_cuda_f16(a, "gemm_lora.a"); _need_cuda_f16(w, "gemm_lora.w")
+    M, K = a.shape
+    N = w.shape[0]
+    if out is None:
+        out = torch.empty((M, N // 2 if mode == 1 else N), dtype=torch.float16, device=a.device)
+    if workspace is None and (mode == 1 or residual is not None):
+        workspace = torch.empty((M, N), dtype=torch.float16, device=a.device)
+    d = GemmLoraDesc()
+    g = d.gemm
+    g.M, g.N, g.K = M, N, K
+    g.A, g.lda = a.data_ptr(), a.stride(0)
+    g.W, g.ldw = w.data_ptr(), w.stride(0)
+    g.out, g.ldo = out.data_ptr(), out.stride(0)
+    g.residual = _p(residual)
+    g.ldr = residual.stride(0) if residual is not None else 0
+    g.mode, g.bn = mode, bn
+    d.lora = lora
+    d.lora.workspace = _p(workspace)
+    with on(a.device):
+        check(load().seedb200_gemm_lora(C.byref(d), stream_ptr(a.device)), "seedb200_gemm_lora")
+    return out
+
+
+def gemv_lora(x: torch.Tensor, w: torch.Tensor, lora: LoraOperand, residual: Optional[torch.Tensor] = None,
+              norm_w: Optional[torch.Tensor] = None, eps: float = 1e-6, mode: int = 0,
+              out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gemv() with the LoRA expand in its epilogue (`lora`); x [M <= 4, K] dense, out dense rows."""
+    _need_cuda_f16(x, "gemv_lora.x"); _need_cuda_f16(w, "gemv_lora.w")
+    M, K = x.shape
+    N = w.shape[0]
+    x = x.contiguous()
+    if out is None:
+        out = torch.empty((M, N // 2 if mode == 1 else N), dtype=torch.float16, device=x.device)
+    elif not out.is_contiguous():
+        raise RuntimeError("gemv_lora: out must be contiguous")
+    lo = LoraOperand.from_buffer_copy(lora)
+    with on(x.device):
+        check(load().seedb200_gemv_lora(x.data_ptr(), w.data_ptr(), w.stride(0), out.data_ptr(), _p(residual),
+                                        _p(norm_w), eps, M, N, K, mode, C.byref(lo), stream_ptr(x.device)),
+              "seedb200_gemv_lora")
     return out
 
 
@@ -978,6 +1074,30 @@ class Llama:
         with on(self.device):
             check(load().seedb200_llama_int8_load_weight(self._h, name.encode(), w.data_ptr(), w.stride(0),
                                                          stream_ptr(self.device)), "seedb200_llama_int8_load_weight")
+
+    def lora_load(self, tensors: Dict[str, torch.Tensor], r: int, alpha: float) -> None:
+        """copy a LoRA adapter ("model.layers.N.<...>.lora_A.weight" / ".lora_B.weight", fp16 on this device) into the
+        handle; replaces an earlier one.  The tensors may be dropped afterwards."""
+        arr, keep = _tensor_array(tensors)
+        with on(self.device):
+            check(load().seedb200_llama_lora_load(self._h, arr, len(tensors), int(r), float(alpha)),
+                  "seedb200_llama_lora_load")
+
+    def lora_merge(self) -> None:
+        """add the loaded adapter into the weights (o_proj / down_proj are borrowed: changed in place) and drop it"""
+        with on(self.device):
+            check(load().seedb200_llama_lora_merge(self._h), "seedb200_llama_lora_merge")
+
+    def replace_weights(self, tensors: Dict[str, torch.Tensor]) -> None:
+        """re-point embed_tokens / lm_head (together when the vocabulary changes) and the norms; the handle borrows
+        them, so they are kept referenced here"""
+        arr, keep = _tensor_array(tensors)
+        with on(self.device):
+            check(load().seedb200_llama_replace_weights(self._h, arr, len(tensors)), "seedb200_llama_replace_weights")
+        self._weights.update(tensors)
+        if "model.embed_tokens.weight" in tensors:
+            self.vocab = int(tensors["model.embed_tokens.weight"].shape[0])
+            self.vpad = (self.vocab + 7) // 8 * 8
 
     @property
     def used_graph(self) -> int:

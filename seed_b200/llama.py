@@ -9,6 +9,7 @@ Reference behaviours kept on purpose (SURVEY.md section 7 "quirks"):
     to choose between a causal and an unmasked xformers call (llama_xformer.py:240-256);
   * q_len == 1 attends to the whole cache without a mask; q_len > 1 is causal;
   * logits are returned for every position in fp16.
+`resize_token_embeddings` follows transformers 4.30.2; unmerged LoRA adapters are loaded through seed_b200/peft.py.
 `load_in_8bit=True` runs the seven linear layers of every decoder layer as LLM.int8() (transformers' bitsandbytes
 path, threshold `llm_int8_threshold`): int8 weights with per-row scales, per-call activation quantisation with fp16
 outlier columns; embed_tokens, lm_head and the norms stay fp16 (include/seedb200.h states the arithmetic).
@@ -180,6 +181,31 @@ class LlamaForCausalLM(nn.Module):
 
     def half(self):
         return self
+
+    def resize_token_embeddings(self, new_num_tokens: Optional[int] = None) -> nn.Embedding:
+        """transformers 4.30.2 PreTrainedModel.resize_token_embeddings (untied embeddings): embed_tokens and lm_head
+        get `new_num_tokens` rows; the first min(old, new) rows are kept and new rows are drawn from
+        N(0, config.initializer_range) (torch's default generator, fp32 draw rounded to fp16); config.vocab_size
+        follows.  Resizing drops the handle's KV cache (the vocabulary-sized buffers are reallocated)."""
+        old = self._llm._weights["model.embed_tokens.weight"]
+        if new_num_tokens is None or int(new_num_tokens) == old.shape[0]:
+            return nn.Embedding.from_pretrained(old, freeze=True)
+        n = int(new_num_tokens)
+        if n < 1:
+            raise ValueError(f"new_num_tokens must be >= 1 (got {n})")
+        std = float(getattr(self.config, "initializer_range", 0.02))
+        keep = min(n, old.shape[0])
+        new = {}
+        for name in ("model.embed_tokens.weight", "lm_head.weight"):
+            src = self._llm._weights[name]
+            t = torch.empty((n, src.shape[1]), dtype=torch.float32, device=self._device).normal_(0.0, std).half()
+            t[:keep] = src[:keep]
+            new[name] = t
+        self._llm.replace_weights(new)
+        self._weight_bytes += 2 * (n - old.shape[0]) * old.shape[1] * 2
+        self.config.vocab_size = n
+        self._cache_len, self._cache_batch = 0, 0
+        return nn.Embedding.from_pretrained(new["model.embed_tokens.weight"], freeze=True)
 
     def to(self, *args, **kwargs):
         tgt = kwargs.get("device", args[0] if args else None)
