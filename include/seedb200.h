@@ -379,6 +379,40 @@ int seedb200_encoder_detokenize(seedb200_encoder* enc, const int64_t* ids, int B
  * [B*32,768]; 2 = ln_vision output [B*257,1408].  Returns element count.       */
 int64_t seedb200_encoder_tap(seedb200_encoder* enc, int what, void* dst, int64_t max_elems, void* stream);
 
+/* ---- bitsandbytes 4-bit linear layers (transformers load_in_4bit=True: Linear4bit, blocksize 64) ----------------
+ * Follows bitsandbytes 0.39-0.41 quantize_4bit / dequantize_4bit / MatMul4Bit (restated in tests/quant4_ref.py; not
+ * checked against bitsandbytes itself).  W fp16 [N,K], K % 64 == 0, is cut row-major into blocks of 64 weights
+ * (blocks never cross rows):
+ *   absmax[n, b] = max |W| over the block (fp32, fmaxf: NaN dropped)
+ *   v            = fp32(w) * (1.0f / absmax)          (correctly rounded reciprocal; an all-zero block gives NaN)
+ *   NF4 code     = the number of the 15 fp32 midpoints (a + b) * 0.5f of adjacent NF4 values (table below) that v
+ *                  strictly exceeds: a value on a midpoint takes the lower code, NaN takes code 0
+ *   FP4 code     = 8 if v < 0 (-0 and NaN: no sign bit) | the 3-bit code of the bucket of |v| among the pivots
+ *                  0.00260417, 0.0859375, 0.20833333, 0.29166667, 0.4166667, 0.583333, 0.8333333 (strict >); the
+ *                  buckets in ascending order have the codes 0, 1, 6, 7, 4, 5, 2, 3
+ *   packed       = uint8 [N, K/2], two codes per byte, the even-index element in the HIGH nibble; absmax fp32 [N, K/64]
+ *   W'           = fp16_rn(value[code] * absmax) with the fp32 values
+ *                  FP4 codes 0..7: 0, 0.005208333333, 0.66666667, 1, 0.33333333, 0.5, 0.16666667, 0.25 (bit 8: negated)
+ *                  NF4 codes 0..15: -1, -0.6961928009986877, -0.5250730514526367, -0.39491748809814453,
+ *                  -0.28444138169288635, -0.18477343022823334, -0.09105003625154495, 0, 0.07958029955625534,
+ *                  0.16093020141124725, 0.24611230194568634, 0.33791524171829224, 0.44070982933044434,
+ *                  0.5626170039176941, 0.7229568362236023, 1
+ *   linear4(x)   = fp16(x . W'^T) with fp32 accumulation (MatMul4Bit's dequantise-then-linear form, exact for an fp32
+ *                  or fp16 compute dtype; bitsandbytes >= 0.40's one-token gemv_4bit kernel may sum and round
+ *                  differently and is not the contract).  seedb200_gemv_4bit equals seedb200_gemv on W' bit for bit.
+ * Double quantisation and a bf16 compute dtype are not supported.                                                   */
+enum seedb200_quant4 { SEEDB200_Q4_FP4 = 0, SEEDB200_Q4_NF4 = 1 };
+/* W fp16 [N,K] (row stride ldw elements, 0 = K; 16-byte aligned rows) -> packed uint8 [N, K/2], absmax fp32 [N, K/64] */
+int seedb200_quantize_4bit(const void* W, int64_t ldw, int N, int K, int quant_type, void* packed, void* absmax,
+                           void* stream);
+/* packed + absmax -> W' fp16 [N,K] (row stride ldo elements, 0 = K)                                                  */
+int seedb200_dequantize_4bit(const void* packed, const void* absmax, int N, int K, int quant_type, void* out,
+                             int64_t ldo, void* stream);
+/* out = epilogue(linear4(x)) for M <= 4 rows: seedb200_gemv's modes (0 with optional residual; 1 = SiLU gate over
+ * [128 gate | 128 up] row blocks) and norm_w (RMSNorm folded into the staging); packed / absmax dense.               */
+int seedb200_gemv_4bit(const void* x, const void* norm_w, float eps, const void* packed, const void* absmax,
+                       int quant_type, void* out, const void* residual, int M, int N, int K, int mode, void* stream);
+
 /* ------------------------------------------------------------------------- */
 /* LLaMA: models/llama_xformer.py LlamaForCausalLM                              */
 /* ------------------------------------------------------------------------- */
@@ -408,6 +442,18 @@ int seedb200_llama_create_int8(const seedb200_llama_config* cfg, const seedb200_
  * (which refuse otherwise).  Loading one fp16 tensor at a time keeps device memory at the int8 model plus that
  * tensor.  Enqueued on `stream`; W may be freed once the stream has passed this call.                          */
 int seedb200_llama_int8_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream);
+/* The same model with bitsandbytes 4-bit decoder linears (from_pretrained(load_in_4bit=True), see seedb200_quant4):
+ * `weights` holds the fp16 tensors other than the seven decoder linears (which are refused here); every linear is
+ * then quantised into the handle by seedb200_llama_4bit_load_weight, and forward / generate refuse to run until all
+ * are.  The handle also owns an fp16 scratch of 2 * ffn * hidden elements: more than 4 rows (prefill, or a decode
+ * step of more than 4 rows) dequantise each fused linear into it and run the fp16 GEMM, as MatMul4Bit does, so the
+ * logits equal an fp16 model holding W'.  Up to 4 rows use seedb200_gemv_4bit.  LoRA adapters are refused.          */
+int seedb200_llama_create_4bit(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
+                               int quant_type, seedb200_llama** out);
+/* Quantises the fp16 decoder linear `name` ([N,K], row stride ldw elements, 0 = K) into the 4-bit handle's fused
+ * layout (q|k|v concatenated, gate|up in 128-row blocks).  Enqueued on `stream`; W may be freed once the stream has
+ * passed this call.                                                                                                  */
+int seedb200_llama_4bit_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream);
 void seedb200_llama_destroy(seedb200_llama* llm);
 
 /* LlamaForCausalLM.forward (llama_xformer.py:661-743).  input_ids [B,S] int64
@@ -508,7 +554,8 @@ int seedb200_gemv_lora(const void* x, const void* W, int64_t ldw, void* out, con
 /* Loads a PEFT LoRA adapter into an fp16 handle: "model.layers.N.<self_attn|mlp>.<proj>.lora_A.weight" [r,K] and
  * ".lora_B.weight" [N,r], fp16.  Every layer must carry the same target set; one r and alpha for all (s = alpha / r).
  * Every tensor is validated before anything is allocated, then copied into handle-owned fused layouts (the caller
- * may free them).  A second load replaces the first.  Captured decode graphs are dropped.  int8 handles refuse.  */
+ * may free them).  A second load replaces the first.  Captured decode graphs are dropped.  int8 and 4-bit
+ * handles refuse.                                                                                                    */
 int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors, int n, int r, float alpha);
 /* Adds the loaded adapter into the fused weights (W = fp16(W + fp16(fp16(B A) * s))) and frees it; the model then
  * runs exactly the base kernels.  o_proj and down_proj are borrowed, so the caller's tensors change in place, as

@@ -16,6 +16,9 @@
 // fp32 SCB and are copied into handle-owned fused layouts (q|k|v concatenated, gate|up interleaved in 128-row blocks,
 // the scales the same way); lin8() sends them to the int8 GEMV (<= 4 rows) or quantises the activations and runs the
 // int8 wgmma GEMM.
+// 4-bit mode (seedb200_llama_create_4bit, bitsandbytes FP4 / NF4): the seven decoder linears are quantised one at a time
+// into handle-owned packed codes + absmax in the same fused layouts; lin4() sends them to the 4-bit GEMV (<= 4 rows) or
+// dequantises the fused weight into a handle-owned fp16 scratch and runs the unchanged fp16 path on it.
 #include <string.h>
 
 #include <map>
@@ -33,6 +36,9 @@ struct LlamaLayerW {
   // int8 mode: CB [N,K] and SCB [N] of the fused projections
   const int8_t *qkv8, *o8, *gu8, *down8;
   const float *qkv_s, *o_s, *gu_s, *down_s;
+  // 4-bit mode: packed codes [N, K/2] and absmax [N, K/64] of the fused projections
+  const uint8_t *qkv4, *o4, *gu4, *down4;
+  const float *qkv_a, *o_a, *gu_a, *down_a;
 };
 // LoRA adapter of one layer, per fused linear g (0 q|k|v, 1 o, 2 gate|up, 3 down): A_cat [nsub r, K], B [N, r]
 struct LoraLayer {
@@ -74,12 +80,16 @@ struct seedb200_llama {
   // ---- int8 mode ----
   int int8;
   float threshold;
-  std::vector<uint8_t> i8_loaded; // [layers][7]: the int8 linear holds its weights
+  std::vector<uint8_t> q_loaded;  // [layers][7]: the quantised (int8 or 4-bit) linear holds its weights
   __half* corr;                   // [max_batch * max_seq, 2 * ffn] outlier correction of the GEMM path
   int8_t* ca;                     // [max_batch * max_seq, max(hidden, ffn)] quantised activations (GEMM path)
   float* sca;                     // [max_batch * max_seq]
   int* olist;                     // [max(hidden, ffn)] outlier columns
   int* ocount;
+  // ---- 4-bit mode ----
+  int quant4;
+  int q4type;                     // SEEDB200_Q4_FP4 / SEEDB200_Q4_NF4
+  __half* q4_scratch;             // [max fused linear] fp16 W' of the linear the GEMM path runs
   // ---- LoRA adapter (seedb200_llama_lora_load) ----
   int lora_r;                     // 0: no adapter
   float lora_s;                   // lora_alpha / r
@@ -145,21 +155,37 @@ static int llama_find_i8(const seedb200_llama* m, const std::string& base, int64
 static const char* const kI8Lin[7] = {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj",
                                      "mlp.gate_proj", "mlp.up_proj", "mlp.down_proj"};
 
-// Where int8 linear i of layer L lives in the handle's fused buffers: CB rows r of [N,K] go to row
-// (r / grp) * gstride + r % grp + off of the fused weight, SCB entries likewise (gate|up: blocks of 128 rows).
-struct I8Slot { int8_t* cb; float* scb; int64_t N, K, grp, gstride, off; };
-static I8Slot i8_slot(const seedb200_llama* m, int layer, int i) {
+// "model.layers.<l>.<linear i>.weight" -> (l, i); false for any other name
+static bool linear_of(const char* name, int* layer, int* lin) {
+  for (int k = 0; k < 7; ++k) {
+    char tail[64];
+    snprintf(tail, sizeof(tail), ".%s.weight", kI8Lin[k]);
+    int l = -1, n = 0;
+    if (sscanf(name, "model.layers.%d%n", &l, &n) == 1 && strcmp(name + n, tail) == 0) { *layer = l; *lin = k; return true; }
+  }
+  return false;
+}
+
+// Where quantised linear i of layer L lives in the handle's fused buffers: rows r of [N,K] go to row
+// (r / grp) * gstride + r % grp + off of the fused weight (int8 CB / 4-bit packed codes), and the scales of row r
+// (int8 SCB / 4-bit absmax) likewise (gate|up: blocks of 128 rows).
+struct QSlot { uint8_t* w; float* s; int64_t N, K, grp, gstride, off; };
+static QSlot q_slot(const seedb200_llama* m, int layer, int i) {
   const int64_t h = m->cfg.hidden, ffn = m->cfg.ffn;
   const sb::LlamaLayerW& L = m->layers[layer];
-  I8Slot t;
+  const int g = i < 3 ? 0 : (i == 3 ? 1 : (i < 6 ? 2 : 3));      // fused linear: q|k|v, o, gate|up, down
+  const void* w8[4] = {L.qkv8, L.o8, L.gu8, L.down8};
+  const float* s8[4] = {L.qkv_s, L.o_s, L.gu_s, L.down_s};
+  const void* w4[4] = {L.qkv4, L.o4, L.gu4, L.down4};
+  const float* s4[4] = {L.qkv_a, L.o_a, L.gu_a, L.down_a};
+  QSlot t;
+  t.w = static_cast<uint8_t*>(const_cast<void*>(m->quant4 ? w4[g] : w8[g]));
+  t.s = const_cast<float*>(m->quant4 ? s4[g] : s8[g]);
   t.K = i == 6 ? ffn : h;
   t.N = i == 6 ? h : (i >= 4 ? ffn : h);
   t.grp = t.N; t.gstride = 0; t.off = 0;
-  if (i < 3) { t.cb = const_cast<int8_t*>(L.qkv8); t.scb = const_cast<float*>(L.qkv_s); t.off = i * h; }
-  else if (i == 3) { t.cb = const_cast<int8_t*>(L.o8); t.scb = const_cast<float*>(L.o_s); }
-  else if (i < 6) { t.cb = const_cast<int8_t*>(L.gu8); t.scb = const_cast<float*>(L.gu_s); t.grp = 128; t.gstride = 256;
-                    t.off = i == 5 ? 128 : 0; }
-  else { t.cb = const_cast<int8_t*>(L.down8); t.scb = const_cast<float*>(L.down_s); }
+  if (i < 3) t.off = i * h;
+  else if (i == 4 || i == 5) { t.grp = 128; t.gstride = 256; t.off = i == 5 ? 128 : 0; }
   return t;
 }
 
@@ -264,8 +290,15 @@ static int llama_build(seedb200_llama* m) {
         snprintf(nm, sizeof(nm), "model.layers.%d.%s", l, kI8Lin[i]);
         SB_PROPAGATE(llama_find_i8(m, nm, N, K, &cb, &scb));
       }
-    m->i8_loaded.assign((size_t)c.layers * 7, 0);
   }
+  if (m->quant4) {  // no pre-packed 4-bit names exist: every decoder linear comes through seedb200_llama_4bit_load_weight
+    for (const auto& kv : m->w) {
+      int l, i;
+      SB_REQUIRE(!linear_of(kv.first.c_str(), &l, &i), "llama_create_4bit: '%s' is a decoder linear: load it with "
+                 "seedb200_llama_4bit_load_weight", kv.first.c_str());
+    }
+  }
+  if (m->int8 || m->quant4) m->q_loaded.assign((size_t)c.layers * 7, 0);
   m->layers.resize(c.layers);
   for (int l = 0; l < c.layers; ++l) {
     LlamaLayerW& L = m->layers[l];
@@ -276,6 +309,24 @@ static int llama_build(seedb200_llama* m) {
     L.qkv_w = L.o_w = L.gu_w = L.down_w = nullptr;
     L.qkv8 = L.o8 = L.gu8 = L.down8 = nullptr;
     L.qkv_s = L.o_s = L.gu_s = L.down_s = nullptr;
+    L.qkv4 = L.o4 = L.gu4 = L.down4 = nullptr;
+    L.qkv_a = L.o_a = L.gu_a = L.down_a = nullptr;
+    if (m->quant4) {
+      // handle-owned fused buffers as in int8 mode: packed codes [N, K/2] and absmax [N, K/64]
+      uint8_t *q4, *o4, *g4, *d4;
+      float *qa, *oa, *ga, *da;
+      SB_PROPAGATE(llama_alloc(m, &q4, (size_t)3 * h * h / 2));
+      SB_PROPAGATE(llama_alloc(m, &qa, (size_t)3 * h * h / 64));
+      SB_PROPAGATE(llama_alloc(m, &o4, (size_t)h * h / 2));
+      SB_PROPAGATE(llama_alloc(m, &oa, (size_t)h * h / 64));
+      SB_PROPAGATE(llama_alloc(m, &g4, (size_t)2 * ffn * h / 2));
+      SB_PROPAGATE(llama_alloc(m, &ga, (size_t)2 * ffn * h / 64));
+      SB_PROPAGATE(llama_alloc(m, &d4, (size_t)h * ffn / 2));
+      SB_PROPAGATE(llama_alloc(m, &da, (size_t)h * ffn / 64));
+      L.qkv4 = q4; L.o4 = o4; L.gu4 = g4; L.down4 = d4;
+      L.qkv_a = qa; L.o_a = oa; L.gu_a = ga; L.down_a = da;
+      continue;
+    }
     if (m->int8) {
       // handle-owned fused buffers: q|k|v, o, [ffn/128] blocks of [128 gate | 128 up], down; scales alike
       int8_t *q8, *o8, *g8, *d8;
@@ -291,17 +342,17 @@ static int llama_build(seedb200_llama* m) {
       L.qkv8 = q8; L.o8 = o8; L.gu8 = g8; L.down8 = d8;
       L.qkv_s = qs; L.o_s = os; L.gu_s = gs; L.down_s = ds;
       for (int i = 0; i < 7; ++i) {
-        const I8Slot t = i8_slot(m, l, i);
+        const QSlot t = q_slot(m, l, i);
         const int8_t* cb;
         const float* scb;
         SB_PROPAGATE(llama_find_i8(m, key(kI8Lin[i]), t.N, t.K, &cb, &scb));
         if (cb == nullptr) continue;     // quantised into its slot later
         const int64_t blocks = t.N / t.grp, dst_rows = t.grp == t.N ? t.N : t.gstride;
-        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.cb + t.off * t.K, (size_t)(dst_rows * t.K), cb, (size_t)(t.grp * t.K),
+        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.w + t.off * t.K, (size_t)(dst_rows * t.K), cb, (size_t)(t.grp * t.K),
                                         (size_t)(t.grp * t.K), (size_t)blocks, cudaMemcpyDeviceToDevice, st));
-        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.scb + t.off, (size_t)(dst_rows * 4), scb, (size_t)(t.grp * 4),
+        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.s + t.off, (size_t)(dst_rows * 4), scb, (size_t)(t.grp * 4),
                                         (size_t)(t.grp * 4), (size_t)blocks, cudaMemcpyDeviceToDevice, st));
-        m->i8_loaded[(size_t)l * 7 + i] = 1;
+        m->q_loaded[(size_t)l * 7 + i] = 1;
       }
       continue;
     }
@@ -327,6 +378,11 @@ static int llama_build(seedb200_llama* m) {
     L.gu_w = fg;
   }
   SB_PROPAGATE(get_rope_tables(c.head_dim, c.rope_base, c.max_seq, &m->cos_t, &m->sin_t, &m->max_pos, st));
+  m->q4_scratch = nullptr;
+  if (m->quant4) {   // allocated here so that peak memory does not depend on the first prefill
+    const size_t qkv = (size_t)3 * h * h, gu = (size_t)2 * ffn * h;
+    SB_PROPAGATE(llama_alloc(m, &m->q4_scratch, qkv > gu ? qkv : gu));
+  }
   m->olist = nullptr; m->ocount = nullptr;
   if (m->int8) {
     SB_PROPAGATE(llama_alloc(m, &m->olist, (size_t)(ffn > h ? ffn : h)));
@@ -379,10 +435,24 @@ static seedb200_lora_operand lora_operand(const seedb200_llama* m, int l, int g,
   return lo;
 }
 
-// fp16 decoder linear g of layer l: lin(), plus the adapter's LoRA branch when one covers this linear
+// fp16 decoder linear g of layer l: lin(), plus the adapter's LoRA branch when one covers this linear (lin4() on a
+// 4-bit handle)
+// 4-bit decoder linear g of layer l: the 4-bit GEMV for M <= 4 (norm folded as lin() folds it), otherwise the fused
+// weight is dequantised into the scratch and lin() runs on it (MatMul4Bit's dequantise-then-linear).
+static int lin4(seedb200_llama* m, cudaStream_t st, int l, int g, int M, int N, int K, const void* A, void* out,
+                int64_t ldo, const void* residual, int mode, const void* norm_w, float eps) {
+  const LlamaLayerW& L = m->layers[l];
+  const uint8_t* P[4] = {L.qkv4, L.o4, L.gu4, L.down4};
+  const float* S[4] = {L.qkv_a, L.o_a, L.gu_a, L.down_a};
+  if (M <= 4) return gemv_4bit(A, norm_w, eps, P[g], S[g], m->q4type, out, residual, M, N, K, mode, st);
+  SB_PROPAGATE(dequantize_4bit(P[g], S[g], N, K, m->q4type, m->q4_scratch, K, st));
+  return lin(st, m->cfg.gemm_ctas, M, N, K, A, m->q4_scratch, out, ldo, residual, mode);
+}
+
 static int lin_lora(seedb200_llama* m, cudaStream_t st, int l, int g, int M, int N, int K, const void* A,
                     const void* W, void* out, int64_t ldo, const void* residual, int mode,
                     const void* norm_w = nullptr, float eps = 0.0f) {
+  if (m->quant4) return lin4(m, st, l, g, M, N, K, A, out, ldo, residual, mode, norm_w, eps);
   if (m->lora_r == 0 || m->lora_mask[g] == 0)
     return lin(st, m->cfg.gemm_ctas, M, N, K, A, W, out, ldo, residual, mode, norm_w, eps);
   const seedb200_lora_operand lo =
@@ -674,12 +744,16 @@ static void llama_drop_graphs(seedb200_llama* m) {
   m->graphs.clear();
 }
 
-// every int8 linear must hold its weights before the model runs
-static int llama_int8_ready(const seedb200_llama* m) {
-  for (size_t i = 0; i < m->i8_loaded.size(); ++i)
-    if (!m->i8_loaded[i]) {
-      set_error("llama: int8 weight 'model.layers.%d.%s.weight' was neither given to create_int8 nor loaded",
-                (int)(i / 7), kI8Lin[i % 7]);
+// every quantised (int8 or 4-bit) linear must hold its weights before the model runs
+static int llama_linears_ready(const seedb200_llama* m) {
+  for (size_t i = 0; i < m->q_loaded.size(); ++i)
+    if (!m->q_loaded[i]) {
+      if (m->quant4)
+        set_error("llama: 4-bit weight 'model.layers.%d.%s.weight' has not been loaded (seedb200_llama_4bit_load_weight)",
+                  (int)(i / 7), kI8Lin[i % 7]);
+      else
+        set_error("llama: int8 weight 'model.layers.%d.%s.weight' was neither given to create_int8 nor loaded",
+                  (int)(i / 7), kI8Lin[i % 7]);
       return SEEDB200_ERR_INVALID;
     }
   return 0;
@@ -689,8 +763,9 @@ static int llama_int8_ready(const seedb200_llama* m) {
 
 extern "C" {
 
+// q4type: -1 = no 4-bit linears
 static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights, int int8,
-                        float threshold, seedb200_llama** out) {
+                        float threshold, int q4type, seedb200_llama** out) {
   if (!cfg || !weights || !out) {
     sb::set_error("llama_create: null argument");
     return SEEDB200_ERR_INVALID;
@@ -713,6 +788,8 @@ static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor*
   memset(&m->beam, 0, sizeof(m->beam));
   m->int8 = int8;
   m->threshold = threshold;
+  m->quant4 = q4type >= 0;
+  m->q4type = q4type;
   m->lora_r = 0;
   m->lora_s = 0.0f;
   memset(m->lora_mask, 0, sizeof(m->lora_mask));
@@ -730,35 +807,55 @@ static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor*
 
 int seedb200_llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
                           seedb200_llama** out) {
-  return llama_create(cfg, weights, n_weights, 0, 0.0f, out);
+  return llama_create(cfg, weights, n_weights, 0, 0.0f, -1, out);
 }
 
 int seedb200_llama_create_int8(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
                                float threshold, seedb200_llama** out) {
   SB_REQUIRE(threshold > 0.0f, "llama_create_int8: threshold must be > 0 (got %g)", (double)threshold);
   SB_REQUIRE(cfg == nullptr || cfg->hidden % 16 == 0, "llama_create_int8: hidden must be a multiple of 16");
-  return llama_create(cfg, weights, n_weights, 1, threshold, out);
+  return llama_create(cfg, weights, n_weights, 1, threshold, -1, out);
+}
+
+int seedb200_llama_create_4bit(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
+                               int quant_type, seedb200_llama** out) {
+  SB_REQUIRE(quant_type == SEEDB200_Q4_FP4 || quant_type == SEEDB200_Q4_NF4,
+             "llama_create_4bit: quant_type %d is neither FP4 (0) nor NF4 (1)", quant_type);
+  SB_REQUIRE(cfg == nullptr || (cfg->hidden % 64 == 0 && cfg->ffn % 64 == 0),
+             "llama_create_4bit: hidden %d and ffn %d must be multiples of the 4-bit blocksize 64",
+             cfg ? cfg->hidden : 0, cfg ? cfg->ffn : 0);
+  return llama_create(cfg, weights, n_weights, 0, 0.0f, quant_type, out);
 }
 
 int seedb200_llama_int8_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream) {
   SB_REQUIRE(llm && name && W, "llama_int8_load_weight: null argument");
   SB_REQUIRE(llm->int8, "llama_int8_load_weight: the handle was not made by seedb200_llama_create_int8");
   int layer = -1, i = -1;
-  for (int k = 0; k < 7 && i < 0; ++k) {
-    char tail[64];
-    snprintf(tail, sizeof(tail), ".%s.weight", sb::kI8Lin[k]);
-    int l = -1, n = 0;
-    if (sscanf(name, "model.layers.%d%n", &l, &n) == 1 && strcmp(name + n, tail) == 0) { layer = l; i = k; }
-  }
-  SB_REQUIRE(i >= 0 && layer >= 0 && layer < (int)llm->layers.size(),
+  SB_REQUIRE(sb::linear_of(name, &layer, &i) && layer >= 0 && layer < (int)llm->layers.size(),
              "llama_int8_load_weight: '%s' is not a decoder linear of this model", name);
-  const sb::I8Slot t = sb::i8_slot(llm, layer, i);
+  const sb::QSlot t = sb::q_slot(llm, layer, i);
   if (ldw == 0) ldw = t.K;
   SB_REQUIRE(ldw >= t.K, "llama_int8_load_weight: ldw %lld below K %lld", (long long)ldw, (long long)t.K);
   sb::DeviceGuard guard(llm->device);
-  SB_PROPAGATE(sb::int8_quantize_weight_rows(W, ldw, (int)t.N, (int)t.K, t.cb, t.scb, (int)t.grp, (int)t.gstride,
+  SB_PROPAGATE(sb::int8_quantize_weight_rows(W, ldw, (int)t.N, (int)t.K, t.w, t.s, (int)t.grp, (int)t.gstride,
                                              (int)t.off, static_cast<cudaStream_t>(stream)));
-  llm->i8_loaded[(size_t)layer * 7 + i] = 1;
+  llm->q_loaded[(size_t)layer * 7 + i] = 1;
+  return 0;
+}
+
+int seedb200_llama_4bit_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream) {
+  SB_REQUIRE(llm && name && W, "llama_4bit_load_weight: null argument");
+  SB_REQUIRE(llm->quant4, "llama_4bit_load_weight: the handle was not made by seedb200_llama_create_4bit");
+  int layer = -1, i = -1;
+  SB_REQUIRE(sb::linear_of(name, &layer, &i) && layer >= 0 && layer < (int)llm->layers.size(),
+             "llama_4bit_load_weight: '%s' is not a decoder linear of this model", name);
+  const sb::QSlot t = sb::q_slot(llm, layer, i);
+  if (ldw == 0) ldw = t.K;
+  SB_REQUIRE(ldw >= t.K, "llama_4bit_load_weight: ldw %lld below K %lld", (long long)ldw, (long long)t.K);
+  sb::DeviceGuard guard(llm->device);
+  SB_PROPAGATE(sb::quantize_4bit_rows(W, ldw, (int)t.N, (int)t.K, llm->q4type, t.w, t.s, (int)t.grp, (int)t.gstride,
+                                      (int)t.off, static_cast<cudaStream_t>(stream)));
+  llm->q_loaded[(size_t)layer * 7 + i] = 1;
   return 0;
 }
 
@@ -785,7 +882,7 @@ int seedb200_llama_forward_ld(seedb200_llama* llm, const int64_t* input_ids, con
   SB_REQUIRE(logits_mode == 0 || logits_mode == 1, "llama_forward: logits_mode must be 0 or 1");
   SB_REQUIRE(logits_out == nullptr || logits_ld >= llm->cfg.vocab, "llama_forward: logits_ld %lld < vocab %d",
              (long long)logits_ld, llm->cfg.vocab);
-  SB_PROPAGATE(sb::llama_int8_ready(llm));
+  SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_forward(llm, input_ids, inputs_embeds, position_ids, B, S, past_len, logits_mode, logits_out,
                            logits_ld, static_cast<cudaStream_t>(stream));
@@ -807,7 +904,7 @@ int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int 
   SB_REQUIRE(S >= 1 && max_new_tokens >= 1 && S + max_new_tokens <= llm->cfg.max_seq,
              "llama_generate: prompt %d + %d new tokens exceeds max_seq %d", S, max_new_tokens, llm->cfg.max_seq);
   SB_REQUIRE(!sp->do_sample || (sp->temperature > 0.0f && sp->top_p > 0.0f), "llama_generate: temperature and top_p must be > 0");
-  SB_PROPAGATE(sb::llama_int8_ready(llm));
+  SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_generate(llm, prompt_ids, B, S, max_new_tokens, sp, eos_id, pad_id, use_graph, tokens_out,
                             n_generated_host, static_cast<cudaStream_t>(stream));
@@ -831,7 +928,7 @@ int seedb200_llama_beam_generate(seedb200_llama* llm, const int64_t* prompt_ids,
   SB_REQUIRE(bp->early_stopping >= 0 && bp->early_stopping <= 2, "llama_beam_generate: early_stopping %d not in {0,1,2}",
              bp->early_stopping);
   SB_REQUIRE(eos_id < llm->cfg.vocab, "llama_beam_generate: eos_id %lld outside the vocabulary", (long long)eos_id);
-  SB_PROPAGATE(sb::llama_int8_ready(llm));
+  SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_beam_generate(llm, prompt_ids, B, S, max_new_tokens, bp, eos_id, pad_id, use_graph, tokens_out,
                                  n_out_host, best_scores_out, static_cast<cudaStream_t>(stream));
@@ -892,6 +989,7 @@ extern "C" {
 int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors, int n, int r, float alpha) {
   SB_REQUIRE(llm && (tensors || n == 0), "llama_lora_load: null argument");
   SB_REQUIRE(!llm->int8, "llama_lora_load: LoRA on an int8 (load_in_8bit) model is not supported");
+  SB_REQUIRE(!llm->quant4, "llama_lora_load: LoRA on a 4-bit (load_in_4bit) model is not supported");
   SB_REQUIRE(r >= 1 && r <= sb::LORA_MAX_R, "llama_lora_load: r %d outside [1,%d]", r, sb::LORA_MAX_R);
   SB_REQUIRE(alpha == alpha && alpha > -1e30f && alpha < 1e30f, "llama_lora_load: lora_alpha must be finite");
   const int nl = (int)llm->layers.size();

@@ -4,8 +4,11 @@
 //                     LlamaDecoderLayer (llama_xformer.py:186,223-225,258) and lm_head (:718)
 //   decode_attention  one query token against the KV cache (llama_xformer.py:240-256 with attn_bias=None),
 //                     split over the key axis so that B*H*splits CTAs cover the SMs
+#include <type_traits>
+
 #include "common.cuh"
 #include "ops.h"
+#include "quant4.cuh"
 
 namespace sb {
 
@@ -72,16 +75,55 @@ __device__ __forceinline__ uint4 gemv_ldw(const uint4* p) {
     return v;
   }
 }
+template <bool NA>
+__device__ __forceinline__ uint32_t gemv_ldw(const uint32_t* p) {
+  if constexpr (!NA) {
+    return __ldg(p);
+  } else {
+    uint32_t v;
+    asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(v) : "l"(p));
+    return v;
+  }
+}
+
+// WF: the weight format.  0 = fp16 W [N, ldw halves], one 16-byte vector per group of 8 weights.  1 + quant type
+// (SEEDB200_Q4_FP4 / SEEDB200_Q4_NF4) = bitsandbytes 4-bit codes [N, ldw bytes] with absmax [N, K/64]: 4 packed
+// bytes per group, dequantised in registers to the halves the fp16 GEMV would read from dequantize_4bit(W) and then
+// summed exactly like them (same lane -> group mapping, same dot8 order), so the output is bit-identical.
+template <int WF>
+using GemvVec = std::conditional_t<WF == 0, uint4, uint32_t>;
+template <int WF>
+constexpr int kGemvVecsPerLine = WF == 0 ? 8 : 32;     // vectors per 128-byte line
+
+template <int WF>
+__device__ __forceinline__ const GemvVec<WF>* gemv_row(const __half* W, long long r, long long ldw) {
+  if constexpr (WF == 0) return reinterpret_cast<const uint4*>(W + r * ldw);
+  else return reinterpret_cast<const uint32_t*>(reinterpret_cast<const uint8_t*>(W) + r * ldw);
+}
+
+// the dequantisation table of a 4-bit instantiation (the fp16 ones declare no shared table)
+template <int WF>
+__device__ __forceinline__ float* gemv_q4_table() {
+  __shared__ float tab[16];
+  return tab;
+}
+
+template <int WF>
+__device__ __forceinline__ uint4 gemv_wvec(const GemvVec<WF>& w, float absmax, const float* tab) {
+  if constexpr (WF == 0) return w;
+  else return q4_deq8(w, absmax, tab);
+}
 
 // LORA: the LoRA expand of include/seedb200.h in the epilogue (lo.T staged in shared memory; ksplit must be 1).  Lane
 // 2 m + i of the warp that owns a row pair finishes output row r_i of activation row m: y = fp16(fp16(acc) + c), then
 // the residual add or (mode 1, gate and up exchanged between the two lanes) the SiLU gate.  Without LORA the code is
 // the plain GEMV.
-template <int M, int MODE, bool NORM, int U, bool NA, bool LORA>
+template <int M, int MODE, bool NORM, int U, bool NA, bool LORA, int WF>
 __global__ void __launch_bounds__(256)
 gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long long ldw, __half* __restrict__ out,
             const __half* __restrict__ residual, const __half* __restrict__ norm_w, float eps, int N, int K,
-            int ksplit, int iters, long long ldo, int pf_lines, seedb200_lora_operand lo) {
+            int ksplit, int iters, long long ldo, int pf_lines, seedb200_lora_operand lo,
+            const float* __restrict__ absmax) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __shared__ float lts[LORA ? M * LORA_MAX_RTOT : 1];
   uint4* xs = reinterpret_cast<uint4*>(smem_raw);     // [M][K/8]
@@ -103,24 +145,29 @@ gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long lon
     if (MODE == 1) { r0 = (long long)(t / 128) * 256 + (t % 128); r1 = r0 + 128; }
     else { r0 = 2LL * t; r1 = min(r0 + 1, (long long)N - 1); }
   };
+  const int nblk = K / Q4_BLOCK;                      // 4-bit: absmax entries per row
   // first batch of this warp's first task: in flight while the activations are staged
-  uint4 wa[U], wb[U];
+  GemvVec<WF> wa[U], wb[U];
+  float sa[WF ? U : 1], sb[WF ? U : 1];               // 4-bit: absmax of each vector's block
   const int t_first = blockIdx.x * tpi + tin;
   if (t_first < n_tasks) {
     long long r0, r1;
     rows_of(t_first, r0, r1);
-    const uint4* w0 = reinterpret_cast<const uint4*>(W + r0 * ldw);
-    const uint4* w1 = reinterpret_cast<const uint4*>(W + r1 * ldw);
+    const GemvVec<WF>* w0 = gemv_row<WF>(W, r0, ldw);
+    const GemvVec<WF>* w1 = gemv_row<WF>(W, r1, ldw);
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int vi = v0 + lane + u * 32;
-      if (vi < v1) { wa[u] = gemv_ldw<NA>(w0 + vi); wb[u] = gemv_ldw<NA>(w1 + vi); }
+      if (vi < v1) {
+        wa[u] = gemv_ldw<NA>(w0 + vi); wb[u] = gemv_ldw<NA>(w1 + vi);
+        if constexpr (WF != 0) { sa[u] = __ldg(absmax + r0 * nblk + vi / 8); sb[u] = __ldg(absmax + r1 * nblk + vi / 8); }
+      }
     }
     // ... and the next pf_lines 128-byte lines of both rows go to L2: with programmatic dependent launch this CTA is
     // resident long before its predecessor has finished, and the dependency wait + activation staging below would
     // otherwise leave HBM idle (weights never depend on the predecessor).  Sized by the host to ~24 MB per launch.
     for (int l = lane; l < pf_lines; l += 32) {
-      const int vi = v0 + 32 * U + l * 8;
+      const int vi = v0 + 32 * U + l * kGemvVecsPerLine<WF>;
       if (vi < v1) { prefetch_l2(w0 + vi); prefetch_l2(w1 + vi); }
     }
   }
@@ -161,6 +208,9 @@ gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long lon
   } else {
     for (int i = threadIdx.x; i < M * nvec; i += nthr) xs[i] = reinterpret_cast<const uint4*>(x)[i];
   }
+  if constexpr (WF != 0) {
+    if (threadIdx.x < 16) gemv_q4_table<WF>()[threadIdx.x] = kQ4Value[WF - 1][threadIdx.x];
+  }
   if constexpr (LORA) {
     const int rt = lo.r * lo.nsub;
     for (int i = threadIdx.x; i < M * rt; i += nthr)
@@ -177,25 +227,34 @@ gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long lon
     for (int m = 0; m < M; ++m) { a0[m] = 0.0f; a1[m] = 0.0f; }
     if (valid) {
       rows_of(t, r0, r1);
-      const uint4* w0 = reinterpret_cast<const uint4*>(W + r0 * ldw);
-      const uint4* w1 = reinterpret_cast<const uint4*>(W + r1 * ldw);
+      const GemvVec<WF>* w0 = gemv_row<WF>(W, r0, ldw);
+      const GemvVec<WF>* w1 = gemv_row<WF>(W, r1, ldw);
       for (int v = v0 + lane; v < v1; v += 32 * U) {
         if (it != 0 || v != v0 + lane) {    // the very first batch is already in registers
 #pragma unroll
           for (int u = 0; u < U; ++u) {
             const int vi = v + u * 32;
-            if (vi < v1) { wa[u] = gemv_ldw<NA>(w0 + vi); wb[u] = gemv_ldw<NA>(w1 + vi); }
+            if (vi < v1) {
+              wa[u] = gemv_ldw<NA>(w0 + vi); wb[u] = gemv_ldw<NA>(w1 + vi);
+              if constexpr (WF != 0) {
+                sa[u] = __ldg(absmax + r0 * nblk + vi / 8); sb[u] = __ldg(absmax + r1 * nblk + vi / 8);
+              }
+            }
           }
         }
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int vi = v + u * 32;
           if (vi < v1) {
+            const float* tab = nullptr;
+            if constexpr (WF != 0) tab = gemv_q4_table<WF>();
+            const uint4 da = gemv_wvec<WF>(wa[u], sa[WF ? u : 0], tab);
+            const uint4 db = gemv_wvec<WF>(wb[u], sb[WF ? u : 0], tab);
 #pragma unroll
             for (int m = 0; m < M; ++m) {
               const uint4 xv = xs[m * nvec + vi];
-              dot8(wa[u], xv, a0[m]);
-              dot8(wb[u], xv, a1[m]);
+              dot8(da, xv, a0[m]);
+              dot8(db, xv, a1[m]);
             }
           }
         }
@@ -273,8 +332,15 @@ gemv_kernel(const __half* __restrict__ x, const __half* __restrict__ W, long lon
   }
 }
 
-int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w, float eps,
-         int M, int N, int K, int mode, cudaStream_t stream, int64_t ldo, const seedb200_lora_operand* lora) {
+// U of the 4-bit instantiations: 16 groups per row in flight (64 bytes of codes per lane and row, the fp16 GEMV's
+// bytes in flight per lane); -Xptxas -v shows no spills
+constexpr int GEMV_U_Q4 = 16;
+
+// WF as in gemv_kernel; 4-bit: W = packed codes (ldw in bytes), absmax, no LoRA, no-allocate weight loads
+template <int WF>
+static int gemv_impl(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w,
+                     float eps, int M, int N, int K, int mode, cudaStream_t stream, int64_t ldo,
+                     const seedb200_lora_operand* lora, const float* absmax) {
   if (ldo <= 0) ldo = mode == 1 ? N / 2 : N;
   seedb200_lora_operand lo;
   memset(&lo, 0, sizeof(lo));
@@ -287,6 +353,7 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
   SB_REQUIRE(M >= 1 && M <= GEMV_MAXM, "gemv: M=%d outside [1,%d]", M, GEMV_MAXM);
   SB_REQUIRE(K % 8 == 0 && ldw % 8 == 0, "gemv: K and ldw must be multiples of 8");
   SB_REQUIRE(mode == 0 || (mode == 1 && N % 256 == 0 && residual == nullptr), "gemv: bad mode/shape");
+  if constexpr (WF != 0) SB_REQUIRE(lora == nullptr && absmax != nullptr, "gemv_4bit: bad operands");
   const size_t smem = (size_t)M * K * 2;
   SB_REQUIRE(smem <= 200 * 1024, "gemv: activation rows do not fit shared memory (M=%d K=%d)", M, K);
   const int n_tasks = mode == 1 ? N / 2 : (N + 1) / 2;
@@ -299,7 +366,7 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
   __half* op = static_cast<__half*>(out);
 #define SB_GEMV_LAUNCH(M_, MD_, NM_, U_, NA_, LO_)                                                         \
   {                                                                                                        \
-    auto kern = gemv_kernel<M_, MD_, NM_, U_, NA_, LO_>;                                                        \
+    auto kern = gemv_kernel<M_, MD_, NM_, U_, NA_, LO_, WF>;                                               \
     const int threads = 256;                                                                               \
     static size_t attr_smem_dev[SB_MAX_DEVICES] = {};   /* per device: cudaFuncSetAttribute is */          \
     const int dev_ = cur_device();                                                                         \
@@ -330,24 +397,30 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
     /* L2 prefetch ahead of the dependency wait: ~24 MB per launch, spread over the tasks' first lines */    \
     int pf_lines = get_option("gemv_prefetch_mb") > 0                                                       \
                        ? (int)(((long long)get_option("gemv_prefetch_mb") << 20) / (2LL * n_tasks * 128)) : 0; \
-    if (pf_lines > (K * 2 / ksplit) / 128) pf_lines = (K * 2 / ksplit) / 128;                               \
+    const int row_bytes = WF ? K / 2 : K * 2;                                                              \
+    if (pf_lines > (row_bytes / ksplit) / 128) pf_lines = (row_bytes / ksplit) / 128;                       \
     SB_CHECK_CUDA(launch_chain(kern, dim3(blocks), dim3(threads), smem, stream, xp, wp, (long long)ldw, op, rp, np, eps, N, K, \
-                               ksplit, iters, (long long)ldo, pf_lines, lo));                              \
+                               ksplit, iters, (long long)ldo, pf_lines, lo, absmax));                      \
     SB_LAUNCH_CHECK();                                                                                     \
     return 0;                                                                                              \
   }
 #define SB_GEMV(M_, MD_)                                                                                   \
   if (M == M_ && mode == MD_) {                                                                            \
-    if (lora != nullptr) {                                                                                 \
-      if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, true, true)                                  \
-      SB_GEMV_LAUNCH(M_, MD_, false, 4, true, true)                                                        \
+    if constexpr (WF != 0) {                                                                               \
+      if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, GEMV_U_Q4, true, false)                         \
+      SB_GEMV_LAUNCH(M_, MD_, false, GEMV_U_Q4, true, false)                                               \
+    } else {                                                                                               \
+      if (lora != nullptr) {                                                                               \
+        if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, true, true)                                \
+        SB_GEMV_LAUNCH(M_, MD_, false, 4, true, true)                                                      \
+      }                                                                                                    \
+      if (no_alloc) {                                                                                      \
+        if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, true, false)                               \
+        SB_GEMV_LAUNCH(M_, MD_, false, 4, true, false)                                                     \
+      }                                                                                                    \
+      if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, false, false)                                \
+      SB_GEMV_LAUNCH(M_, MD_, false, 4, false, false)                                                      \
     }                                                                                                      \
-    if (no_alloc) {                                                                                        \
-      if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, true, false)                                 \
-      SB_GEMV_LAUNCH(M_, MD_, false, 4, true, false)                                                       \
-    }                                                                                                      \
-    if (norm_w != nullptr) SB_GEMV_LAUNCH(M_, MD_, true, 4, false, false)                                  \
-    SB_GEMV_LAUNCH(M_, MD_, false, 4, false, false)                                                        \
   }
   SB_GEMV(1, 0) SB_GEMV(2, 0) SB_GEMV(3, 0) SB_GEMV(4, 0)
   SB_GEMV(1, 1) SB_GEMV(2, 1) SB_GEMV(3, 1) SB_GEMV(4, 1)
@@ -355,6 +428,23 @@ int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* resid
 #undef SB_GEMV_LAUNCH
   set_error("gemv: unsupported configuration");
   return SEEDB200_ERR_UNSUPPORTED;
+}
+
+int gemv(const void* x, const void* W, int64_t ldw, void* out, const void* residual, const void* norm_w, float eps,
+         int M, int N, int K, int mode, cudaStream_t stream, int64_t ldo, const seedb200_lora_operand* lora) {
+  return gemv_impl<0>(x, W, ldw, out, residual, norm_w, eps, M, N, K, mode, stream, ldo, lora, nullptr);
+}
+
+int gemv_4bit(const void* x, const void* norm_w, float eps, const void* packed, const float* absmax, int type,
+              void* out, const void* residual, int M, int N, int K, int mode, cudaStream_t stream) {
+  SB_PROPAGATE(q4_check("gemv_4bit", type, N, K));
+  SB_REQUIRE(x && packed && absmax && out, "gemv_4bit: null operand");
+  SB_REQUIRE((reinterpret_cast<uintptr_t>(packed) & 15) == 0, "gemv_4bit: packed codes must be 16-byte aligned");
+  if (type == SEEDB200_Q4_FP4)
+    return gemv_impl<1 + SEEDB200_Q4_FP4>(x, packed, K / 2, out, residual, norm_w, eps, M, N, K, mode, stream, 0,
+                                          nullptr, absmax);
+  return gemv_impl<1 + SEEDB200_Q4_NF4>(x, packed, K / 2, out, residual, norm_w, eps, M, N, K, mode, stream, 0,
+                                        nullptr, absmax);
 }
 
 // ----------------------------------------------------------------------------
@@ -760,6 +850,12 @@ int seedb200_gemv(const void* x, const void* W, int64_t ldw, void* out, const vo
                   float eps, int M, int N, int K, int mode, void* stream) {
   SB_REQUIRE(x && W && out, "seedb200_gemv: null operand");
   return sb::gemv(x, W, ldw, out, residual, norm_w, eps, M, N, K, mode, static_cast<cudaStream_t>(stream));
+}
+
+int seedb200_gemv_4bit(const void* x, const void* norm_w, float eps, const void* packed, const void* absmax,
+                       int quant_type, void* out, const void* residual, int M, int N, int K, int mode, void* stream) {
+  return sb::gemv_4bit(x, norm_w, eps, packed, static_cast<const float*>(absmax), quant_type, out, residual, M, N, K,
+                       mode, static_cast<cudaStream_t>(stream));
 }
 
 int64_t seedb200_decode_attention_workspace_bytes(int B, int H, int max_seq) {

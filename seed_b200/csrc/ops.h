@@ -120,6 +120,16 @@ int int8_correction(const void* A16, int64_t lda, const void* W, int64_t ldw, co
                     const int* n_outliers, int M, int N, void* corr, cudaStream_t stream);
 int gemv_int8(const void* x, const void* norm_w, float eps, float threshold, const void* W, const void* SCB, void* out,
               const void* residual, int M, int N, int K, int mode, cudaStream_t stream);
+// bitsandbytes 4-bit weights (quant4.cu; the GEMV in misc.cu).  type: SEEDB200_Q4_FP4 / SEEDB200_Q4_NF4
+int q4_check(const char* who, int type, int N, int K);   // quant type and K % 64, reported through set_error
+// row n of W -> row (n / grp) * gstride + n % grp + off of packed [*, K/2] / absmax [*, K/64]
+int quantize_4bit_rows(const void* W, int64_t ldw, int N, int K, int type, void* packed, void* absmax, int grp,
+                       int gstride, int off, cudaStream_t stream);
+int dequantize_4bit(const void* packed, const void* absmax, int N, int K, int type, void* out, int64_t ldo,
+                    cudaStream_t stream);
+// seedb200_gemv on dequantize_4bit(packed, absmax), bit for bit, without materialising it
+int gemv_4bit(const void* x, const void* norm_w, float eps, const void* packed, const float* absmax, int type,
+              void* out, const void* residual, int M, int N, int K, int mode, cudaStream_t stream);
 // LoRA (lora.cu)
 constexpr int LORA_MAX_R = 64, LORA_MAX_RTOT = 3 * LORA_MAX_R;
 int lora_shrink(const void* x, int64_t ldx, const void* norm_w, float eps, const void* A, int M, int K, int rtot,

@@ -41,9 +41,13 @@ EXPORTS = [
     "seedb200_decode_attention_lineage", "seedb200_decode_attention_rope_lineage",
     "seedb200_lora_shrink", "seedb200_gemm_lora", "seedb200_gemv_lora", "seedb200_llama_lora_load",
     "seedb200_llama_lora_merge", "seedb200_llama_replace_weights",
+    "seedb200_quantize_4bit", "seedb200_dequantize_4bit", "seedb200_gemv_4bit", "seedb200_llama_create_4bit",
+    "seedb200_llama_4bit_load_weight",
 ]
 
 DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
+Q4_FP4, Q4_NF4 = 0, 1       # enum seedb200_quant4
+_Q4_TYPES = {"fp4": Q4_FP4, "nf4": Q4_NF4}
 _DTYPE_CODE = {torch.float16: DTYPE_F16, torch.float32: DTYPE_F32, torch.int8: DTYPE_I8}
 
 
@@ -240,6 +244,15 @@ def load() -> C.CDLL:
     lib.seedb200_llama_lora_load.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int, C.c_int, C.c_float]
     lib.seedb200_llama_lora_merge.argtypes = [C.c_void_p]
     lib.seedb200_llama_replace_weights.argtypes = [C.c_void_p, C.POINTER(Tensor), C.c_int]
+    lib.seedb200_quantize_4bit.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                           C.c_void_p]
+    lib.seedb200_dequantize_4bit.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64,
+                                             C.c_void_p]
+    lib.seedb200_gemv_4bit.argtypes = [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                       C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]
+    lib.seedb200_llama_create_4bit.argtypes = [C.POINTER(LlamaConfig), C.POINTER(Tensor), C.c_int, C.c_int,
+                                               C.POINTER(C.c_void_p)]
+    lib.seedb200_llama_4bit_load_weight.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p]
     _lib = lib
     return lib
 
@@ -681,6 +694,75 @@ def gemv_int8(x: torch.Tensor, cb: torch.Tensor, scb: torch.Tensor, threshold: f
     return out
 
 
+def quant4_type(quant_type) -> int:
+    """"fp4" / "nf4" (bitsandbytes' bnb_4bit_quant_type) or Q4_FP4 / Q4_NF4 -> the enum value"""
+    if isinstance(quant_type, str):
+        if quant_type not in _Q4_TYPES:
+            raise ValueError(f"bnb_4bit_quant_type must be 'fp4' or 'nf4' (got {quant_type!r})")
+        return _Q4_TYPES[quant_type]
+    if quant_type not in (Q4_FP4, Q4_NF4):
+        raise ValueError(f"4-bit quant type must be Q4_FP4 (0) or Q4_NF4 (1) (got {quant_type!r})")
+    return int(quant_type)
+
+
+def quantize_4bit(w: torch.Tensor, quant_type="fp4"):
+    """bitsandbytes 4-bit quantisation (blocks of 64): fp16 [N,K] -> (packed uint8 [N, K/2], absmax fp32 [N, K/64])."""
+    _need_cuda_f16(w, "quantize_4bit.w")
+    qt = quant4_type(quant_type)
+    N, K = w.shape
+    if w.stride(1) != 1 or w.stride(0) % 8 != 0 or w.data_ptr() % 16 != 0:
+        w = w.contiguous()
+    packed = torch.empty((N, K // 2), dtype=torch.uint8, device=w.device)
+    absmax = torch.empty((N, max(K // 64, 1)), dtype=torch.float32, device=w.device)
+    with on(w.device):
+        check(load().seedb200_quantize_4bit(w.data_ptr(), w.stride(0), N, K, qt, packed.data_ptr(), absmax.data_ptr(),
+                                            stream_ptr(w.device)), "seedb200_quantize_4bit")
+    return packed, absmax
+
+
+def _need_q4(packed: torch.Tensor, absmax: torch.Tensor, K: int, what: str) -> None:
+    N = packed.shape[0]
+    if (not packed.is_cuda or packed.dtype != torch.uint8 or tuple(packed.shape) != (N, K // 2)
+            or not packed.is_contiguous()):
+        raise RuntimeError(f"{what}: packed must be a contiguous CUDA uint8 [N, K/2] = [{N}, {K // 2}] tensor")
+    if (not absmax.is_cuda or absmax.dtype != torch.float32 or tuple(absmax.shape) != (N, K // 64)
+            or not absmax.is_contiguous()):
+        raise RuntimeError(f"{what}: absmax must be a contiguous CUDA float32 [N, K/64] = [{N}, {K // 64}] tensor")
+
+
+def dequantize_4bit(packed: torch.Tensor, absmax: torch.Tensor, quant_type="fp4",
+                    out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """packed uint8 [N, K/2] + absmax fp32 [N, K/64] -> W' fp16 [N, K]."""
+    qt = quant4_type(quant_type)
+    N, K = packed.shape[0], packed.shape[1] * 2
+    _need_q4(packed, absmax, K, "dequantize_4bit")
+    if out is None:
+        out = torch.empty((N, K), dtype=torch.float16, device=packed.device)
+    with on(packed.device):
+        check(load().seedb200_dequantize_4bit(packed.data_ptr(), absmax.data_ptr(), N, K, qt, out.data_ptr(),
+                                              out.stride(0), stream_ptr(packed.device)), "seedb200_dequantize_4bit")
+    return out
+
+
+def gemv_4bit(x: torch.Tensor, packed: torch.Tensor, absmax: torch.Tensor, quant_type="fp4",
+              residual: Optional[torch.Tensor] = None, norm_w: Optional[torch.Tensor] = None, eps: float = 1e-6,
+              mode: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gemv() on dequantize_4bit(packed, absmax), bit for bit, for M <= 4 rows without materialising W'."""
+    _need_cuda_f16(x, "gemv_4bit.x")
+    qt = quant4_type(quant_type)
+    x = x.contiguous()
+    M, K = x.shape
+    N = packed.shape[0]
+    _need_q4(packed, absmax, K, "gemv_4bit")
+    if out is None:
+        out = torch.empty((M, N // 2 if mode == 1 else N), dtype=torch.float16, device=x.device)
+    with on(x.device):
+        check(load().seedb200_gemv_4bit(x.data_ptr(), _p(norm_w), eps, packed.data_ptr(), absmax.data_ptr(), qt,
+                                        out.data_ptr(), _p(residual), M, N, K, mode, stream_ptr(x.device)),
+              "seedb200_gemv_4bit")
+    return out
+
+
 def decode_attention(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, kv_len: int,
                      scale: float) -> torch.Tensor:
     """q [B,H,D] against the first kv_len rows of caches [B,H,max_seq,D] -> [B, H*D]."""
@@ -957,10 +1039,14 @@ class Llama:
 
     def __init__(self, weights: Dict[str, torch.Tensor], hidden: int, layers: int, heads: int, ffn: int, vocab: int,
                  max_batch: int = 1, max_seq: int = 4096, rms_eps: float = 1e-6, rope_base: float = 10000.0,
-                 gemm_ctas: int = 0, int8_threshold: Optional[float] = None):
+                 gemm_ctas: int = 0, int8_threshold: Optional[float] = None, quant4=None):
         """int8_threshold: None = fp16 weights (seedb200_llama_create); a float = LLM.int8() decoder linears given as
         int8 "<name>.weight" + fp32 "<name>.SCB" (seedb200_llama_create_int8), which the handle copies: only the
-        fp16 tensors stay referenced after construction."""
+        fp16 tensors stay referenced after construction.  quant4 ("fp4" / "nf4"): bitsandbytes 4-bit decoder
+        linears (seedb200_llama_create_4bit); `weights` then holds no decoder linear, and each is given to
+        load_4bit_weight() before the model runs."""
+        if int8_threshold is not None and quant4 is not None:
+            raise ValueError("int8_threshold and quant4 are exclusive")
         lib = load()
         self._weights = dict(weights)
         arr, keep = _tensor_array(self._weights)
@@ -969,7 +1055,10 @@ class Llama:
                           rope_base, gemm_ctas)
         h = C.c_void_p()
         with on(self.device):
-            if int8_threshold is None:
+            if quant4 is not None:
+                check(lib.seedb200_llama_create_4bit(C.byref(cfg), arr, len(self._weights), quant4_type(quant4),
+                                                     C.byref(h)), "seedb200_llama_create_4bit")
+            elif int8_threshold is None:
                 check(lib.seedb200_llama_create(C.byref(cfg), arr, len(self._weights), C.byref(h)),
                       "seedb200_llama_create")
             else:
@@ -1074,6 +1163,22 @@ class Llama:
         with on(self.device):
             check(load().seedb200_llama_int8_load_weight(self._h, name.encode(), w.data_ptr(), w.stride(0),
                                                          stream_ptr(self.device)), "seedb200_llama_int8_load_weight")
+
+    def load_4bit_weight(self, name: str, w: torch.Tensor) -> None:
+        """quantise the fp16 decoder linear `name` straight into the 4-bit handle's fused layout"""
+        _need_cuda_f16(w, name)
+        if w.stride(1) != 1 or w.device != self.device:
+            raise RuntimeError(f"{name}: expected rows with contiguous columns on {self.device}")
+        lin = name.split(".")[-2] if name.count(".") >= 2 else ""
+        N, K = {"q_proj": (self.hidden, self.hidden), "k_proj": (self.hidden, self.hidden),
+                "v_proj": (self.hidden, self.hidden), "o_proj": (self.hidden, self.hidden),
+                "gate_proj": (self.ffn, self.hidden), "up_proj": (self.ffn, self.hidden),
+                "down_proj": (self.hidden, self.ffn)}.get(lin, tuple(w.shape))
+        if tuple(w.shape) != (N, K):
+            raise RuntimeError(f"{name}: expected shape [{N}, {K}], got {list(w.shape)}")
+        with on(self.device):
+            check(load().seedb200_llama_4bit_load_weight(self._h, name.encode(), w.data_ptr(), w.stride(0),
+                                                         stream_ptr(self.device)), "seedb200_llama_4bit_load_weight")
 
     def lora_load(self, tensors: Dict[str, torch.Tensor], r: int, alpha: float) -> None:
         """copy a LoRA adapter ("model.layers.N.<...>.lora_A.weight" / ".lora_B.weight", fp16 on this device) into the

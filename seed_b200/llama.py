@@ -13,6 +13,9 @@ Reference behaviours kept on purpose (SURVEY.md section 7 "quirks"):
 `load_in_8bit=True` runs the seven linear layers of every decoder layer as LLM.int8() (transformers' bitsandbytes
 path, threshold `llm_int8_threshold`): int8 weights with per-row scales, per-call activation quantisation with fp16
 outlier columns; embed_tokens, lm_head and the norms stay fp16 (include/seedb200.h states the arithmetic).
+`load_in_4bit=True` runs the same seven linears as bitsandbytes 4-bit weights (`bnb_4bit_quant_type` "fp4" or "nf4",
+blocks of 64 with an fp32 absmax): decode steps of up to 4 rows stream the packed codes through the 4-bit GEMV;
+longer calls dequantise each linear into an fp16 scratch and run the fp16 GEMM, as bitsandbytes' MatMul4Bit does.
 Differences: `past_key_values` are views of the handle's preallocated cache (no torch.cat per step);
 `output_attentions` / `output_hidden_states` are not available (the reference's xformers path never computed
 attention weights either).
@@ -38,13 +41,53 @@ class _CudaView:
                                          "strides": tuple(s * 2 for s in strides_elems)}
 
 
-_INT8_LINEARS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
+_QUANTISED_LINEARS = ("q_proj", "k_proj", "v_proj", "o_proj", "gate_proj", "up_proj", "down_proj")
 
 
-def _is_int8_linear(name: str) -> bool:
-    """the decoder-layer nn.Linear weights transformers' load_in_8bit replaces (lm_head is kept in fp16)"""
+def _is_quantised_linear(name: str) -> bool:
+    """the decoder-layer nn.Linear weights transformers' load_in_8bit / load_in_4bit replace (lm_head stays fp16)"""
     parts = name.split(".")
-    return ".layers." in name and len(parts) >= 2 and parts[-1] == "weight" and parts[-2] in _INT8_LINEARS
+    return ".layers." in name and len(parts) >= 2 and parts[-1] == "weight" and parts[-2] in _QUANTISED_LINEARS
+
+
+_QUANT_DEFAULTS = {"load_in_8bit": False, "load_in_4bit": False, "llm_int8_threshold": 6.0,
+                   "bnb_4bit_quant_type": "fp4", "bnb_4bit_compute_dtype": None, "bnb_4bit_use_double_quant": False}
+
+
+def quant_options(quantization_config=None, **given) -> dict:
+    """transformers 4.30.2's bitsandbytes options -> {load_in_8bit, llm_int8_threshold, load_in_4bit,
+    bnb_4bit_quant_type}.  `given` holds the keywords the caller passed; `quantization_config` (a BitsAndBytesConfig,
+    read by attribute, or a dict) replaces them, and passing both is an error, as in transformers.  Everything that
+    cannot run here is refused by name before any weight is read or allocated."""
+    unknown = set(given) - set(_QUANT_DEFAULTS)
+    if unknown:
+        raise TypeError(f"unknown quantisation options {sorted(unknown)}")
+    if quantization_config is not None:
+        if given:
+            raise ValueError(f"pass either quantization_config or {sorted(given)}, not both")
+        cfg = quantization_config
+
+        def get(k):
+            return cfg.get(k) if isinstance(cfg, dict) else getattr(cfg, k, None)
+
+        given = {k: get(k) for k in _QUANT_DEFAULTS if get(k) is not None}
+    o = dict(_QUANT_DEFAULTS)
+    o.update(given)
+    if o["load_in_8bit"] and o["load_in_4bit"]:
+        raise ValueError("load_in_8bit and load_in_4bit are both True, and only one can be used at the same time")
+    if o["bnb_4bit_use_double_quant"]:
+        raise NotImplementedError("bnb_4bit_use_double_quant=True: double quantisation of the 4-bit absmax values is "
+                                  "not supported")
+    cd = o["bnb_4bit_compute_dtype"]
+    if isinstance(cd, str):
+        cd = getattr(torch, cd, cd)
+    if cd not in (None, torch.float32, torch.float16):
+        raise NotImplementedError(f"bnb_4bit_compute_dtype={o['bnb_4bit_compute_dtype']!r}: only None, torch.float32 "
+                                  f"and torch.float16 are supported (they give the same fp16 result; bf16 does not)")
+    if o["bnb_4bit_quant_type"] not in ("fp4", "nf4"):
+        raise ValueError(f"bnb_4bit_quant_type must be 'fp4' or 'nf4' (got {o['bnb_4bit_quant_type']!r})")
+    return {"load_in_8bit": bool(o["load_in_8bit"]), "llm_int8_threshold": float(o["llm_int8_threshold"]),
+            "load_in_4bit": bool(o["load_in_4bit"]), "bnb_4bit_quant_type": o["bnb_4bit_quant_type"]}
 
 
 def _one_device(device_map) -> torch.device:
@@ -80,8 +123,13 @@ def _linear_items(state_dict, names):
 class LlamaForCausalLM(nn.Module):
     def __init__(self, config: LlamaConfig, state_dict, device="cuda", max_batch: int = 1,
                  max_seq: Optional[int] = None, gemm_ctas: int = 0, load_in_8bit: bool = False,
-                 llm_int8_threshold: float = 6.0):
+                 llm_int8_threshold: float = 6.0, load_in_4bit: bool = False, bnb_4bit_quant_type: str = "fp4",
+                 bnb_4bit_compute_dtype=None, bnb_4bit_use_double_quant: bool = False):
         super().__init__()
+        q = quant_options(load_in_8bit=load_in_8bit, llm_int8_threshold=llm_int8_threshold, load_in_4bit=load_in_4bit,
+                          bnb_4bit_quant_type=bnb_4bit_quant_type, bnb_4bit_compute_dtype=bnb_4bit_compute_dtype,
+                          bnb_4bit_use_double_quant=bnb_4bit_use_double_quant)
+        load_in_8bit, load_in_4bit = q["load_in_8bit"], q["load_in_4bit"]
         dev = torch.device(device)
         if dev.type != "cuda" or not torch.cuda.is_available():
             raise RuntimeError("LlamaForCausalLM (seed_b200) needs a CUDA device: there is no CPU path")
@@ -92,17 +140,18 @@ class LlamaForCausalLM(nn.Module):
             raise ValueError("grouped-query attention is not part of models/llama_xformer.py")
         self.max_batch = max_batch
         self.max_seq = max_seq or config.max_position_embeddings
-        self.is_loaded_in_8bit = bool(load_in_8bit)
-        if load_in_8bit:
+        self.is_loaded_in_8bit = load_in_8bit
+        self.is_loaded_in_4bit = load_in_4bit
+        if load_in_8bit or load_in_4bit:
             # the handle is made with the fp16 tensors only; then each linear goes to the device in fp16, is quantised
-            # straight into the handle's int8 buffers, and is dropped before the next: device memory stays at the
-            # int8 model plus one fp16 tensor
+            # straight into the handle's int8 / 4-bit buffers, and is dropped before the next: device memory stays at
+            # the quantised model plus one fp16 tensor
             weights, linears = {}, []
             items = iter(state_dict.items())
             for k, v in items:
                 if "rotary_emb" in k:
                     continue
-                if _is_int8_linear(k):
+                if _is_quantised_linear(k):
                     linears.append(k)
                     continue
                 weights[k] = v.detach().to(device=dev, dtype=torch.float16).contiguous()
@@ -110,14 +159,19 @@ class LlamaForCausalLM(nn.Module):
             self._llm = L.Llama(weights, hidden=h, layers=nl, heads=nh, ffn=config.intermediate_size,
                                 vocab=config.vocab_size, max_batch=max_batch, max_seq=self.max_seq,
                                 rms_eps=config.rms_norm_eps, gemm_ctas=gemm_ctas,
-                                int8_threshold=float(llm_int8_threshold))
+                                int8_threshold=q["llm_int8_threshold"] if load_in_8bit else None,
+                                quant4=q["bnb_4bit_quant_type"] if load_in_4bit else None)
             for k, v in _linear_items(state_dict, linears):
                 w16 = v.detach().to(device=dev, dtype=torch.float16)
-                if w16.stride(-1) != 1:
+                if w16.stride(-1) != 1 or (load_in_4bit and not w16.is_contiguous()):
                     w16 = w16.contiguous()
-                self._llm.int8_load_weight(k, w16)
-                # int8 values plus one fp32 scale per row
-                self._weight_bytes += w16.shape[0] * w16.shape[1] + 4 * w16.shape[0]
+                N, K = w16.shape
+                if load_in_8bit:
+                    self._llm.int8_load_weight(k, w16)
+                    self._weight_bytes += N * K + 4 * N           # int8 values plus one fp32 scale per row
+                else:
+                    self._llm.load_4bit_weight(k, w16)
+                    self._weight_bytes += N * K // 2 + 4 * (N * K // 64)   # packed codes plus one fp32 absmax per 64
                 del w16, v     # stream-ordered: the allocator reuses this block only after the kernel has read it
         else:
             weights = {k: v.detach().to(device=dev, dtype=torch.float16).contiguous() for k, v in state_dict.items()
@@ -140,7 +194,11 @@ class LlamaForCausalLM(nn.Module):
     def from_pretrained(cls, pretrained_model_name_or_path, torch_dtype=torch.float16, device="cuda", device_map=None,
                         **kwargs):
         """HF checkpoint directory (config.json + *.safetensors or pytorch_model*.bin).  `load_in_8bit`,
-        `llm_int8_threshold` and a single-device `device_map` are honoured as transformers does."""
+        `llm_int8_threshold`, `load_in_4bit`, `bnb_4bit_quant_type`, `bnb_4bit_compute_dtype`,
+        `bnb_4bit_use_double_quant`, a `quantization_config` holding them (attributes or a dict) and a single-device
+        `device_map` are honoured as transformers does."""
+        quant = quant_options(kwargs.pop("quantization_config", None),
+                              **{k: kwargs.pop(k) for k in list(kwargs) if k in _QUANT_DEFAULTS})
         if device_map is not None:
             device = _one_device(device_map)
         path = str(pretrained_model_name_or_path)
@@ -162,9 +220,8 @@ class LlamaForCausalLM(nn.Module):
                 sd.update(torch.load(fn, map_location="cpu"))
         if not sd:
             raise RuntimeError(f"no weight files found under {path}")
-        kwargs = {k: v for k, v in kwargs.items()
-                  if k in ("max_batch", "max_seq", "gemm_ctas", "load_in_8bit", "llm_int8_threshold")}
-        return cls(config, sd, device=device, **kwargs)
+        kwargs = {k: v for k, v in kwargs.items() if k in ("max_batch", "max_seq", "gemm_ctas")}
+        return cls(config, sd, device=device, **kwargs, **quant)
 
     # ---- nn.Module conveniences ------------------------------------------------------------------
     @property
@@ -175,8 +232,11 @@ class LlamaForCausalLM(nn.Module):
         return self
 
     def get_memory_footprint(self) -> int:
-        """device bytes of the model's weights (int8 linears count their int8 values and fp32 scales); the KV cache
-        and workspaces are excluded, as in transformers."""
+        """device bytes of the model's weights; the KV cache and workspaces are excluded, as in transformers.  int8
+        linears count their int8 values and fp32 scales, 4-bit linears their packed codes (half a byte per weight)
+        and fp32 absmax values (one per 64 weights).  Counting the scales differs from transformers, which counts
+        only the quantised parameters.  The 4-bit handle's fp16 dequantisation scratch (2 * ffn * hidden
+        elements) is workspace and not counted."""
         return int(self._weight_bytes)
 
     def half(self):

@@ -169,6 +169,8 @@ class PeftModel:
             raise NotImplementedError("is_trainable=True: seed_b200 runs LoRA adapters for inference only")
         if getattr(model, "is_loaded_in_8bit", False):
             raise NotImplementedError("LoRA adapters on load_in_8bit models are not supported")
+        if getattr(model, "is_loaded_in_4bit", False):
+            raise NotImplementedError("LoRA adapters on load_in_4bit models are not supported")
         cfg, sd = load_adapter_files(model_id)
         r, alpha, targets, save = check_adapter_config(cfg)
         lora, saved = split_adapter(sd, targets, save)

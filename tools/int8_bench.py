@@ -1,11 +1,13 @@
-"""fp16 vs LLM.int8() LLaMA on one GPU: 13B decode and 7B prefill, random-init weights made on the device.
+"""fp16 vs LLM.int8() vs 4-bit (NF4) LLaMA on one GPU: 13B decode and 7B prefill, random-init weights made on the device.
 
     python tools/int8_bench.py [--reps 3] [--json OUT]
 
-Both handles of a shape are built in one process and timed alternately (fp16, int8, fp16, int8, ...):
+The three handles of a shape are built in one process and timed alternately (fp16, int8, nf4, fp16, ...):
   * 13B decode: prompt P = 256, 128 new tokens through seedb200_llama_generate (greedy, graph-replayed steps);
     ms/token = (time(129 new tokens) - time(1 new token)) / 128, i.e. without the prefill.  Achieved GB/s counts the
-    weight bytes one decode step must read (int8 decoder linears + their scales + fp16 lm_head row reads).
+    weight bytes one decode step must read (quantised decoder linears + their scales + fp16 lm_head row reads).
+  * 13B beam search, B = 1, k = 5: ms per decode step = (time(33 new tokens) - time(1 new token)) / 32.  Five rows
+    take the GEMM path: the 4-bit model dequantises every decoder linear in every step.
   * 7B prefill: B = 1, S = 2048, logits of the last position only; tokens/s.
   * device memory: get_memory_footprint() (weights) of each model.
 The card name and power limit are read in the same run.
@@ -53,12 +55,16 @@ def random_state_dict(h, nl, ffn, V, seed=0):
     return SD()
 
 
-def build(shape, int8, max_seq, max_batch=1):
+KINDS = ("fp16", "int8", "nf4")
+
+
+def build(shape, kind, max_seq, max_batch=1):
     h, nl, nh, ffn, V = shape
     cfg = LlamaConfig(vocab_size=V, hidden_size=h, intermediate_size=ffn, num_hidden_layers=nl, num_attention_heads=nh,
                       num_key_value_heads=nh, rms_norm_eps=1e-6, max_position_embeddings=max(max_seq, 2048))
+    q = {"int8": {"load_in_8bit": True}, "nf4": {"load_in_4bit": True, "bnb_4bit_quant_type": "nf4"}}.get(kind, {})
     return LlamaForCausalLM(cfg, random_state_dict(h, nl, ffn, V), device="cuda", max_batch=max_batch,
-                            max_seq=max_seq, load_in_8bit=int8)
+                            max_seq=max_seq, **q)
 
 
 def timed(fn, reps=1):
@@ -77,11 +83,17 @@ def decode_ms_per_token(m, prompt, new):
     return (timed(lambda: gen(new + 1), 2) - timed(lambda: gen(1), 2)) / new
 
 
-def step_bytes(shape, int8):
+def beam_ms_per_step(m, prompt, new, k):
+    gen = lambda n: m._llm.beam_generate(prompt, n, k, eos_token_id=-1)   # noqa: E731
+    return (timed(lambda: gen(new + 1), 2) - timed(lambda: gen(1), 2)) / new
+
+
+def step_bytes(shape, kind):
     h, nl, nh, ffn, V = shape
     lin = nl * (4 * h * h + 3 * h * ffn)
     rows = nl * (3 * h + h + 2 * ffn + h)
-    return (lin + 4 * rows if int8 else 2 * lin) + 2 * V * h
+    q = {"fp16": 2 * lin, "int8": lin + 4 * rows, "nf4": lin // 2 + 4 * (lin // 64)}[kind]
+    return q + 2 * V * h
 
 
 def main():
@@ -96,27 +108,31 @@ def main():
     res = {"card": card}
     P, NEW = 256, 128
     shape = SHAPES["13b"]
-    models = {k: build(shape, k == "int8", P + NEW + 8) for k in ("fp16", "int8")}
+    BEAMS, BNEW = 5, 32
+    models = {k: build(shape, k, P + NEW + 8, max_batch=BEAMS) for k in KINDS}
     for k, m in models.items():
         res[f"13b_{k}_weight_GB"] = m.get_memory_footprint() / 1e9
     prompt = torch.randint(0, shape[4], (1, P), device="cuda", generator=torch.Generator(device="cuda").manual_seed(1))
-    dec = {"fp16": [], "int8": []}
+    dec = {k: [] for k in KINDS}
+    beam = {k: [] for k in KINDS}
     for _ in range(args.reps):
         for k, m in models.items():
             dec[k].append(decode_ms_per_token(m, prompt, NEW))
+            beam[k].append(beam_ms_per_step(m, prompt, BNEW, BEAMS))
     for k in dec:
         ms = min(dec[k])
         res[f"13b_decode_{k}_ms_per_token"] = dec[k]
-        res[f"13b_decode_{k}_GBps"] = step_bytes(shape, k == "int8") / (ms * 1e-3) / 1e9
+        res[f"13b_decode_{k}_GBps"] = step_bytes(shape, k) / (ms * 1e-3) / 1e9
+        res[f"13b_beam{BEAMS}_{k}_ms_per_step"] = beam[k]
     del models, m
     torch.cuda.empty_cache()
     shape = SHAPES["7b"]
     S = 2048
-    models = {k: build(shape, k == "int8", S) for k in ("fp16", "int8")}
+    models = {k: build(shape, k, S) for k in KINDS}
     for k, m in models.items():
         res[f"7b_{k}_weight_GB"] = m.get_memory_footprint() / 1e9
     ids = torch.randint(0, shape[4], (1, S), device="cuda", generator=torch.Generator(device="cuda").manual_seed(2))
-    pre = {"fp16": [], "int8": []}
+    pre = {k: [] for k in KINDS}
     for _ in range(args.reps):
         for k, m in models.items():
             pre[k].append(S / (timed(lambda: m._llm.forward(input_ids=ids, last_only=True), 3) * 1e-3))
