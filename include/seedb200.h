@@ -253,8 +253,10 @@ int seedb200_gemv_int8(const void* x, const void* norm_w, float eps, float thres
                        void* out, const void* residual, int M, int N, int K, int mode, void* stream);
 
 /* LlamaAttention.forward with q_len == 1 (llama_xformer.py:240-256, attn_bias=None): q [B,H,D] against the first
- * kv_len rows of caches laid out [B,H,max_seq,D]; out [B,H*D] fp16; D must be 128.  workspace: at least
- * seedb200_decode_attention_workspace_bytes(B, H, max_seq) bytes of device memory (split-KV partials).          */
+ * kv_len rows of caches laid out [B,H,max_seq,D]; out [B,H*D] fp16; D must be 128.  q and the caches must be
+ * 16-byte aligned.  workspace: at least seedb200_decode_attention_workspace_bytes(B, H, max_seq) bytes of device
+ * memory: split-KV partials for the largest split count of any kv_len <= max_seq (min(64, ceil(max_seq / 128))
+ * splits per head; the split count is not monotone in kv_len), then B*H int tickets.                            */
 int64_t seedb200_decode_attention_workspace_bytes(int B, int H, int max_seq);
 int seedb200_decode_attention(const void* q, const void* k_cache, const void* v_cache, void* out, int B, int H, int D,
                               int kv_len, int max_seq, float scale, void* workspace, void* stream);

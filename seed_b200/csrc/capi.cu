@@ -191,6 +191,8 @@ int seedb200_rope_kv_append(const void* qkv, const int64_t* positions, int B, in
 /* the fused decode form: RoPE + append + attention of one new token per sequence, one launch */
 int seedb200_decode_attention_rope(const void* qkv, const int64_t* positions, int B, int H, int D, int past_len,
                                    int max_seq, void* k_cache, void* v_cache, void* out, float scale, void* stream) {
+  SB_REQUIRE(sb::aligned16(qkv) && sb::aligned16(k_cache) && sb::aligned16(v_cache),
+             "seedb200_decode_attention_rope: qkv and the caches must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const void *cos_t, *sin_t;
   int max_pos;
@@ -203,6 +205,8 @@ int seedb200_decode_attention_rope_lineage(const void* qkv, const int64_t* posit
                                            int D, int past_len, int max_seq, void* k_cache, void* v_cache, void* out,
                                            float scale, void* stream) {
   SB_REQUIRE(slot != nullptr, "seedb200_decode_attention_rope_lineage: null slot table");
+  SB_REQUIRE(sb::aligned16(qkv) && sb::aligned16(k_cache) && sb::aligned16(v_cache),
+             "seedb200_decode_attention_rope_lineage: qkv and the caches must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const void *cos_t, *sin_t;
   int max_pos;

@@ -52,6 +52,9 @@ void count_launch(int n = 1);
     if (_s != 0) return _s;                                                              \
   } while (0)
 
+// kernels that load an operand as uint4 need it 16-byte aligned (checked on the host, before any device work)
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 constexpr int SB_MAX_DEVICES = 64;
 int cur_device();     // cudaGetDevice(), clamped to [0, SB_MAX_DEVICES)
 int num_sms();        // of the current device

@@ -352,6 +352,8 @@ static int gemv_impl(const void* x, const void* W, int64_t ldw, void* out, const
   }
   SB_REQUIRE(M >= 1 && M <= GEMV_MAXM, "gemv: M=%d outside [1,%d]", M, GEMV_MAXM);
   SB_REQUIRE(K % 8 == 0 && ldw % 8 == 0, "gemv: K and ldw must be multiples of 8");
+  SB_REQUIRE(aligned16(x) && aligned16(W) && (norm_w == nullptr || aligned16(norm_w)),
+             "gemv: x, W and norm_w must be 16-byte aligned");
   SB_REQUIRE(mode == 0 || (mode == 1 && N % 256 == 0 && residual == nullptr), "gemv: bad mode/shape");
   if constexpr (WF != 0) SB_REQUIRE(lora == nullptr && absmax != nullptr, "gemv_4bit: bad operands");
   const size_t smem = (size_t)M * K * 2;
@@ -495,8 +497,9 @@ decode_attn_partial(const __half* __restrict__ q, const __half* __restrict__ kc,
   pdl_wait();
   if (dyn != nullptr) {
     // graph-replayed decode step: the cache length lives in device memory (dyn[0] = tokens already cached, this
-    // step's token has just been appended); the grid was sized for max_seq keys, surplus splits exit
-    kv_len = dyn[0] + 1;
+    // step's token has just been appended); the grid was sized for max_seq keys, surplus splits exit.  Clamped to
+    // the cache like the append kernels clamp their row.
+    kv_len = min(dyn[0] + 1, max_seq);
     da_split(kv_len, nsplit, chunk);
     if (split >= nsplit) return;
   }
@@ -597,7 +600,8 @@ decode_attn_partial(const __half* __restrict__ q, const __half* __restrict__ kc,
     ll += __ldcg(src + sidx * (DA_D + 2) + 1) * c;
     acc += __ldcg(src + sidx * (DA_D + 2) + 2 + tid) * c;
   }
-  out[((long long)b * H + h) * DA_D + tid] = __float2half_rn(ll > 0.0f ? acc / ll : 0.0f);
+  // ll is 0 only without keys; a NaN score makes it NaN, and the output NaN as torch's softmax does
+  out[((long long)b * H + h) * DA_D + tid] = __float2half_rn(ll != 0.0f ? acc / ll : 0.0f);
 }
 
 __global__ void __launch_bounds__(DA_D)
@@ -617,7 +621,7 @@ decode_attn_merge(const float* __restrict__ ws, __half* __restrict__ out, int ns
     ll += src[s * (DA_D + 2) + 1] * c;
     acc += src[s * (DA_D + 2) + 2 + d] * c;
   }
-  out[bh * DA_D + d] = __float2half_rn(ll > 0.0f ? acc / ll : 0.0f);
+  out[bh * DA_D + d] = __float2half_rn(ll != 0.0f ? acc / ll : 0.0f);
 }
 
 // ----------------------------------------------------------------------------
@@ -779,7 +783,7 @@ decode_attn_rope_kernel(const __half* __restrict__ qkv, const long long* __restr
     ll += s_ml[sidx][1] * cc;
     acc += s_part[sidx][gt] * cc;
   }
-  out[((long long)b * H + h) * DA_D + gt] = __float2half_rn(ll > 0.0f ? acc / ll : 0.0f);
+  out[((long long)b * H + h) * DA_D + gt] = __float2half_rn(ll != 0.0f ? acc / ll : 0.0f);
 }
 
 bool decode_attention_rope_supported(int D, int max_seq) {
@@ -793,6 +797,8 @@ int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int 
                           int max_pos, const void* cos_t, const void* sin_t, void* k_cache, void* v_cache, void* out,
                           float scale, cudaStream_t stream, const int* dyn, const int* slot) {
   SB_REQUIRE(qkv && k_cache && v_cache && out && cos_t && sin_t, "decode_attention_rope: null operand");
+  SB_REQUIRE(aligned16(qkv) && aligned16(k_cache) && aligned16(v_cache),
+             "decode_attention_rope: qkv and the caches must be 16-byte aligned");
   SB_REQUIRE(decode_attention_rope_supported(D, max_seq),
              "decode_attention_rope: head_dim %d / max_seq %d unsupported (head_dim 128, max_seq <= %d)", D, max_seq,
              4 * DAF_MAX_GROUPS * DA_BLK);
@@ -810,10 +816,12 @@ int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int 
   return 0;
 }
 
+// the most splits any kv_len <= max_seq takes.  da_split is not monotone in kv_len (8192 keys: 64 splits of 128,
+// 8193 keys: 33 splits of 256), so da_split(max_seq) itself is not a bound; ceil(kv_len / 128) capped at
+// DA_MAX_SPLITS is (every chunk holds at least one 128-key block).
 int decode_attention_max_splits(int max_seq) {
-  int nsplit, chunk;
-  da_split(max_seq < 1 ? 1 : max_seq, nsplit, chunk);
-  return nsplit;
+  const int n = ((max_seq < 1 ? 1 : max_seq) + DA_BLK - 1) / DA_BLK;
+  return n > DA_MAX_SPLITS ? DA_MAX_SPLITS : n;
 }
 
 // workspace: [B*H*max_splits*(D+2)] floats of partials (+ [B*H] int tickets when `tickets` is NULL: zeroed here on
@@ -824,8 +832,12 @@ int decode_attention(const void* q, const void* k_cache, const void* v_cache, vo
                      int* tickets, const int* slot) {
   SB_REQUIRE(D == DA_D, "decode_attention: head_dim %d unsupported (LLaMA uses 128)", D);
   SB_REQUIRE(dyn != nullptr || (kv_len >= 1 && kv_len <= max_seq), "decode_attention: kv_len %d outside [1,%d]", kv_len, max_seq);
-  int nsplit, chunk;
-  da_split(dyn != nullptr ? max_seq : kv_len, nsplit, chunk);    // dyn: grid for the longest cache, trimmed in-kernel
+  SB_REQUIRE(aligned16(q) && aligned16(k_cache) && aligned16(v_cache),
+             "decode_attention: q and the caches must be 16-byte aligned");
+  // dyn: the grid covers the split count of every cache length up to max_seq (surplus splits exit in-kernel, and
+  // the kernel derives its chunk from dyn)
+  int nsplit = decode_attention_max_splits(max_seq), chunk = 0;
+  if (dyn == nullptr) da_split(kv_len, nsplit, chunk);
   if (tickets == nullptr) {
     tickets = reinterpret_cast<int*>(static_cast<float*>(workspace) +
                                      (size_t)B * H * decode_attention_max_splits(max_seq) * (DA_D + 2));

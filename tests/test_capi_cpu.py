@@ -194,3 +194,51 @@ def test_gemm_plan_for_single_tile_rows_and_tuned_shapes(L):
                         (65792, 1408, 6144, 176)):
         p = _plan(L, M, N, K)
         assert (p["bn"], p["ctas"], p["sched"]) == (bn, 1, 0), p
+
+
+def _da_nsplit(kv_len):
+    """the split-KV decode attention's key-axis split (misc.cu da_split): one split per 128-key block up to 64
+    splits, then whole 128-key blocks per split, no empty split -- not monotone in kv_len (8192 -> 64, 8193 -> 33)"""
+    nsplit = min(64, -(-kv_len // 128))
+    chunk = -(-(-(-kv_len // nsplit)) // 128) * 128
+    return -(-kv_len // chunk)
+
+
+def test_decode_attention_workspace_covers_every_cache_length(L):
+    """the workspace for max_seq holds the partials of every kv_len <= max_seq (a graph-replayed decode step runs at
+    whatever length the cache has reached), plus B*H tickets.  Sized by da_split(max_seq) alone it fell short for
+    11,552 of the max_seq swept here (max_seq 8300: 33 splits, while kv_len 4225..8192 take 34..64)"""
+    h = L.load()
+    assert [_da_nsplit(n) for n in (1, 128, 129, 4225, 8192, 8193, 8300, 12000, 16384)] == [1, 1, 2, 34, 64, 33, 33, 47,
+                                                                                             64]
+    need = 0
+    for max_seq in range(1, 20001):
+        need = max(need, _da_nsplit(max_seq))            # the most splits of any kv_len <= max_seq
+        for B, H in ((1, 1), (3, 40)):
+            got = h.seedb200_decode_attention_workspace_bytes(B, H, max_seq)
+            assert B * H * (need * 130 * 4 + 4) <= got <= B * H * (64 * 130 * 4 + 4), (B, H, max_seq, need, got)
+
+
+def test_vector_loads_refuse_misaligned_pointers(L):
+    """the GEMV and the decode attentions load x / W / norm_w, q / qkv and the caches as 16-byte vectors: a pointer
+    off by 2, 4 or 8 bytes (a column-offset view) is refused with an error before any device work"""
+    h = L.load()
+    A = 1 << 20                                              # fake, 16-byte aligned device addresses: never touched
+
+    def refused(rc, what):
+        assert rc == 1, (what, rc, h.seedb200_last_error())
+        assert b"16-byte aligned" in h.seedb200_last_error(), (what, h.seedb200_last_error())
+
+    for x, w, nw in ((A + 2, A, None), (A, A + 8, None), (A, A, A + 4)):
+        for mode in (0, 1):
+            refused(h.seedb200_gemv(x, w, 512, A, None, nw, 1e-6, 2, 512, 512, mode, None), ("gemv", x, w, nw, mode))
+    for q, k, v in ((A + 2, A, A), (A, A + 8, A), (A, A, A + 4)):
+        refused(h.seedb200_decode_attention(q, k, v, A, 1, 2, 128, 5, 16, 0.088, A, None), ("decode_attention", q, k, v))
+        refused(h.seedb200_decode_attention_lineage(q, k, v, A, A, 1, 2, 128, 5, 16, 0.088, A, None),
+                ("decode_attention_lineage", q, k, v))
+        rope = h.seedb200_decode_attention_rope
+        rope.argtypes = [C.c_void_p, C.c_void_p] + [C.c_int] * 5 + [C.c_void_p] * 3 + [C.c_float, C.c_void_p]
+        refused(rope(q, None, 1, 2, 128, 4, 16, k, v, A, 0.088, None), ("decode_attention_rope", q, k, v))
+        rope_lin = h.seedb200_decode_attention_rope_lineage
+        rope_lin.argtypes = [C.c_void_p] * 3 + [C.c_int] * 5 + [C.c_void_p] * 3 + [C.c_float, C.c_void_p]
+        refused(rope_lin(q, None, A, 1, 2, 128, 4, 16, k, v, A, 0.088, None), ("decode_attention_rope_lineage", q, k, v))
