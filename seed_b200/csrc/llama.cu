@@ -9,16 +9,12 @@
 //   * the KV cache is preallocated [B, H, max_seq, D] and appended in place by the RoPE kernel instead of
 //     torch.cat per layer per step (:236-237);
 //   * batch-1 decode (S == 1) switches to the HBM-bound GEMV / split-KV kernels.
-// Weights named like the HF checkpoint (model.layers.N.self_attn.q_proj.weight ...).  o_proj, down_proj,
-// norms, embed_tokens and lm_head are borrowed; q/k/v and gate/up are copied into their fused layouts and
-// the originals are not referenced after create.
-// int8 mode (seedb200_llama_create_int8, LLM.int8()): the seven decoder linears of every layer arrive as int8 CB plus
-// fp32 SCB and are copied into handle-owned fused layouts (q|k|v concatenated, gate|up interleaved in 128-row blocks,
-// the scales the same way); lin8() sends them to the int8 GEMV (<= 4 rows) or quantises the activations and runs the
-// int8 wgmma GEMM.
-// 4-bit mode (seedb200_llama_create_4bit, bitsandbytes FP4 / NF4): the seven decoder linears are quantised one at a time
-// into handle-owned packed codes + absmax in the same fused layouts; lin4() sends them to the 4-bit GEMV (<= 4 rows) or
-// dequantises the fused weight into a handle-owned fp16 scratch and runs the unchanged fp16 path on it.
+// Weights named like the HF checkpoint (model.layers.N.self_attn.q_proj.weight ...); norms, embed_tokens and lm_head
+// are borrowed.  The seven decoder linears of a layer (kLinear) are sub-blocks of four fused linears (fused()): q|k|v
+// concatenated, o, gate|up interleaved in blocks of 128 rows, down.  Weights, their scales and LoRA B share that row
+// order.  A handle holds its decoder linears in one WeightFormat -- fp16 (q|k|v and gate|up copied into handle-owned
+// buffers, o and down borrowed), LLM.int8() CB + SCB, or bitsandbytes FP4 / NF4 codes + absmax -- and
+// decoder_linear() is the one place that picks the kernels for it.
 #include <string.h>
 
 #include <map>
@@ -30,15 +26,14 @@
 #include "ops.h"
 
 namespace sb {
+enum WeightFormat { W_F16, W_INT8, W_4BIT };
+// one fused decoder linear [N, K]: fp16 w (s == nullptr), int8 CB [N, K] + SCB [N], or 4-bit packed codes [N, K/2] +
+// absmax [N, K/64]
+struct LinW { const void* w; const float* s; };
 struct LlamaLayerW {
-  const __half *in_ln, *post_ln, *qkv_w, *o_w, *gu_w, *down_w;
+  const __half *in_ln, *post_ln;
   __half *k_cache, *v_cache;
-  // int8 mode: CB [N,K] and SCB [N] of the fused projections
-  const int8_t *qkv8, *o8, *gu8, *down8;
-  const float *qkv_s, *o_s, *gu_s, *down_s;
-  // 4-bit mode: packed codes [N, K/2] and absmax [N, K/64] of the fused projections
-  const uint8_t *qkv4, *o4, *gu4, *down4;
-  const float *qkv_a, *o_a, *gu_a, *down_a;
+  LinW lin[4];
 };
 // LoRA adapter of one layer, per fused linear g (0 q|k|v, 1 o, 2 gate|up, 3 down): A_cat [nsub r, K], B [N, r]
 struct LoraLayer {
@@ -77,8 +72,8 @@ struct seedb200_llama {
   sb::BeamState beam;             // beam-search state (rows = batch * beams <= max_batch)
   int used_graph;
   int gen_cache_len;
-  // ---- int8 mode ----
-  int int8;
+  sb::WeightFormat fmt;           // of the decoder linears
+  // ---- int8 ----
   float threshold;
   std::vector<uint8_t> q_loaded;  // [layers][7]: the quantised (int8 or 4-bit) linear holds its weights
   __half* corr;                   // [max_batch * max_seq, 2 * ffn] outlier correction of the GEMM path
@@ -86,8 +81,7 @@ struct seedb200_llama {
   float* sca;                     // [max_batch * max_seq]
   int* olist;                     // [max(hidden, ffn)] outlier columns
   int* ocount;
-  // ---- 4-bit mode ----
-  int quant4;
+  // ---- 4-bit ----
   int q4type;                     // SEEDB200_Q4_FP4 / SEEDB200_Q4_NF4
   __half* q4_scratch;             // [max fused linear] fp16 W' of the linear the GEMM path runs
   // ---- LoRA adapter (seedb200_llama_lora_load) ----
@@ -152,59 +146,56 @@ static int llama_find_i8(const seedb200_llama* m, const std::string& base, int64
   return 0;
 }
 
-static const char* const kI8Lin[7] = {"self_attn.q_proj", "self_attn.k_proj", "self_attn.v_proj", "self_attn.o_proj",
-                                     "mlp.gate_proj", "mlp.up_proj", "mlp.down_proj"};
+// The decoder linears of a layer in HF order, each sub-block `sub` of fused linear g
+struct DecoderLinear { const char* name; int g, sub; };
+static const DecoderLinear kLinear[7] = {{"self_attn.q_proj", 0, 0}, {"self_attn.k_proj", 0, 1},
+                                         {"self_attn.v_proj", 0, 2}, {"self_attn.o_proj", 1, 0},
+                                         {"mlp.gate_proj", 2, 0},    {"mlp.up_proj", 2, 1},
+                                         {"mlp.down_proj", 3, 0}};
 
-// "model.layers.<l>.<linear i>.weight" -> (l, i); false for any other name
-static bool linear_of(const char* name, int* layer, int* lin) {
+// fused linear g of a layer: N x K, nsub sub-blocks of N / nsub rows interleaved in groups of grp rows
+struct Fused { int N, K, grp, nsub; };
+static Fused fused(const seedb200_llama* m, int g) {
+  const int h = m->cfg.hidden, ffn = m->cfg.ffn;
+  if (g == 0) return {3 * h, h, h, 3};
+  if (g == 1) return {h, h, h, 1};
+  if (g == 2) return {2 * ffn, h, 128, 2};
+  return {h, ffn, h, 1};
+}
+
+// "model.layers.<l>.<linear i><suffix>" -> (l, i); false for any other name
+static bool linear_of(const char* name, const char* suffix, int* layer, int* lin) {
   for (int k = 0; k < 7; ++k) {
-    char tail[64];
-    snprintf(tail, sizeof(tail), ".%s.weight", kI8Lin[k]);
+    char tail[96];
+    snprintf(tail, sizeof(tail), ".%s%s", kLinear[k].name, suffix);
     int l = -1, n = 0;
     if (sscanf(name, "model.layers.%d%n", &l, &n) == 1 && strcmp(name + n, tail) == 0) { *layer = l; *lin = k; return true; }
   }
   return false;
 }
 
-// Where quantised linear i of layer L lives in the handle's fused buffers: rows r of [N,K] go to row
-// (r / grp) * gstride + r % grp + off of the fused weight (int8 CB / 4-bit packed codes), and the scales of row r
-// (int8 SCB / 4-bit absmax) likewise (gate|up: blocks of 128 rows).
-struct QSlot { uint8_t* w; float* s; int64_t N, K, grp, gstride, off; };
-static QSlot q_slot(const seedb200_llama* m, int layer, int i) {
-  const int64_t h = m->cfg.hidden, ffn = m->cfg.ffn;
-  const sb::LlamaLayerW& L = m->layers[layer];
-  const int g = i < 3 ? 0 : (i == 3 ? 1 : (i < 6 ? 2 : 3));      // fused linear: q|k|v, o, gate|up, down
-  const void* w8[4] = {L.qkv8, L.o8, L.gu8, L.down8};
-  const float* s8[4] = {L.qkv_s, L.o_s, L.gu_s, L.down_s};
-  const void* w4[4] = {L.qkv4, L.o4, L.gu4, L.down4};
-  const float* s4[4] = {L.qkv_a, L.o_a, L.gu_a, L.down_a};
-  QSlot t;
-  t.w = static_cast<uint8_t*>(const_cast<void*>(m->quant4 ? w4[g] : w8[g]));
-  t.s = const_cast<float*>(m->quant4 ? s4[g] : s8[g]);
-  t.K = i == 6 ? ffn : h;
-  t.N = i == 6 ? h : (i >= 4 ? ffn : h);
-  t.grp = t.N; t.gstride = 0; t.off = 0;
-  if (i < 3) t.off = i * h;
-  else if (i == 4 || i == 5) { t.grp = 128; t.gstride = 256; t.off = i == 5 ? 128 : 0; }
-  return t;
-}
-
-template <typename T>
-static int llama_alloc(seedb200_llama* m, T** p, size_t elems) {
-  void* q = nullptr;
-  size_t bytes = elems * sizeof(T);
-  SB_CHECK_CUDA(cudaMalloc(&q, bytes < 256 ? 256 : bytes));
-  m->owned.push_back(q);
-  *p = static_cast<T*>(q);
+// copy the N / nsub rows (row_bytes each) of sub-block `sub` from src into their rows of fused linear F at dst
+static int place_rows(void* dst, const void* src, size_t row_bytes, const Fused& F, int sub, cudaStream_t st) {
+  const size_t grp = (size_t)F.grp * row_bytes;
+  SB_CHECK_CUDA(cudaMemcpy2DAsync(static_cast<uint8_t*>(dst) + sub * grp, F.nsub * grp, src, grp, grp,
+                                  (size_t)(F.N / F.nsub / F.grp), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
 
+// bytes of one row of K weights (*w) and of its scales (*s) in the handle's format
+static void row_bytes(const seedb200_llama* m, int64_t K, size_t* w, size_t* s) {
+  if (m->fmt == W_INT8) { *w = K; *s = 4; }
+  else if (m->fmt == W_4BIT) { *w = K / 2; *s = K / 64 * 4; }
+  else { *w = 2 * K; *s = 0; }
+}
+
+// at least 256 bytes, recorded in `list` (m->owned, or m->row_owned for the buffers sized by max_batch)
 template <typename T>
-static int llama_alloc_row(seedb200_llama* m, T** p, size_t elems) {
+static int llama_alloc(std::vector<void*>& list, T** p, size_t elems) {
   void* q = nullptr;
   size_t bytes = elems * sizeof(T);
   SB_CHECK_CUDA(cudaMalloc(&q, bytes < 256 ? 256 : bytes));
-  m->row_owned.push_back(q);
+  list.push_back(q);
   *p = static_cast<T*>(q);
   return 0;
 }
@@ -214,56 +205,57 @@ static int llama_alloc_rows(seedb200_llama* m, cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
   const int64_t h = c.hidden, ffn = c.ffn;
   const size_t cache_elems = (size_t)c.max_batch * c.heads * c.max_seq * c.head_dim;
+  std::vector<void*>& rows = m->row_owned;
   for (LlamaLayerW& L : m->layers) {
-    SB_PROPAGATE(llama_alloc_row(m, &L.k_cache, cache_elems));
-    SB_PROPAGATE(llama_alloc_row(m, &L.v_cache, cache_elems));
+    SB_PROPAGATE(llama_alloc(rows, &L.k_cache, cache_elems));
+    SB_PROPAGATE(llama_alloc(rows, &L.v_cache, cache_elems));
   }
   const size_t T = (size_t)c.max_batch * c.max_seq;
-  SB_PROPAGATE(llama_alloc_row(m, &m->x, T * h));
-  SB_PROPAGATE(llama_alloc_row(m, &m->nb, T * h));
-  SB_PROPAGATE(llama_alloc_row(m, &m->qkv, T * 3 * h));
-  SB_PROPAGATE(llama_alloc_row(m, &m->q, T * h));
-  SB_PROPAGATE(llama_alloc_row(m, &m->att, T * h));
-  SB_PROPAGATE(llama_alloc_row(m, &m->gu, T * ffn));
-  SB_PROPAGATE(llama_alloc_row(m, &m->hn, T * h));
-  SB_PROPAGATE(llama_alloc_row(m, &m->last, (size_t)c.max_batch * h));
+  SB_PROPAGATE(llama_alloc(rows, &m->x, T * h));
+  SB_PROPAGATE(llama_alloc(rows, &m->nb, T * h));
+  SB_PROPAGATE(llama_alloc(rows, &m->qkv, T * 3 * h));
+  SB_PROPAGATE(llama_alloc(rows, &m->q, T * h));
+  SB_PROPAGATE(llama_alloc(rows, &m->att, T * h));
+  SB_PROPAGATE(llama_alloc(rows, &m->gu, T * ffn));
+  SB_PROPAGATE(llama_alloc(rows, &m->hn, T * h));
+  SB_PROPAGATE(llama_alloc(rows, &m->last, (size_t)c.max_batch * h));
   m->ca = nullptr; m->sca = nullptr; m->corr = nullptr;
-  if (m->int8) {
-    SB_PROPAGATE(llama_alloc_row(m, &m->corr, T * (size_t)(2 * ffn > 3 * h ? 2 * ffn : 3 * h)));
-    SB_PROPAGATE(llama_alloc_row(m, &m->ca, T * (size_t)(ffn > h ? ffn : h)));
-    SB_PROPAGATE(llama_alloc_row(m, &m->sca, T));
+  if (m->fmt == W_INT8) {
+    SB_PROPAGATE(llama_alloc(rows, &m->corr, T * (size_t)(2 * ffn > 3 * h ? 2 * ffn : 3 * h)));
+    SB_PROPAGATE(llama_alloc(rows, &m->ca, T * (size_t)(ffn > h ? ffn : h)));
+    SB_PROPAGATE(llama_alloc(rows, &m->sca, T));
   }
   m->lora_t = nullptr; m->lora_base = nullptr;
   if (m->lora_r > 0) {
-    SB_PROPAGATE(llama_alloc_row(m, &m->lora_t, T * 3 * (size_t)m->lora_r));
-    SB_PROPAGATE(llama_alloc_row(m, &m->lora_base, T * (size_t)(2 * ffn > h ? 2 * ffn : h)));
+    SB_PROPAGATE(llama_alloc(rows, &m->lora_t, T * 3 * (size_t)m->lora_r));
+    SB_PROPAGATE(llama_alloc(rows, &m->lora_base, T * (size_t)(2 * ffn > h ? 2 * ffn : h)));
   }
-  SB_PROPAGATE(llama_alloc_row(m, &m->da_ws, (size_t)c.max_batch * c.heads * decode_attention_max_splits(c.max_seq) * (128 + 2)));
-  SB_PROPAGATE(llama_alloc_row(m, &m->da_tickets, (size_t)c.max_batch * c.heads));   // zero now, left zero by every launch
+  SB_PROPAGATE(llama_alloc(rows, &m->da_ws, (size_t)c.max_batch * c.heads * decode_attention_max_splits(c.max_seq) * (128 + 2)));
+  SB_PROPAGATE(llama_alloc(rows, &m->da_tickets, (size_t)c.max_batch * c.heads));   // zero now, left zero by every launch
   SB_CHECK_CUDA(cudaMemsetAsync(m->da_tickets, 0, (size_t)c.max_batch * c.heads * sizeof(int), st));
-  SB_PROPAGATE(llama_alloc_row(m, &m->gfinished, (size_t)c.max_batch));
-  SB_PROPAGATE(llama_alloc_row(m, &m->gtok, (size_t)c.max_batch));
-  SB_PROPAGATE(llama_alloc_row(m, &m->gout, (size_t)c.max_batch * c.max_seq));
-  SB_PROPAGATE(llama_alloc_row(m, &m->glogits, (size_t)c.max_batch * m->vpad));
+  SB_PROPAGATE(llama_alloc(rows, &m->gfinished, (size_t)c.max_batch));
+  SB_PROPAGATE(llama_alloc(rows, &m->gtok, (size_t)c.max_batch));
+  SB_PROPAGATE(llama_alloc(rows, &m->gout, (size_t)c.max_batch * c.max_seq));
+  SB_PROPAGATE(llama_alloc(rows, &m->glogits, (size_t)c.max_batch * m->vpad));
   BeamState& b = m->beam;
   const size_t R = (size_t)c.max_batch;
   b.tokens = reinterpret_cast<long long*>(m->gtok);
   b.state = m->gstate;
-  SB_PROPAGATE(llama_alloc_row(m, &b.beam_scores, R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.row_stats, 5 * R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.cand_score, 2 * R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.cand_idx, 2 * R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.slot, R * c.max_seq));
-  SB_PROPAGATE(llama_alloc_row(m, &b.slot_tmp, R * c.max_seq));
-  SB_PROPAGATE(llama_alloc_row(m, &b.hist_tok, R * c.max_seq));
-  SB_PROPAGATE(llama_alloc_row(m, &b.hist_par, R * c.max_seq));
-  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_score, R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_len, R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_beam, R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_step, R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.hyp_n, R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.worst, R));
-  SB_PROPAGATE(llama_alloc_row(m, &b.done, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.beam_scores, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.row_stats, 5 * R));
+  SB_PROPAGATE(llama_alloc(rows, &b.cand_score, 2 * R));
+  SB_PROPAGATE(llama_alloc(rows, &b.cand_idx, 2 * R));
+  SB_PROPAGATE(llama_alloc(rows, &b.slot, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc(rows, &b.slot_tmp, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc(rows, &b.hist_tok, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc(rows, &b.hist_par, R * c.max_seq));
+  SB_PROPAGATE(llama_alloc(rows, &b.hyp_score, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.hyp_len, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.hyp_beam, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.hyp_step, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.hyp_n, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.worst, R));
+  SB_PROPAGATE(llama_alloc(rows, &b.done, R));
   b.max_seq = c.max_seq;
   return 0;
 }
@@ -278,121 +270,79 @@ static int llama_build(seedb200_llama* m) {
   const int64_t h = c.hidden, ffn = c.ffn, V = c.vocab;
   cudaStream_t st = 0;
   char nm[256];
+  // every tensor is checked before anything is allocated
   SB_PROPAGATE(llama_find(m, "model.embed_tokens.weight", &m->embed, V * h));
   SB_PROPAGATE(llama_find(m, "model.norm.weight", &m->norm_w, h));
   SB_PROPAGATE(llama_find(m, "lm_head.weight", &m->lm_head, V * h));
-  if (m->int8) {    // every int8 tensor is checked before anything is allocated
-    for (int l = 0; l < c.layers; ++l)
-      for (int i = 0; i < 7; ++i) {
-        const int64_t N = i == 6 ? h : (i >= 4 ? ffn : h), K = i == 6 ? ffn : h;
-        const int8_t* cb;
-        const float* scb;
-        snprintf(nm, sizeof(nm), "model.layers.%d.%s", l, kI8Lin[i]);
-        SB_PROPAGATE(llama_find_i8(m, nm, N, K, &cb, &scb));
-      }
-  }
-  if (m->quant4) {  // no pre-packed 4-bit names exist: every decoder linear comes through seedb200_llama_4bit_load_weight
+  if (m->fmt == W_4BIT) {  // no pre-packed 4-bit names exist: every decoder linear comes through seedb200_llama_4bit_load_weight
     for (const auto& kv : m->w) {
       int l, i;
-      SB_REQUIRE(!linear_of(kv.first.c_str(), &l, &i), "llama_create_4bit: '%s' is a decoder linear: load it with "
-                 "seedb200_llama_4bit_load_weight", kv.first.c_str());
+      SB_REQUIRE(!linear_of(kv.first.c_str(), ".weight", &l, &i), "llama_create_4bit: '%s' is a decoder linear: load "
+                 "it with seedb200_llama_4bit_load_weight", kv.first.c_str());
     }
   }
-  if (m->int8 || m->quant4) m->q_loaded.assign((size_t)c.layers * 7, 0);
-  m->layers.resize(c.layers);
+  // [layer][linear] the checkpoint's fp16 weight or int8 CB, and the int8 SCB (null: quantised into its rows later)
+  std::vector<const void*> src((size_t)c.layers * 7, nullptr);
+  std::vector<const float*> src_s((size_t)c.layers * 7, nullptr);
+  m->layers.assign(c.layers, LlamaLayerW{});
   for (int l = 0; l < c.layers; ++l) {
     LlamaLayerW& L = m->layers[l];
     auto key = [&](const char* s) { snprintf(nm, sizeof(nm), "model.layers.%d.%s", l, s); return std::string(nm); };
-    const __half *wq, *wk, *wv, *wg, *wu;
     SB_PROPAGATE(llama_find(m, key("input_layernorm.weight"), &L.in_ln, h));
     SB_PROPAGATE(llama_find(m, key("post_attention_layernorm.weight"), &L.post_ln, h));
-    L.qkv_w = L.o_w = L.gu_w = L.down_w = nullptr;
-    L.qkv8 = L.o8 = L.gu8 = L.down8 = nullptr;
-    L.qkv_s = L.o_s = L.gu_s = L.down_s = nullptr;
-    L.qkv4 = L.o4 = L.gu4 = L.down4 = nullptr;
-    L.qkv_a = L.o_a = L.gu_a = L.down_a = nullptr;
-    if (m->quant4) {
-      // handle-owned fused buffers as in int8 mode: packed codes [N, K/2] and absmax [N, K/64]
-      uint8_t *q4, *o4, *g4, *d4;
-      float *qa, *oa, *ga, *da;
-      SB_PROPAGATE(llama_alloc(m, &q4, (size_t)3 * h * h / 2));
-      SB_PROPAGATE(llama_alloc(m, &qa, (size_t)3 * h * h / 64));
-      SB_PROPAGATE(llama_alloc(m, &o4, (size_t)h * h / 2));
-      SB_PROPAGATE(llama_alloc(m, &oa, (size_t)h * h / 64));
-      SB_PROPAGATE(llama_alloc(m, &g4, (size_t)2 * ffn * h / 2));
-      SB_PROPAGATE(llama_alloc(m, &ga, (size_t)2 * ffn * h / 64));
-      SB_PROPAGATE(llama_alloc(m, &d4, (size_t)h * ffn / 2));
-      SB_PROPAGATE(llama_alloc(m, &da, (size_t)h * ffn / 64));
-      L.qkv4 = q4; L.o4 = o4; L.gu4 = g4; L.down4 = d4;
-      L.qkv_a = qa; L.o_a = oa; L.gu_a = ga; L.down_a = da;
-      continue;
-    }
-    if (m->int8) {
-      // handle-owned fused buffers: q|k|v, o, [ffn/128] blocks of [128 gate | 128 up], down; scales alike
-      int8_t *q8, *o8, *g8, *d8;
-      float *qs, *os, *gs, *ds;
-      SB_PROPAGATE(llama_alloc(m, &q8, (size_t)3 * h * h));
-      SB_PROPAGATE(llama_alloc(m, &qs, (size_t)3 * h));
-      SB_PROPAGATE(llama_alloc(m, &o8, (size_t)h * h));
-      SB_PROPAGATE(llama_alloc(m, &os, (size_t)h));
-      SB_PROPAGATE(llama_alloc(m, &g8, (size_t)2 * ffn * h));
-      SB_PROPAGATE(llama_alloc(m, &gs, (size_t)2 * ffn));
-      SB_PROPAGATE(llama_alloc(m, &d8, (size_t)h * ffn));
-      SB_PROPAGATE(llama_alloc(m, &ds, (size_t)h));
-      L.qkv8 = q8; L.o8 = o8; L.gu8 = g8; L.down8 = d8;
-      L.qkv_s = qs; L.o_s = os; L.gu_s = gs; L.down_s = ds;
-      for (int i = 0; i < 7; ++i) {
-        const QSlot t = q_slot(m, l, i);
+    for (int i = 0; i < 7; ++i) {
+      const Fused F = fused(m, kLinear[i].g);
+      const int64_t N = F.N / F.nsub, K = F.K;
+      const size_t j = (size_t)l * 7 + i;
+      if (m->fmt == W_F16) {
+        const __half* w;
+        SB_PROPAGATE(llama_find(m, key(kLinear[i].name) + ".weight", &w, N * K));
+        src[j] = w;
+      } else if (m->fmt == W_INT8) {
         const int8_t* cb;
-        const float* scb;
-        SB_PROPAGATE(llama_find_i8(m, key(kI8Lin[i]), t.N, t.K, &cb, &scb));
-        if (cb == nullptr) continue;     // quantised into its slot later
-        const int64_t blocks = t.N / t.grp, dst_rows = t.grp == t.N ? t.N : t.gstride;
-        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.w + t.off * t.K, (size_t)(dst_rows * t.K), cb, (size_t)(t.grp * t.K),
-                                        (size_t)(t.grp * t.K), (size_t)blocks, cudaMemcpyDeviceToDevice, st));
-        SB_CHECK_CUDA(cudaMemcpy2DAsync(t.s + t.off, (size_t)(dst_rows * 4), scb, (size_t)(t.grp * 4),
-                                        (size_t)(t.grp * 4), (size_t)blocks, cudaMemcpyDeviceToDevice, st));
-        m->q_loaded[(size_t)l * 7 + i] = 1;
+        SB_PROPAGATE(llama_find_i8(m, key(kLinear[i].name), N, K, &cb, &src_s[j]));
+        src[j] = cb;
       }
-      continue;
     }
-    SB_PROPAGATE(llama_find(m, key("self_attn.q_proj.weight"), &wq, h * h));
-    SB_PROPAGATE(llama_find(m, key("self_attn.k_proj.weight"), &wk, h * h));
-    SB_PROPAGATE(llama_find(m, key("self_attn.v_proj.weight"), &wv, h * h));
-    SB_PROPAGATE(llama_find(m, key("self_attn.o_proj.weight"), &L.o_w, h * h));
-    SB_PROPAGATE(llama_find(m, key("mlp.gate_proj.weight"), &wg, ffn * h));
-    SB_PROPAGATE(llama_find(m, key("mlp.up_proj.weight"), &wu, ffn * h));
-    SB_PROPAGATE(llama_find(m, key("mlp.down_proj.weight"), &L.down_w, h * ffn));
-    __half *fq, *fg;
-    SB_PROPAGATE(llama_alloc(m, &fq, (size_t)3 * h * h));
-    SB_CHECK_CUDA(cudaMemcpyAsync(fq, wq, (size_t)h * h * 2, cudaMemcpyDeviceToDevice, st));
-    SB_CHECK_CUDA(cudaMemcpyAsync(fq + (size_t)h * h, wk, (size_t)h * h * 2, cudaMemcpyDeviceToDevice, st));
-    SB_CHECK_CUDA(cudaMemcpyAsync(fq + (size_t)2 * h * h, wv, (size_t)h * h * 2, cudaMemcpyDeviceToDevice, st));
-    L.qkv_w = fq;
-    // [ffn/128] blocks of [128 gate rows | 128 up rows]
-    SB_PROPAGATE(llama_alloc(m, &fg, (size_t)2 * ffn * h));
-    const size_t blk = (size_t)128 * h * 2;
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(fg, 2 * blk, wg, blk, blk, ffn / 128, cudaMemcpyDeviceToDevice, st));
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(reinterpret_cast<uint8_t*>(fg) + blk, 2 * blk, wu, blk, blk, ffn / 128,
-                                    cudaMemcpyDeviceToDevice, st));
-    L.gu_w = fg;
   }
+  // then the fused linears: handle-owned buffers filled with the checkpoint's rows
+  if (m->fmt != W_F16) m->q_loaded.assign((size_t)c.layers * 7, 0);
+  for (int l = 0; l < c.layers; ++l)
+    for (int g = 0; g < 4; ++g) {
+      const Fused F = fused(m, g);
+      const bool borrow = m->fmt == W_F16 && F.nsub == 1;   // fp16 o and down are used (and LoRA-merged) in place
+      size_t wrow, srow;
+      row_bytes(m, F.K, &wrow, &srow);
+      uint8_t* w = nullptr;
+      float* s = nullptr;
+      if (!borrow) SB_PROPAGATE(llama_alloc(m->owned, &w, (size_t)F.N * wrow));
+      if (srow > 0) SB_PROPAGATE(llama_alloc(m->owned, &s, (size_t)F.N * srow / 4));
+      m->layers[l].lin[g] = {w, s};
+      for (int i = 0; i < 7; ++i) {
+        const size_t j = (size_t)l * 7 + i;
+        if (kLinear[i].g != g || src[j] == nullptr) continue;
+        if (borrow) m->layers[l].lin[g].w = src[j];
+        else SB_PROPAGATE(place_rows(w, src[j], wrow, F, kLinear[i].sub, st));
+        if (s) SB_PROPAGATE(place_rows(s, src_s[j], srow, F, kLinear[i].sub, st));
+        if (m->fmt != W_F16) m->q_loaded[j] = 1;
+      }
+    }
   SB_PROPAGATE(get_rope_tables(c.head_dim, c.rope_base, c.max_seq, &m->cos_t, &m->sin_t, &m->max_pos, st));
   m->q4_scratch = nullptr;
-  if (m->quant4) {   // allocated here so that peak memory does not depend on the first prefill
+  if (m->fmt == W_4BIT) {   // allocated here so that peak memory does not depend on the first prefill
     const size_t qkv = (size_t)3 * h * h, gu = (size_t)2 * ffn * h;
-    SB_PROPAGATE(llama_alloc(m, &m->q4_scratch, qkv > gu ? qkv : gu));
+    SB_PROPAGATE(llama_alloc(m->owned, &m->q4_scratch, qkv > gu ? qkv : gu));
   }
   m->olist = nullptr; m->ocount = nullptr;
-  if (m->int8) {
-    SB_PROPAGATE(llama_alloc(m, &m->olist, (size_t)(ffn > h ? ffn : h)));
-    SB_PROPAGATE(llama_alloc(m, &m->ocount, 1));
+  if (m->fmt == W_INT8) {
+    SB_PROPAGATE(llama_alloc(m->owned, &m->olist, (size_t)(ffn > h ? ffn : h)));
+    SB_PROPAGATE(llama_alloc(m->owned, &m->ocount, 1));
   }
   m->vpad = (c.vocab + 7) / 8 * 8;
-  SB_PROPAGATE(llama_alloc(m, &m->gstate, 8));
-  SB_PROPAGATE(llama_alloc(m, &m->gparams, 1));
-  SB_PROPAGATE(llama_alloc(m, &m->beam.params, 1));
-  SB_PROPAGATE(llama_alloc(m, &m->beam.n_out, 1));
+  SB_PROPAGATE(llama_alloc(m->owned, &m->gstate, 8));
+  SB_PROPAGATE(llama_alloc(m->owned, &m->gparams, 1));
+  SB_PROPAGATE(llama_alloc(m->owned, &m->beam.params, 1));
+  SB_PROPAGATE(llama_alloc(m->owned, &m->beam.n_out, 1));
   SB_PROPAGATE(llama_alloc_rows(m, st));
   SB_CHECK_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->gstate_host), 8 * sizeof(int)));
   SB_CHECK_CUDA(cudaStreamCreateWithFlags(&m->gstream, cudaStreamNonBlocking));
@@ -402,31 +352,24 @@ static int llama_build(seedb200_llama* m) {
 
 int get_option(const char* key);
 
-static int lin(cudaStream_t st, int ctas, int M, int N, int K, const void* A, const void* W, void* out, int64_t ldo,
-               const void* residual, int mode, const void* norm_w = nullptr, float eps = 0.0f) {
-  // norm_w: only on the M <= 4 (decode) path, where the GEMV normalises its activations while staging them
-  if (M <= 4) return gemv(A, W, K, out, residual, norm_w, eps, M, N, K, mode, st, ldo);
+static seedb200_gemm_desc gemm_desc(int ctas, int M, int N, int K, const void* A, const void* W, void* out, int64_t ldo,
+                                    const void* residual, int mode) {
   seedb200_gemm_desc d;
   memset(&d, 0, sizeof(d));
   d.M = M; d.N = N; d.K = K; d.A = A; d.lda = K; d.W = W; d.ldw = K;
   d.out = out; d.ldo = ldo; d.residual = residual; d.ldr = ldo; d.mode = mode; d.ctas = ctas;
-  return gemm(d, st);
+  return d;
 }
 
-// shape of fused linear g of a layer in the LoRA adapter: N x K, sub-blocks of grp rows cycling over nsub adapters
-struct LoraGeom { int N, K, grp, nsub; };
-static LoraGeom lora_geom(const seedb200_llama* m, int g) {
-  const int h = m->cfg.hidden, ffn = m->cfg.ffn;
-  if (g == 0) return {3 * h, h, h, 3};
-  if (g == 1) return {h, h, h, 1};
-  if (g == 2) return {2 * ffn, h, 128, 2};
-  return {h, ffn, h, 1};
+static int lin(cudaStream_t st, int ctas, int M, int N, int K, const void* A, const void* W, void* out, int64_t ldo,
+               const void* residual, int mode, const void* norm_w = nullptr, float eps = 0.0f) {
+  // norm_w: only on the M <= 4 (decode) path, where the GEMV normalises its activations while staging them
+  if (M <= 4) return gemv(A, W, K, out, residual, norm_w, eps, M, N, K, mode, st, ldo);
+  return gemm(gemm_desc(ctas, M, N, K, A, W, out, ldo, residual, mode), st);
 }
-// decoder linear i (kI8Lin order) -> (fused linear, sub-block)
-static const int kLoraGroup[7] = {0, 0, 0, 1, 2, 2, 3}, kLoraSub[7] = {0, 1, 2, 0, 0, 1, 0};
 
 static seedb200_lora_operand lora_operand(const seedb200_llama* m, int l, int g, void* workspace) {
-  const LoraGeom G = lora_geom(m, g);
+  const Fused G = fused(m, g);
   seedb200_lora_operand lo;
   memset(&lo, 0, sizeof(lo));
   lo.T = m->lora_t; lo.ldt = (int64_t)G.nsub * m->lora_r; lo.B = m->lora[l].B[g];
@@ -435,50 +378,48 @@ static seedb200_lora_operand lora_operand(const seedb200_llama* m, int l, int g,
   return lo;
 }
 
-// fp16 decoder linear g of layer l: lin(), plus the adapter's LoRA branch when one covers this linear (lin4() on a
-// 4-bit handle)
-// 4-bit decoder linear g of layer l: the 4-bit GEMV for M <= 4 (norm folded as lin() folds it), otherwise the fused
-// weight is dequantised into the scratch and lin() runs on it (MatMul4Bit's dequantise-then-linear).
-static int lin4(seedb200_llama* m, cudaStream_t st, int l, int g, int M, int N, int K, const void* A, void* out,
-                int64_t ldo, const void* residual, int mode, const void* norm_w, float eps) {
-  const LlamaLayerW& L = m->layers[l];
-  const uint8_t* P[4] = {L.qkv4, L.o4, L.gu4, L.down4};
-  const float* S[4] = {L.qkv_a, L.o_a, L.gu_a, L.down_a};
-  if (M <= 4) return gemv_4bit(A, norm_w, eps, P[g], S[g], m->q4type, out, residual, M, N, K, mode, st);
-  SB_PROPAGATE(dequantize_4bit(P[g], S[g], N, K, m->q4type, m->q4_scratch, K, st));
-  return lin(st, m->cfg.gemm_ctas, M, N, K, A, m->q4_scratch, out, ldo, residual, mode);
-}
-
-static int lin_lora(seedb200_llama* m, cudaStream_t st, int l, int g, int M, int N, int K, const void* A,
-                    const void* W, void* out, int64_t ldo, const void* residual, int mode,
-                    const void* norm_w = nullptr, float eps = 0.0f) {
-  if (m->quant4) return lin4(m, st, l, g, M, N, K, A, out, ldo, residual, mode, norm_w, eps);
+// Fused decoder linear g of layer l on M rows of A, in the handle's weight format, plus the adapter's LoRA branch when
+// one covers g.  Outputs are dense rows of N columns (N/2 in mode 1: SiLU(gate) * up).  norm_w: only for M <= 4, where
+// the GEMV normalises its activations while staging them.
+static int decoder_linear(seedb200_llama* m, cudaStream_t st, int l, int g, int M, const void* A, void* out,
+                          const void* residual, int mode, const void* norm_w = nullptr, float eps = 0.0f) {
+  const Fused F = fused(m, g);
+  const LinW& W = m->layers[l].lin[g];
+  const int64_t ldo = mode == 1 ? F.N / 2 : F.N;
+  const int ctas = m->cfg.gemm_ctas;
+  if (m->fmt == W_INT8) {   // more rows: activation quantisation + int8 wgmma GEMM
+    if (M <= 4) return gemv_int8(A, norm_w, eps, m->threshold, W.w, W.s, out, residual, M, F.N, F.K, mode, st);
+    SB_PROPAGATE(int8_quantize_act(A, F.K, M, F.K, m->threshold, m->ca, m->sca, m->olist, m->ocount, st));
+    seedb200_gemm_int8_desc d;
+    memset(&d, 0, sizeof(d));
+    d.M = M; d.N = F.N; d.K = F.K;
+    d.A = m->ca; d.SCA = m->sca; d.A16 = A; d.outliers = m->olist; d.n_outliers = m->ocount;
+    d.W = W.w; d.SCB = W.s; d.out = out; d.residual = residual; d.mode = mode; d.workspace = m->corr;
+    return gemm_int8(d, st);
+  }
+  if (m->fmt == W_4BIT) {   // more rows: MatMul4Bit's dequantise-then-linear, through the fp16 scratch
+    if (M <= 4) return gemv_4bit(A, norm_w, eps, W.w, W.s, m->q4type, out, residual, M, F.N, F.K, mode, st);
+    SB_PROPAGATE(dequantize_4bit(W.w, W.s, F.N, F.K, m->q4type, m->q4_scratch, F.K, st));
+    return lin(st, ctas, M, F.N, F.K, A, m->q4_scratch, out, ldo, residual, mode);
+  }
   if (m->lora_r == 0 || m->lora_mask[g] == 0)
-    return lin(st, m->cfg.gemm_ctas, M, N, K, A, W, out, ldo, residual, mode, norm_w, eps);
+    return lin(st, ctas, M, F.N, F.K, A, W.w, out, ldo, residual, mode, norm_w, eps);
   const seedb200_lora_operand lo =
       lora_operand(m, l, g, mode == 0 && residual == nullptr ? nullptr : static_cast<void*>(m->lora_base));
-  SB_PROPAGATE(lora_shrink(A, K, norm_w, eps, m->lora[l].A[g], M, K, (int)lo.ldt, m->lora_t, lo.ldt, st));
-  if (M <= 4) return gemv_lora(A, W, K, out, residual, norm_w, eps, M, N, K, mode, lo, st, ldo);
-  seedb200_gemm_desc d;
-  memset(&d, 0, sizeof(d));
-  d.M = M; d.N = N; d.K = K; d.A = A; d.lda = K; d.W = W; d.ldw = K;
-  d.out = out; d.ldo = ldo; d.residual = residual; d.ldr = ldo; d.mode = mode; d.ctas = m->cfg.gemm_ctas;
-  return gemm_lora(d, lo, st);
+  SB_PROPAGATE(lora_shrink(A, F.K, norm_w, eps, m->lora[l].A[g], M, F.K, (int)lo.ldt, m->lora_t, lo.ldt, st));
+  if (M <= 4) return gemv_lora(A, W.w, F.K, out, residual, norm_w, eps, M, F.N, F.K, mode, lo, st, ldo);
+  return gemm_lora(gemm_desc(ctas, M, F.N, F.K, A, W.w, out, ldo, residual, mode), lo, st);
 }
 
-// int8 decoder linear: GEMV for M <= 4 (with the RMSNorm folded in when norm_w is given), otherwise activation
-// quantisation + int8 wgmma GEMM.  Outputs are dense rows of N (N/2 in mode 1) columns.
-static int lin8(seedb200_llama* m, cudaStream_t st, int M, int N, int K, const void* A, const int8_t* W,
-                const float* scb, void* out, const void* residual, int mode, const void* norm_w = nullptr,
-                float eps = 0.0f) {
-  if (M <= 4) return gemv_int8(A, norm_w, eps, m->threshold, W, scb, out, residual, M, N, K, mode, st);
-  SB_PROPAGATE(int8_quantize_act(A, K, M, K, m->threshold, m->ca, m->sca, m->olist, m->ocount, st));
-  seedb200_gemm_int8_desc d;
-  memset(&d, 0, sizeof(d));
-  d.M = M; d.N = N; d.K = K;
-  d.A = m->ca; d.SCA = m->sca; d.A16 = A; d.outliers = m->olist; d.n_outliers = m->ocount;
-  d.W = W; d.SCB = scb; d.out = out; d.residual = residual; d.mode = mode; d.workspace = m->corr;
-  return gemm_int8(d, st);
+// decoder linear g on RMSNorm(m->x) with weight norm_w: folded into the GEMV for T <= 4 rows, otherwise normalised
+// into m->nb first
+static int normed_linear(seedb200_llama* m, cudaStream_t st, int l, int g, int T, const __half* norm_w, void* out,
+                         int mode) {
+  const int h = m->cfg.hidden;
+  const float eps = m->cfg.rms_eps;
+  if (T <= 4) return decoder_linear(m, st, l, g, T, m->x, out, nullptr, mode, norm_w, eps);
+  SB_PROPAGATE(rmsnorm(m->x, h, norm_w, m->nb, h, T, h, eps, st));
+  return decoder_linear(m, st, l, g, T, m->nb, out, nullptr, mode);
 }
 
 // dyn (device, optional): {cache length, ...} read by the RoPE/append and decode-attention kernels instead of the
@@ -487,7 +428,7 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
                          const int64_t* position_ids, int B, int S, int past_len, int logits_mode, void* logits,
                          int64_t logits_ld, cudaStream_t st, const int* dyn = nullptr, const int* slot = nullptr) {
   const seedb200_llama_config& c = m->cfg;
-  const int h = c.hidden, H = c.heads, D = c.head_dim, ffn = c.ffn, V = c.vocab, ct = c.gemm_ctas;
+  const int h = c.hidden, H = c.heads, D = c.head_dim, V = c.vocab, ct = c.gemm_ctas;
   const int T = B * S;
   if (input_ids)
     SB_PROPAGATE(embedding(m->embed, h, input_ids, T, h, m->x, h, V, st));
@@ -495,24 +436,11 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
     SB_CHECK_CUDA(cudaMemcpyAsync(m->x, inputs_embeds, (size_t)T * h * 2, cudaMemcpyDeviceToDevice, st));
   const float scale = 1.0f / sqrtf((float)D);   // xformers default scale
   const int kv_len = past_len + S;
-  const bool fuse_norm = T <= 4;     // decode: RMSNorm folded into the GEMV that consumes it
   PdlScope pdl(T <= 4 && get_option("decode_pdl") != 0);   // decode chain: programmatic dependent launches
   const bool fused_attn = S == 1 && get_option("decode_fused_attention") != 0 && decode_attention_rope_supported(D, c.max_seq);
   for (int l = 0; l < c.layers; ++l) {
     const LlamaLayerW& L = m->layers[l];
-    if (m->int8) {
-      if (fuse_norm) {
-        SB_PROPAGATE(lin8(m, st, T, 3 * h, h, m->x, L.qkv8, L.qkv_s, m->qkv, nullptr, 0, L.in_ln, c.rms_eps));
-      } else {
-        SB_PROPAGATE(rmsnorm(m->x, h, L.in_ln, m->nb, h, T, h, c.rms_eps, st));
-        SB_PROPAGATE(lin8(m, st, T, 3 * h, h, m->nb, L.qkv8, L.qkv_s, m->qkv, nullptr, 0));
-      }
-    } else if (fuse_norm) {
-      SB_PROPAGATE(lin_lora(m, st, l, 0, T, 3 * h, h, m->x, L.qkv_w, m->qkv, 3 * h, nullptr, 0, L.in_ln, c.rms_eps));
-    } else {
-      SB_PROPAGATE(rmsnorm(m->x, h, L.in_ln, m->nb, h, T, h, c.rms_eps, st));
-      SB_PROPAGATE(lin_lora(m, st, l, 0, T, 3 * h, h, m->nb, L.qkv_w, m->qkv, 3 * h, nullptr, 0));
-    }
+    SB_PROPAGATE(normed_linear(m, st, l, 0, T, L.in_ln, m->qkv, 0));
     // qkv rows are [q | k | v] per token, each [H, D]
     if (fused_attn) {
       // cached decode step: RoPE + append + attention in one launch (bit-identical to the pair below up to 512 keys)
@@ -536,25 +464,9 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
       SB_PROPAGATE(attention(a, st));
     }
     }
-    if (m->int8) {
-      SB_PROPAGATE(lin8(m, st, T, h, h, m->att, L.o8, L.o_s, m->x, m->x, 0));
-      if (fuse_norm) {
-        SB_PROPAGATE(lin8(m, st, T, 2 * ffn, h, m->x, L.gu8, L.gu_s, m->gu, nullptr, 1, L.post_ln, c.rms_eps));
-      } else {
-        SB_PROPAGATE(rmsnorm(m->x, h, L.post_ln, m->nb, h, T, h, c.rms_eps, st));
-        SB_PROPAGATE(lin8(m, st, T, 2 * ffn, h, m->nb, L.gu8, L.gu_s, m->gu, nullptr, 1));
-      }
-      SB_PROPAGATE(lin8(m, st, T, h, ffn, m->gu, L.down8, L.down_s, m->x, m->x, 0));
-      continue;
-    }
-    SB_PROPAGATE(lin_lora(m, st, l, 1, T, h, h, m->att, L.o_w, m->x, h, m->x, 0));
-    if (fuse_norm) {
-      SB_PROPAGATE(lin_lora(m, st, l, 2, T, 2 * ffn, h, m->x, L.gu_w, m->gu, ffn, nullptr, 1, L.post_ln, c.rms_eps));
-    } else {
-      SB_PROPAGATE(rmsnorm(m->x, h, L.post_ln, m->nb, h, T, h, c.rms_eps, st));
-      SB_PROPAGATE(lin_lora(m, st, l, 2, T, 2 * ffn, h, m->nb, L.gu_w, m->gu, ffn, nullptr, 1));
-    }
-    SB_PROPAGATE(lin_lora(m, st, l, 3, T, h, ffn, m->gu, L.down_w, m->x, h, m->x, 0));
+    SB_PROPAGATE(decoder_linear(m, st, l, 1, T, m->att, m->x, m->x, 0));
+    SB_PROPAGATE(normed_linear(m, st, l, 2, T, L.post_ln, m->gu, 1));
+    SB_PROPAGATE(decoder_linear(m, st, l, 3, T, m->gu, m->x, m->x, 0));
   }
   SB_PROPAGATE(rmsnorm(m->x, h, m->norm_w, m->hn, h, T, h, c.rms_eps, st));
   m->last_T = T;
@@ -748,14 +660,36 @@ static void llama_drop_graphs(seedb200_llama* m) {
 static int llama_linears_ready(const seedb200_llama* m) {
   for (size_t i = 0; i < m->q_loaded.size(); ++i)
     if (!m->q_loaded[i]) {
-      if (m->quant4)
+      if (m->fmt == W_4BIT)
         set_error("llama: 4-bit weight 'model.layers.%d.%s.weight' has not been loaded (seedb200_llama_4bit_load_weight)",
-                  (int)(i / 7), kI8Lin[i % 7]);
+                  (int)(i / 7), kLinear[i % 7].name);
       else
         set_error("llama: int8 weight 'model.layers.%d.%s.weight' was neither given to create_int8 nor loaded",
-                  (int)(i / 7), kI8Lin[i % 7]);
+                  (int)(i / 7), kLinear[i % 7].name);
       return SEEDB200_ERR_INVALID;
     }
+  return 0;
+}
+
+// seedb200_llama_{int8,4bit}_load_weight: quantise the fp16 decoder linear `name` ([N, K], rows ldw apart) into its
+// rows of the handle's fused linear
+static int load_quantised(seedb200_llama* m, const char* who, const char* name, const void* W, int64_t ldw,
+                          cudaStream_t st) {
+  int layer = -1, i = -1;
+  SB_REQUIRE(linear_of(name, ".weight", &layer, &i) && layer >= 0 && layer < (int)m->layers.size(),
+             "%s: '%s' is not a decoder linear of this model", who, name);
+  const Fused F = fused(m, kLinear[i].g);
+  const int N = F.N / F.nsub, K = F.K, grp = F.grp, gstride = F.grp * F.nsub, off = kLinear[i].sub * F.grp;
+  if (ldw == 0) ldw = K;
+  SB_REQUIRE(ldw >= K, "%s: ldw %lld below K %lld", who, (long long)ldw, (long long)K);
+  void* w = const_cast<void*>(m->layers[layer].lin[kLinear[i].g].w);
+  float* s = const_cast<float*>(m->layers[layer].lin[kLinear[i].g].s);
+  DeviceGuard guard(m->device);
+  if (m->fmt == W_INT8)
+    SB_PROPAGATE(int8_quantize_weight_rows(W, ldw, N, K, w, s, grp, gstride, off, st));
+  else
+    SB_PROPAGATE(quantize_4bit_rows(W, ldw, N, K, m->q4type, w, s, grp, gstride, off, st));
+  m->q_loaded[(size_t)layer * 7 + i] = 1;
   return 0;
 }
 
@@ -763,9 +697,9 @@ static int llama_linears_ready(const seedb200_llama* m) {
 
 extern "C" {
 
-// q4type: -1 = no 4-bit linears
-static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights, int int8,
-                        float threshold, int q4type, seedb200_llama** out) {
+// threshold: int8 only; q4type: 4-bit only (-1 otherwise)
+static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
+                        sb::WeightFormat fmt, float threshold, int q4type, seedb200_llama** out) {
   if (!cfg || !weights || !out) {
     sb::set_error("llama_create: null argument");
     return SEEDB200_ERR_INVALID;
@@ -786,9 +720,8 @@ static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor*
   m->used_graph = -1;
   m->gen_cache_len = 0;
   memset(&m->beam, 0, sizeof(m->beam));
-  m->int8 = int8;
+  m->fmt = fmt;
   m->threshold = threshold;
-  m->quant4 = q4type >= 0;
   m->q4type = q4type;
   m->lora_r = 0;
   m->lora_s = 0.0f;
@@ -807,14 +740,14 @@ static int llama_create(const seedb200_llama_config* cfg, const seedb200_tensor*
 
 int seedb200_llama_create(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
                           seedb200_llama** out) {
-  return llama_create(cfg, weights, n_weights, 0, 0.0f, -1, out);
+  return llama_create(cfg, weights, n_weights, sb::W_F16, 0.0f, -1, out);
 }
 
 int seedb200_llama_create_int8(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
                                float threshold, seedb200_llama** out) {
   SB_REQUIRE(threshold > 0.0f, "llama_create_int8: threshold must be > 0 (got %g)", (double)threshold);
   SB_REQUIRE(cfg == nullptr || cfg->hidden % 16 == 0, "llama_create_int8: hidden must be a multiple of 16");
-  return llama_create(cfg, weights, n_weights, 1, threshold, -1, out);
+  return llama_create(cfg, weights, n_weights, sb::W_INT8, threshold, -1, out);
 }
 
 int seedb200_llama_create_4bit(const seedb200_llama_config* cfg, const seedb200_tensor* weights, int n_weights,
@@ -824,39 +757,19 @@ int seedb200_llama_create_4bit(const seedb200_llama_config* cfg, const seedb200_
   SB_REQUIRE(cfg == nullptr || (cfg->hidden % 64 == 0 && cfg->ffn % 64 == 0),
              "llama_create_4bit: hidden %d and ffn %d must be multiples of the 4-bit blocksize 64",
              cfg ? cfg->hidden : 0, cfg ? cfg->ffn : 0);
-  return llama_create(cfg, weights, n_weights, 0, 0.0f, quant_type, out);
+  return llama_create(cfg, weights, n_weights, sb::W_4BIT, 0.0f, quant_type, out);
 }
 
 int seedb200_llama_int8_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream) {
   SB_REQUIRE(llm && name && W, "llama_int8_load_weight: null argument");
-  SB_REQUIRE(llm->int8, "llama_int8_load_weight: the handle was not made by seedb200_llama_create_int8");
-  int layer = -1, i = -1;
-  SB_REQUIRE(sb::linear_of(name, &layer, &i) && layer >= 0 && layer < (int)llm->layers.size(),
-             "llama_int8_load_weight: '%s' is not a decoder linear of this model", name);
-  const sb::QSlot t = sb::q_slot(llm, layer, i);
-  if (ldw == 0) ldw = t.K;
-  SB_REQUIRE(ldw >= t.K, "llama_int8_load_weight: ldw %lld below K %lld", (long long)ldw, (long long)t.K);
-  sb::DeviceGuard guard(llm->device);
-  SB_PROPAGATE(sb::int8_quantize_weight_rows(W, ldw, (int)t.N, (int)t.K, t.w, t.s, (int)t.grp, (int)t.gstride,
-                                             (int)t.off, static_cast<cudaStream_t>(stream)));
-  llm->q_loaded[(size_t)layer * 7 + i] = 1;
-  return 0;
+  SB_REQUIRE(llm->fmt == sb::W_INT8, "llama_int8_load_weight: the handle was not made by seedb200_llama_create_int8");
+  return sb::load_quantised(llm, "llama_int8_load_weight", name, W, ldw, static_cast<cudaStream_t>(stream));
 }
 
 int seedb200_llama_4bit_load_weight(seedb200_llama* llm, const char* name, const void* W, int64_t ldw, void* stream) {
   SB_REQUIRE(llm && name && W, "llama_4bit_load_weight: null argument");
-  SB_REQUIRE(llm->quant4, "llama_4bit_load_weight: the handle was not made by seedb200_llama_create_4bit");
-  int layer = -1, i = -1;
-  SB_REQUIRE(sb::linear_of(name, &layer, &i) && layer >= 0 && layer < (int)llm->layers.size(),
-             "llama_4bit_load_weight: '%s' is not a decoder linear of this model", name);
-  const sb::QSlot t = sb::q_slot(llm, layer, i);
-  if (ldw == 0) ldw = t.K;
-  SB_REQUIRE(ldw >= t.K, "llama_4bit_load_weight: ldw %lld below K %lld", (long long)ldw, (long long)t.K);
-  sb::DeviceGuard guard(llm->device);
-  SB_PROPAGATE(sb::quantize_4bit_rows(W, ldw, (int)t.N, (int)t.K, llm->q4type, t.w, t.s, (int)t.grp, (int)t.gstride,
-                                      (int)t.off, static_cast<cudaStream_t>(stream)));
-  llm->q_loaded[(size_t)layer * 7 + i] = 1;
-  return 0;
+  SB_REQUIRE(llm->fmt == sb::W_4BIT, "llama_4bit_load_weight: the handle was not made by seedb200_llama_create_4bit");
+  return sb::load_quantised(llm, "llama_4bit_load_weight", name, W, ldw, static_cast<cudaStream_t>(stream));
 }
 
 void seedb200_llama_destroy(seedb200_llama* llm) {
@@ -988,8 +901,8 @@ extern "C" {
 
 int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors, int n, int r, float alpha) {
   SB_REQUIRE(llm && (tensors || n == 0), "llama_lora_load: null argument");
-  SB_REQUIRE(!llm->int8, "llama_lora_load: LoRA on an int8 (load_in_8bit) model is not supported");
-  SB_REQUIRE(!llm->quant4, "llama_lora_load: LoRA on a 4-bit (load_in_4bit) model is not supported");
+  SB_REQUIRE(llm->fmt != sb::W_INT8, "llama_lora_load: LoRA on an int8 (load_in_8bit) model is not supported");
+  SB_REQUIRE(llm->fmt != sb::W_4BIT, "llama_lora_load: LoRA on a 4-bit (load_in_4bit) model is not supported");
   SB_REQUIRE(r >= 1 && r <= sb::LORA_MAX_R, "llama_lora_load: r %d outside [1,%d]", r, sb::LORA_MAX_R);
   SB_REQUIRE(alpha == alpha && alpha > -1e30f && alpha < 1e30f, "llama_lora_load: lora_alpha must be finite");
   const int nl = (int)llm->layers.size();
@@ -997,17 +910,11 @@ int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors
   for (int t = 0; t < n; ++t) {
     const seedb200_tensor& x = tensors[t];
     SB_REQUIRE(x.name != nullptr, "llama_lora_load: tensor %d has no name", t);
-    int layer = -1, lin = -1, ab = -1;
-    for (int i = 0; i < 7 && lin < 0; ++i)
-      for (int k = 0; k < 2 && lin < 0; ++k) {
-        char tail[96];
-        snprintf(tail, sizeof(tail), ".%s.lora_%c.weight", sb::kI8Lin[i], k ? 'B' : 'A');
-        int l = -1, c = 0;
-        if (sscanf(x.name, "model.layers.%d%n", &l, &c) == 1 && strcmp(x.name + c, tail) == 0) { layer = l; lin = i; ab = k; }
-      }
-    SB_REQUIRE(lin >= 0, "llama_lora_load: '%s' is not a lora_A / lora_B of a decoder linear", x.name);
+    int layer = -1, lin = -1, ab = 0;
+    while (ab < 2 && !sb::linear_of(x.name, ab ? ".lora_B.weight" : ".lora_A.weight", &layer, &lin)) ++ab;
+    SB_REQUIRE(ab < 2, "llama_lora_load: '%s' is not a lora_A / lora_B of a decoder linear", x.name);
     SB_REQUIRE(layer >= 0 && layer < nl, "llama_lora_load: '%s': the model has %d layers", x.name, nl);
-    const sb::LoraGeom G = sb::lora_geom(llm, sb::kLoraGroup[lin]);
+    const sb::Fused G = sb::fused(llm, sb::kLinear[lin].g);
     const int64_t N = G.N / G.nsub, K = G.K;
     const bool ok = ab == 0 ? sb::tensor_is(x, r, K) : sb::tensor_is(x, N, r);
     SB_REQUIRE(ok, "llama_lora_load: '%s' must be fp16, 16-byte aligned, [%lld, %lld] (dtype %d, ndim %d)", x.name,
@@ -1021,7 +928,7 @@ int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors
     int here = 0;
     for (int i = 0; i < 7; ++i) {
       const bool a = found[((size_t)l * 7 + i) * 2] != nullptr, b = found[((size_t)l * 7 + i) * 2 + 1] != nullptr;
-      SB_REQUIRE(a == b, "llama_lora_load: model.layers.%d.%s has lora_%c without lora_%c", l, sb::kI8Lin[i],
+      SB_REQUIRE(a == b, "llama_lora_load: model.layers.%d.%s has lora_%c without lora_%c", l, sb::kLinear[i].name,
                  a ? 'A' : 'B', a ? 'B' : 'A');
       if (a) here |= 1 << i;
     }
@@ -1035,7 +942,7 @@ int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors
   sb::lora_free(llm);
   size_t per_layer = 0;
   for (int g = 0; g < 4; ++g) {
-    const sb::LoraGeom G = sb::lora_geom(llm, g);
+    const sb::Fused G = sb::fused(llm, g);
     per_layer += (size_t)G.nsub * r * G.K + (size_t)G.N * r;
   }
   SB_CHECK_CUDA(cudaMalloc(&llm->lora_mem, per_layer * nl * 2 + 256));
@@ -1045,37 +952,28 @@ int seedb200_llama_lora_load(seedb200_llama* llm, const seedb200_tensor* tensors
   __half* p = static_cast<__half*>(llm->lora_mem);
   for (int l = 0; l < nl; ++l)
     for (int g = 0; g < 4; ++g) {
-      const sb::LoraGeom G = sb::lora_geom(llm, g);
+      const sb::Fused G = sb::fused(llm, g);
       llm->lora[l].A[g] = p; p += (size_t)G.nsub * r * G.K;
       llm->lora[l].B[g] = p; p += (size_t)G.N * r;
     }
   for (int l = 0; l < nl; ++l)
     for (int i = 0; i < 7; ++i) {
       if (!((targets >> i) & 1)) continue;
-      const int g = sb::kLoraGroup[i], sub = sb::kLoraSub[i];
-      const sb::LoraGeom G = sb::lora_geom(llm, g);
+      const int g = sb::kLinear[i].g, sub = sb::kLinear[i].sub;
+      const sb::Fused G = sb::fused(llm, g);
       const seedb200_tensor* A = found[((size_t)l * 7 + i) * 2];
       const seedb200_tensor* B = found[((size_t)l * 7 + i) * 2 + 1];
       __half* a_dst = const_cast<__half*>(llm->lora[l].A[g]) + (size_t)sub * r * G.K;
-      __half* b_dst = const_cast<__half*>(llm->lora[l].B[g]);
       SB_CHECK_CUDA(cudaMemcpyAsync(a_dst, A->data, (size_t)r * G.K * 2, cudaMemcpyDeviceToDevice, st));
-      const int64_t rows = G.N / G.nsub;
-      if (g == 2) {   // gate|up: [ffn/128] blocks of [128 gate rows | 128 up rows]
-        const size_t blk = (size_t)128 * r * 2;
-        SB_CHECK_CUDA(cudaMemcpy2DAsync(reinterpret_cast<uint8_t*>(b_dst) + sub * blk, 2 * blk, B->data, blk, blk,
-                                        (size_t)rows / 128, cudaMemcpyDeviceToDevice, st));
-      } else {
-        SB_CHECK_CUDA(cudaMemcpyAsync(b_dst + (size_t)sub * rows * r, B->data, (size_t)rows * r * 2,
-                                      cudaMemcpyDeviceToDevice, st));
-      }
+      SB_PROPAGATE(sb::place_rows(const_cast<__half*>(llm->lora[l].B[g]), B->data, (size_t)r * 2, G, sub, st));
       llm->lora_mask[g] |= 1u << sub;
     }
   llm->lora_r = r;
   llm->lora_s = alpha / (float)r;
   const size_t T = (size_t)llm->cfg.max_batch * llm->cfg.max_seq;
   const size_t wide = (size_t)(2 * llm->cfg.ffn > llm->cfg.hidden ? 2 * llm->cfg.ffn : llm->cfg.hidden);
-  int s = sb::llama_alloc_row(llm, &llm->lora_t, T * 3 * (size_t)r);
-  if (s == 0) s = sb::llama_alloc_row(llm, &llm->lora_base, T * wide);
+  int s = sb::llama_alloc(llm->row_owned, &llm->lora_t, T * 3 * (size_t)r);
+  if (s == 0) s = sb::llama_alloc(llm->row_owned, &llm->lora_base, T * wide);
   if (s != 0) {
     sb::lora_free(llm);
     return s;
@@ -1090,16 +988,13 @@ int seedb200_llama_lora_merge(seedb200_llama* llm) {
   sb::DeviceGuard guard(llm->device);
   cudaStream_t st = 0;
   SB_CHECK_CUDA(cudaDeviceSynchronize());
-  for (int l = 0; l < (int)llm->layers.size(); ++l) {
-    const sb::LlamaLayerW& L = llm->layers[l];
-    const __half* W[4] = {L.qkv_w, L.o_w, L.gu_w, L.down_w};
+  for (int l = 0; l < (int)llm->layers.size(); ++l)
     for (int g = 0; g < 4; ++g) {
       if (llm->lora_mask[g] == 0) continue;
-      const sb::LoraGeom G = sb::lora_geom(llm, g);
+      const sb::Fused G = sb::fused(llm, g);
       const seedb200_lora_operand lo = sb::lora_operand(llm, l, g, nullptr);
-      SB_PROPAGATE(sb::lora_merge(const_cast<__half*>(W[g]), llm->lora[l].A[g], lo, G.N, G.K, st));
+      SB_PROPAGATE(sb::lora_merge(const_cast<void*>(llm->layers[l].lin[g].w), llm->lora[l].A[g], lo, G.N, G.K, st));
     }
-  }
   SB_CHECK_CUDA(cudaStreamSynchronize(st));
   sb::llama_drop_graphs(llm);
   sb::lora_free(llm);

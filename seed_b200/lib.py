@@ -1157,15 +1157,15 @@ class Llama:
 
     def int8_load_weight(self, name: str, w: torch.Tensor) -> None:
         """quantise the fp16 decoder linear `name` straight into the int8 handle's fused layout"""
-        _need_cuda_f16(w, name)
-        if w.stride(1) != 1 or w.device != self.device:
-            raise RuntimeError(f"{name}: expected rows with contiguous columns on {self.device}")
-        with on(self.device):
-            check(load().seedb200_llama_int8_load_weight(self._h, name.encode(), w.data_ptr(), w.stride(0),
-                                                         stream_ptr(self.device)), "seedb200_llama_int8_load_weight")
+        self._load_quantised("seedb200_llama_int8_load_weight", name, w)
 
     def load_4bit_weight(self, name: str, w: torch.Tensor) -> None:
         """quantise the fp16 decoder linear `name` straight into the 4-bit handle's fused layout"""
+        self._load_quantised("seedb200_llama_4bit_load_weight", name, w)
+
+    def _load_quantised(self, fn: str, name: str, w: torch.Tensor) -> None:
+        # the C side reads the [N, K] rows its slot expects from the pointer it is given: the shape is checked here.
+        # A name that is not a decoder linear passes through and is refused by the C side.
         _need_cuda_f16(w, name)
         if w.stride(1) != 1 or w.device != self.device:
             raise RuntimeError(f"{name}: expected rows with contiguous columns on {self.device}")
@@ -1177,8 +1177,7 @@ class Llama:
         if tuple(w.shape) != (N, K):
             raise RuntimeError(f"{name}: expected shape [{N}, {K}], got {list(w.shape)}")
         with on(self.device):
-            check(load().seedb200_llama_4bit_load_weight(self._h, name.encode(), w.data_ptr(), w.stride(0),
-                                                         stream_ptr(self.device)), "seedb200_llama_4bit_load_weight")
+            check(getattr(load(), fn)(self._h, name.encode(), w.data_ptr(), w.stride(0), stream_ptr(self.device)), fn)
 
     def lora_load(self, tensors: Dict[str, torch.Tensor], r: int, alpha: float) -> None:
         """copy a LoRA adapter ("model.layers.N.<...>.lora_A.weight" / ".lora_B.weight", fp16 on this device) into the

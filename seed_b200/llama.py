@@ -108,8 +108,10 @@ def _one_device(device_map) -> torch.device:
 
 
 def _linear_items(state_dict, names):
-    """(name, tensor) of the int8 linears; a state dict that makes its tensors on demand (its items() is a generator)
+    """(name, tensor) of the quantised linears; a state dict that makes its tensors on demand (its items() is a generator)
     is walked again rather than indexed, so nothing is made twice at once"""
+    if not names:
+        return
     wanted = set(names)
     if isinstance(state_dict, dict) and type(state_dict).items is dict.items:
         for k in names:
@@ -142,45 +144,36 @@ class LlamaForCausalLM(nn.Module):
         self.max_seq = max_seq or config.max_position_embeddings
         self.is_loaded_in_8bit = load_in_8bit
         self.is_loaded_in_4bit = load_in_4bit
-        if load_in_8bit or load_in_4bit:
-            # the handle is made with the fp16 tensors only; then each linear goes to the device in fp16, is quantised
-            # straight into the handle's int8 / 4-bit buffers, and is dropped before the next: device memory stays at
-            # the quantised model plus one fp16 tensor
-            weights, linears = {}, []
-            items = iter(state_dict.items())
-            for k, v in items:
-                if "rotary_emb" in k:
-                    continue
-                if _is_quantised_linear(k):
-                    linears.append(k)
-                    continue
-                weights[k] = v.detach().to(device=dev, dtype=torch.float16).contiguous()
-            self._weight_bytes = sum(t.numel() * t.element_size() for t in weights.values())
-            self._llm = L.Llama(weights, hidden=h, layers=nl, heads=nh, ffn=config.intermediate_size,
-                                vocab=config.vocab_size, max_batch=max_batch, max_seq=self.max_seq,
-                                rms_eps=config.rms_norm_eps, gemm_ctas=gemm_ctas,
-                                int8_threshold=q["llm_int8_threshold"] if load_in_8bit else None,
-                                quant4=q["bnb_4bit_quant_type"] if load_in_4bit else None)
-            for k, v in _linear_items(state_dict, linears):
-                w16 = v.detach().to(device=dev, dtype=torch.float16)
-                if w16.stride(-1) != 1 or (load_in_4bit and not w16.is_contiguous()):
-                    w16 = w16.contiguous()
-                N, K = w16.shape
-                if load_in_8bit:
-                    self._llm.int8_load_weight(k, w16)
-                    self._weight_bytes += N * K + 4 * N           # int8 values plus one fp32 scale per row
-                else:
-                    self._llm.load_4bit_weight(k, w16)
-                    self._weight_bytes += N * K // 2 + 4 * (N * K // 64)   # packed codes plus one fp32 absmax per 64
-                del w16, v     # stream-ordered: the allocator reuses this block only after the kernel has read it
-        else:
-            weights = {k: v.detach().to(device=dev, dtype=torch.float16).contiguous() for k, v in state_dict.items()
-                       if "rotary_emb" not in k}
-            # device bytes of the weights the handle owns or borrows (HF get_memory_footprint: no KV cache / workspace)
-            self._weight_bytes = sum(t.numel() * t.element_size() for t in weights.values())
-            self._llm = L.Llama(weights, hidden=h, layers=nl, heads=nh, ffn=config.intermediate_size,
-                                vocab=config.vocab_size, max_batch=max_batch, max_seq=self.max_seq,
-                                rms_eps=config.rms_norm_eps, gemm_ctas=gemm_ctas)
+        # With a quantised format the handle is made with the fp16 tensors only; then each linear goes to the device in
+        # fp16, is quantised straight into the handle's int8 / 4-bit buffers, and is dropped before the next: device
+        # memory stays at the quantised model plus one fp16 tensor.
+        weights, linears = {}, []
+        for k, v in state_dict.items():
+            if "rotary_emb" in k:
+                continue
+            if (load_in_8bit or load_in_4bit) and _is_quantised_linear(k):
+                linears.append(k)
+                continue
+            weights[k] = v.detach().to(device=dev, dtype=torch.float16).contiguous()
+        # device bytes of the weights the handle owns or borrows (HF get_memory_footprint: no KV cache / workspace)
+        self._weight_bytes = sum(t.numel() * t.element_size() for t in weights.values())
+        self._llm = L.Llama(weights, hidden=h, layers=nl, heads=nh, ffn=config.intermediate_size,
+                            vocab=config.vocab_size, max_batch=max_batch, max_seq=self.max_seq,
+                            rms_eps=config.rms_norm_eps, gemm_ctas=gemm_ctas,
+                            int8_threshold=q["llm_int8_threshold"] if load_in_8bit else None,
+                            quant4=q["bnb_4bit_quant_type"] if load_in_4bit else None)
+        for k, v in _linear_items(state_dict, linears):
+            w16 = v.detach().to(device=dev, dtype=torch.float16)
+            if w16.stride(-1) != 1 or (load_in_4bit and not w16.is_contiguous()):
+                w16 = w16.contiguous()
+            N, K = w16.shape
+            if load_in_8bit:
+                self._llm.int8_load_weight(k, w16)
+                self._weight_bytes += N * K + 4 * N           # int8 values plus one fp32 scale per row
+            else:
+                self._llm.load_4bit_weight(k, w16)
+                self._weight_bytes += N * K // 2 + 4 * (N * K // 64)   # packed codes plus one fp32 absmax per 64
+            del w16, v     # stream-ordered: the allocator reuses this block only after the kernel has read it
         # q/k/v and gate/up were copied into fused layouts by the handle: drop our references to the originals
         for k in [k for k in self._llm._weights if any(s in k for s in ("q_proj", "k_proj", "v_proj", "gate_proj", "up_proj"))]:
             del self._llm._weights[k]

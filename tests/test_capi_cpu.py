@@ -219,6 +219,35 @@ def test_decode_attention_workspace_covers_every_cache_length(L):
             assert B * H * (need * 130 * 4 + 4) <= got <= B * H * (64 * 130 * 4 + 4), (B, H, max_seq, need, got)
 
 
+def test_llama_create_checks_every_layer_before_allocating(L):
+    """seedb200_llama_create checks the tensors of every layer before it allocates anything: a checkpoint without a
+    linear of its last layer is refused by name, with no device work (the data pointers are never dereferenced)"""
+    h, ffn, V, nl = 256, 256, 64, 2
+    specs = [("model.embed_tokens.weight", (V, h)), ("model.norm.weight", (h,)), ("lm_head.weight", (V, h))]
+    for l in range(nl):
+        specs += [(f"model.layers.{l}.input_layernorm.weight", (h,)),
+                  (f"model.layers.{l}.post_attention_layernorm.weight", (h,))]
+        specs += [(f"model.layers.{l}.{nm}.weight", shape) for nm, shape in (
+            ("self_attn.q_proj", (h, h)), ("self_attn.k_proj", (h, h)), ("self_attn.v_proj", (h, h)),
+            ("self_attn.o_proj", (h, h)), ("mlp.gate_proj", (ffn, h)), ("mlp.up_proj", (ffn, h)),
+            ("mlp.down_proj", (h, ffn)))]
+    specs = [s for s in specs if s[0] != "model.layers.1.mlp.up_proj.weight"]
+    arr = (L.Tensor * len(specs))()
+    names = [name.encode() for name, _ in specs]
+    for i, (name, shape) in enumerate(specs):
+        arr[i].name = names[i]
+        arr[i].data = 4096 * (i + 1)
+        arr[i].dtype = L.DTYPE_F16
+        arr[i].ndim = len(shape)
+        for j in range(4):
+            arr[i].shape[j] = shape[j] if j < len(shape) else 1
+    cfg = L.LlamaConfig(h, nl, h // 128, 128, ffn, V, 1, 32, 1e-6, 10000.0, 0)
+    handle = C.c_void_p()
+    st = L.load().seedb200_llama_create(C.byref(cfg), arr, len(specs), C.byref(handle))
+    msg = L.load().seedb200_last_error().decode()
+    assert st != 0 and "missing weight 'model.layers.1.mlp.up_proj.weight'" in msg, msg
+
+
 def test_vector_loads_refuse_misaligned_pointers(L):
     """the GEMV and the decode attentions load x / W / norm_w, q / qkv and the caches as 16-byte vectors: a pointer
     off by 2, 4 or 8 bytes (a column-offset view) is refused with an error before any device work"""

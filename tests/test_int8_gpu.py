@@ -285,6 +285,13 @@ def test_generate_device_loop_and_batch6(lib):
     assert same_bits(cap, eager)
 
 
+def test_load_weight_refuses_a_wrong_shape(lib):
+    """the handle quantises the [N, K] rows the linear's name implies: a tensor of another shape is refused"""
+    m8, _ = build(512, 1, 4, 1408, 1056, max_batch=1, hot=False)
+    with pytest.raises(RuntimeError, match=r"expected shape \[1408, 512\]"):
+        m8._llm.int8_load_weight("model.layers.0.mlp.up_proj.weight", torch.zeros(1407, 512).half().cuda())
+
+
 def test_memory_7b_shape():
     """7B-shaped model, random-init on the device: int8 needs <= 0.56x the fp16 model's weight bytes"""
     from seed_b200.llama import LlamaForCausalLM
