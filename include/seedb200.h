@@ -126,7 +126,13 @@ typedef struct seedb200_gemm_desc {
    * x + attn(..) / x + mlp(..) is what norm2 / the next block's norm1 normalise).  Needs mode 0, N % 64 == 0, no row
    * remap and a tile width that is a multiple of 64; otherwise SEEDB200_ERR_UNSUPPORTED.                          */
   void* row_moments;
+  /* consumer-warpgroup schedule hint, 0 = auto (the planner's choice, seedb200_gemm_plan_schedule): 1 = cooperative
+   * (both consumer warpgroups on one 128 x bn tile), 2 = ping-pong (mode 0 only: one 128 x 128 tile per warpgroup,
+   * one warpgroup's epilogue under the other's MMAs; a bn hint other than 0 or 128 is SEEDB200_ERR_UNSUPPORTED).
+   * Both give bit-identical results.                                                                            */
+  int32_t wg_schedule;
 } seedb200_gemm_desc;
+enum seedb200_gemm_schedule { SEEDB200_GEMM_COOPERATIVE = 1, SEEDB200_GEMM_PINGPONG = 2 };
 int seedb200_gemm(const seedb200_gemm_desc* d, void* stream);
 /* Host-only views of the GEMM's persistent tile schedule (no GPU needed; tests/test_capi_cpu.py checks that every
  * tile is handed out exactly once).  gemm_plan: what seedb200_gemm would pick for `d` on a device with `sms` SMs --
@@ -137,6 +143,9 @@ int seedb200_gemm(const seedb200_gemm_desc* d, void* stream);
  * units that got one fewer take the last-column tiles; option "gemm_sched" = 2).                                    */
 int seedb200_gemm_plan(const seedb200_gemm_desc* d, int sms, int32_t* out9);
 int seedb200_gemm_schedule_tile(int sched, int round, int unit, int units, int m_tiles, int n_tiles, int tile_shift);
+/* Host-only: the consumer schedule seedb200_gemm runs `d` with on a device with `sms` SMs (*schedule =
+ * SEEDB200_GEMM_COOPERATIVE or SEEDB200_GEMM_PINGPONG); pointers in `d` are only tested against NULL.           */
+int seedb200_gemm_plan_schedule(const seedb200_gemm_desc* d, int sms, int32_t* schedule);
 
 /* The two helpers of the LayerNorm-folded GEMM (seedb200_gemm_desc.ln_stats):
  * row_stats: (mean, rstd = 1/sqrt(var + eps)) of every row of x [rows, cols] fp16, two-pass in fp32 exactly like

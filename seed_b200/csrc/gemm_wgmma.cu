@@ -7,7 +7,8 @@
 //
 // Design (H100 / sm_90a):
 //   * persistent, warp-specialised, 3 warpgroups: warpgroup 0 = TMA producer (one thread),
-//     warpgroups 1 and 2 = consumers, each owning 64 rows of the 128 x BN tile;
+//     warpgroups 1 and 2 = consumers, each owning 64 rows of the 128 x BN tile (cooperative), or, for the
+//     epilogue-heavy GEMMs, each owning alternate whole 128 x 128 tiles (ping-pong, see gemm_wgmma_kernel);
 //   * A and W tiles are fetched by TMA (cp.async.bulk.tensor, 128-byte swizzle) into a
 //     multi-stage shared-memory ring guarded by full/empty mbarriers;
 //   * the consumers run wgmma.mma_async m64nBNk16 straight from shared memory, accumulators in
@@ -78,7 +79,9 @@ struct GemmCfg {
   static constexpr int STAGES_RAW = (200 * 1024) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_RAW > 8 ? 8 : STAGES_RAW;
   static constexpr int SMEM_BYTES = 1024 /*align slack*/ + STAGES * STAGE_BYTES + 2 * STAGES * 8 + 2 * 2 * BN * 4;
-  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
+  // ping-pong: the column vectors once per consumer warpgroup, then the two order barriers
+  static constexpr int PP_SMEM_BYTES = SMEM_BYTES + 2 * 2 * BN * 4 + 2 * 8;
+  static_assert(PP_SMEM_BYTES <= 227 * 1024, "shared memory budget");
   static_assert(B_BYTES % 1024 == 0, "W stage must keep 1024-byte alignment for SWIZZLE_128B");
   static_assert(BN % 16 == 0 && BN <= 256, "invalid wgmma N");
   static_assert(STAGES >= 3, "pipeline too shallow");
@@ -353,10 +356,16 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
   epilogue_chunks<BN, COLS, 0>(p, acc, m0, n0, col_in_pair, lane, col_c, col_b, ln_st, row_ok, out_row, res_row);
 }
 
-template <int BN, int MODE>
+// The ping-pong schedule of MODE 0 (PP, BN = 128) for epilogue-heavy shapes: each consumer warpgroup owns a whole
+// 128 x 128 tile -- warpgroup 1 + (round & 1) takes round `round` of the persistent schedule -- and the two
+// warpgroups' k-loops take turns on the tensor cores (an order barrier pair), so that one warpgroup's epilogue runs
+// while the other's MMAs do.  Per output element the k order, the wgmma shape (m64n128k16) and the epilogue are the
+// cooperative kernel's, so the results are bit-identical to it.
+template <int BN, int MODE, bool PP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const GemmParams p) {
+  static_assert(!PP || (BN == 128 && MODE == 0), "ping-pong: 128 x 128 tiles of mode 0 only");
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
 
@@ -367,6 +376,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const uint32_t full_bar = smem_base + STAGES * Cfg::STAGE_BYTES;   // [STAGES]
   const uint32_t empty_bar = full_bar + STAGES * 8;                  // [STAGES]
   const uint32_t col_vecs = empty_bar + STAGES * 8;                // epilogue column vectors, 2 x 2 x BN floats
+                                                                   // (PP: per consumer warpgroup)
+  const uint32_t order_bar = col_vecs + 2 * 2 * 2 * BN * 4;        // PP: [2], warpgroup w may start its k-loop
 
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);
   const int lane = threadIdx.x & 31;
@@ -375,8 +386,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar + 8 * s, 1);    // the producer's arrive.expect_tx
-      mbar_init(empty_bar + 8 * s, 8);   // one arrive per consumer warp
+      mbar_init(full_bar + 8 * s, 1);              // the producer's arrive.expect_tx
+      mbar_init(empty_bar + 8 * s, PP ? 4 : 8);    // one arrive per warp of the consumer(s) of the stage
+    }
+    if (PP) {
+      mbar_init(order_bar, 4);                     // one arrive per warp of the other warpgroup
+      mbar_init(order_bar + 8, 4);
     }
     fence_mbar_init();
   }
@@ -409,8 +424,102 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     return;
   }
 
-  // ===================== consumers: 64 rows each =====================
   asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  if constexpr (PP) {
+    // ===================== ping-pong consumers: one 128 x BN tile each =====================
+    const int w = wg - 1;                           // this warpgroup's rounds: w, w + 2, w + 4, ...
+    const int cw = (threadIdx.x >> 5) & 3;
+    const int row_in_tile = cw * 16 + (lane >> 2);  // rows r, r + 8 (acc[0]) and r + 64, r + 72 (acc[1])
+    const int col_in_pair = (lane & 3) * 2;
+    const int ct = threadIdx.x & 127;               // 0 .. 127 within the warpgroup (= BN)
+    const int cols = p.ln_stats != nullptr ? EPI_LN : p.bias != nullptr ? EPI_BIAS : EPI_NONE;
+    float* col_smem = reinterpret_cast<float*>(smem_raw + (col_vecs - smem_u32(smem_raw))) + w * 2 * 2 * BN;
+    float acc0[BN / 2], acc1[BN / 2];             // rows r, r + 8 and rows r + 64, r + 72
+    for (int round = w;; round += 2) {
+      const int tile = tile_of(round);
+      if (tile >= total_tiles) break;               // before the order wait: the other warpgroup may be done too
+      const int mt = tile / p.n_tiles, nt = tile % p.n_tiles;
+      const int n0 = nt * BN;
+      // the epilogue's operands, fetched while the other warpgroup's k-loop runs (as in the cooperative consumers)
+      float col_c = 0.0f, col_b = 0.0f;
+      float2 ln0[2] = {make_float2(0.0f, 1.0f), make_float2(0.0f, 1.0f)}, ln1[2] = {ln0[0], ln0[1]};
+      if (n0 + ct < p.N) {
+        if (cols == EPI_LN) { col_c = p.ln_c[n0 + ct]; col_b = p.ln_b[n0 + ct]; }
+        else if (cols == EPI_BIAS) col_b = __half2float(p.bias[n0 + ct]);
+      }
+      if (cols == EPI_LN) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = mt * GEMM_BLOCK_M + row_in_tile + 8 * h;
+          if (m < p.M) ln0[h] = p.ln_stats[m];
+          if (m + 64 < p.M) ln1[h] = p.ln_stats[m + 64];
+        }
+      }
+      const int m = mt * GEMM_BLOCK_M + ct;
+      if (p.residual != nullptr && m < p.M) {
+        const uintptr_t lo = reinterpret_cast<uintptr_t>(p.residual + res_row_of(p, m) * p.ldr + n0);
+        const uintptr_t hi = lo + 2 * (uintptr_t)min(BN, p.N - n0);
+        for (uintptr_t a = lo & ~(uintptr_t)127; a < hi; a += 128) prefetch_l2(reinterpret_cast<const void*>(a));
+      }
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) { acc0[i] = 0.0f; acc1[i] = 0.0f; }
+      // the k-loops alternate: round `round` starts once the other warpgroup has issued all of round - 1
+      if (round > 0) mbar_wait_nocall(order_bar + 8 * w, ((round - 1) >> 1) & 1);
+      const int it0 = round * num_kb;               // the ring position after the earlier rounds' k-blocks
+      int stage = it0 % STAGES; uint32_t phase = (it0 / STAGES) & 1;
+      int prev_stage = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait_nocall(full_bar + 8 * stage, phase);
+        wgmma_fence();
+        const uint64_t adesc0 = wgmma_desc_sw128(smem_a + stage * Cfg::A_BYTES);
+        const uint64_t adesc1 = wgmma_desc_sw128(smem_a + stage * Cfg::A_BYTES + 64 * 128);   // rows 64 .. 127
+        const uint64_t bdesc = wgmma_desc_sw128(smem_b + stage * Cfg::B_BYTES);
+#pragma unroll
+        for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
+          wgmma_f16<BN>(acc0, adesc0 + 2 * k, bdesc + 2 * k);
+          wgmma_f16<BN>(acc1, adesc1 + 2 * k, bdesc + 2 * k);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev_stage >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+        }
+        prev_stage = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(order_bar + 8 * (1 - w));
+      wgmma_wait<0>();
+      acc_fence(acc0);
+      acc_fence(acc1);
+      if (prev_stage >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty_bar + 8 * prev_stage);
+      }
+      // this warpgroup's column vectors, double-buffered by its own rounds (see the cooperative epilogue)
+      float* colv = col_smem + ((round >> 1) & 1) * 2 * BN;
+      if (cols != EPI_NONE) {
+        colv[ct] = col_c; colv[BN + ct] = col_b;
+        if (w == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
+        else asm volatile("bar.sync 2, 128;" ::: "memory");
+      }
+      const int m0 = mt * GEMM_BLOCK_M + row_in_tile;
+      if (cols == EPI_LN) {
+        epilogue_tile<BN, EPI_LN>(p, acc0, m0, n0, col_in_pair, lane, colv, colv + BN, ln0);
+        epilogue_tile<BN, EPI_LN>(p, acc1, m0 + 64, n0, col_in_pair, lane, colv, colv + BN, ln1);
+      } else if (cols == EPI_BIAS) {
+        epilogue_tile<BN, EPI_BIAS>(p, acc0, m0, n0, col_in_pair, lane, colv, colv + BN, ln0);
+        epilogue_tile<BN, EPI_BIAS>(p, acc1, m0 + 64, n0, col_in_pair, lane, colv, colv + BN, ln1);
+      } else {
+        epilogue_tile<BN, EPI_NONE>(p, acc0, m0, n0, col_in_pair, lane, colv, colv + BN, ln0);
+        epilogue_tile<BN, EPI_NONE>(p, acc1, m0 + 64, n0, col_in_pair, lane, colv, colv + BN, ln1);
+      }
+    }
+    return;
+  }
+
+  // ===================== cooperative consumers: 64 rows each =====================
   const int cw = (threadIdx.x >> 5) & 3;          // warp within the warpgroup: rows 16 cw .. 16 cw + 15
   const int row_in_tile = (wg - 1) * 64 + cw * 16 + (lane >> 2);
   const int col_in_pair = (lane & 3) * 2;
@@ -745,14 +854,15 @@ static TileSchedule make_schedule(int M, int N, int bn, int sched, int sms) {
   return t;
 }
 
-template <int BN, int MODE>
+template <int BN, int MODE, bool PP = false>
 static int launch_gemm(const seedb200_gemm_desc& d, cudaStream_t stream, int sched) {
   using Cfg = GemmCfg<BN>;
+  constexpr int smem_bytes = PP ? Cfg::PP_SMEM_BYTES : Cfg::SMEM_BYTES;
   static bool attr_set_dev[SB_MAX_DEVICES] = {};   // cudaFuncSetAttribute is per device
   bool& attr_set = attr_set_dev[cur_device()];
-  auto kern = gemm_wgmma_kernel<BN, MODE>;
+  auto kern = gemm_wgmma_kernel<BN, MODE, PP>;
   if (!attr_set) {
-    SB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    SB_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
     attr_set = true;
   }
   CUtensorMap ta, tb;
@@ -779,7 +889,7 @@ static int launch_gemm(const seedb200_gemm_desc& d, cudaStream_t stream, int sch
   p.ln_b = static_cast<const float*>(d.ln_b);
 
   profile_mark_begin(0, stream);
-  kern<<<ts.units, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, p);
+  kern<<<ts.units, GEMM_THREADS, smem_bytes, stream>>>(ta, tb, p);
   profile_mark_end(0, stream, 2.0 * (double)d.M * (double)d.N * (double)d.K);
   SB_LAUNCH_CHECK();
   return 0;
@@ -843,7 +953,24 @@ static seedb200_gemm_desc with_packed_defaults(seedb200_gemm_desc d) {
   return d;
 }
 
-struct GemmPlan { int bn, sched; };
+struct GemmPlan { int bn, sched; bool pingpong; };
+
+// Ping-pong hides the epilogue but runs 128-wide tiles, which stream a third more operand bytes per FLOP than the
+// cooperative kernel's 256-wide ones.  Measured per shape (tools/gemm_shapes.py, BASELINE.md section 5), it pays for
+//   * a residual epilogue over K <= PINGPONG_MAX_K: ViT proj / fc2, Q-Former output projections, LLaMA o_proj
+//     (+3 to +25 %); LLaMA down_proj (K = 11008) loses 17 to 23 %, its mainloop dwarfs the epilogue;
+//   * the LayerNorm fold: ViT qkv +4 %, fc1 (with GELU) level;
+// and loses on bias-only (-17 %), activation-only (Q-Former fc1 GELU, -9 %) and row-remapped (patch embed, -11 %)
+// GEMMs.  It also needs two 128 x 128 tiles per SM, or a warpgroup has no tile to overlap with.
+constexpr int PINGPONG_MAX_K = 6144;
+static bool pingpong_pays(const seedb200_gemm_desc& d, int sms) {
+  if (d.mode != 0 || d.bn != 0 || d.row_group != 0) return false;
+  const bool residual = d.residual != nullptr && d.K <= PINGPONG_MAX_K;
+  if (!residual && d.ln_stats == nullptr) return false;
+  const long long tiles = (long long)((d.M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M) * ((d.N + 127) / 128);
+  return tiles >= 2LL * sms;
+}
+
 static int choose_plan(const seedb200_gemm_desc& d, int sms, GemmPlan& plan) {
   SB_REQUIRE(d.M > 0 && d.N > 0 && d.K > 0, "gemm: non-positive shape M=%d N=%d K=%d", d.M, d.N, d.K);
   SB_REQUIRE(d.mode == 0 || d.mode == 1, "gemm: unknown mode %d", d.mode);
@@ -884,7 +1011,20 @@ static int choose_plan(const seedb200_gemm_desc& d, int sms, GemmPlan& plan) {
   } else if (d.bn != 0 && get_option("gemm_sched") == 2) {
     sched = 1;                                           // A/B runs with an explicit tile width
   }
-  plan.bn = bn; plan.sched = sched;
+  SB_REQUIRE(d.wg_schedule >= 0 && d.wg_schedule <= SEEDB200_GEMM_PINGPONG,
+             "gemm: wg_schedule must be 0, 1 or 2 (got %d)", d.wg_schedule);
+  bool pingpong = false;
+  if (d.wg_schedule == SEEDB200_GEMM_PINGPONG) {
+    if (d.mode != 0 || (d.bn != 0 && d.bn != 128)) {
+      set_error("gemm: the ping-pong schedule runs 128-wide tiles of mode 0 (mode=%d bn=%d)", d.mode, d.bn);
+      return SEEDB200_ERR_UNSUPPORTED;
+    }
+    pingpong = true;
+  } else if (d.wg_schedule == 0) {
+    pingpong = pingpong_pays(d, sms);
+  }
+  if (pingpong) bn = 128;
+  plan.bn = bn; plan.sched = sched; plan.pingpong = pingpong;
   return 0;
 }
 
@@ -894,6 +1034,7 @@ int gemm(const seedb200_gemm_desc& desc, cudaStream_t stream) {
   SB_PROPAGATE(choose_plan(d, num_sms(), plan));
   SB_REQUIRE(d.A && d.W && d.out, "gemm: null operand");
   const int bn = plan.bn, sched = plan.sched;
+  if (plan.pingpong) return launch_gemm<128, 0, true>(d, stream, sched);
 #define SB_GEMM_CASE(BN_, MD_) \
   if (bn == BN_ && d.mode == MD_) return launch_gemm<BN_, MD_>(d, stream, sched);
   SB_GEMM_CASE(256, 0) SB_GEMM_CASE(192, 0) SB_GEMM_CASE(176, 0) SB_GEMM_CASE(128, 0) SB_GEMM_CASE(64, 0)
@@ -984,6 +1125,17 @@ extern "C" int seedb200_gemm_plan(const seedb200_gemm_desc* d, int sms, int32_t*
   const sb::TileSchedule t = sb::make_schedule(d->M, d->N, plan.bn, plan.sched, sms);
   const int32_t v[9] = {plan.bn, 1, t.sched, 1, t.m_tiles, t.n_tiles, t.units, 0, 0};
   for (int i = 0; i < 9; ++i) out9[i] = v[i];
+  return 0;
+}
+
+extern "C" int seedb200_gemm_plan_schedule(const seedb200_gemm_desc* d, int sms, int32_t* schedule) {
+  if (d == nullptr || schedule == nullptr || sms <= 0) {
+    sb::set_error("seedb200_gemm_plan_schedule: null argument or sms <= 0");
+    return SEEDB200_ERR_INVALID;
+  }
+  sb::GemmPlan plan;
+  SB_PROPAGATE(sb::choose_plan(sb::with_packed_defaults(*d), sms, plan));
+  *schedule = plan.pingpong ? SEEDB200_GEMM_PINGPONG : SEEDB200_GEMM_COOPERATIVE;
   return 0;
 }
 

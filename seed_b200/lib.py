@@ -16,6 +16,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libseedb200.so")
 
 ACT_NONE, ACT_GELU, ACT_TANH, ACT_RELU = 0, 1, 2, 3
+GEMM_COOPERATIVE, GEMM_PINGPONG = 1, 2     # enum seedb200_gemm_schedule (GemmDesc.wg_schedule; 0 = auto)
 VQ_FP16, VQ_FP32 = 0, 1
 
 # every symbol include/seedb200.h declares (tests check the library exports all of them)
@@ -34,7 +35,7 @@ EXPORTS = [
     "seedb200_sample", "seedb200_philox_uniform", "seedb200_image_ids_to_tokens", "seedb200_encoder_encode_tokens",
     "seedb200_llama_forward_ld", "seedb200_llama_generate", "seedb200_llama_generate_used_graph",
     "seedb200_row_stats", "seedb200_row_stats_from_moments", "seedb200_ln_fold_weights",
-    "seedb200_gemm_plan", "seedb200_gemm_schedule_tile", "seedb200_decode_attention_rope",
+    "seedb200_gemm_plan", "seedb200_gemm_schedule_tile", "seedb200_gemm_plan_schedule", "seedb200_decode_attention_rope",
     "seedb200_int8_quantize_weight", "seedb200_int8_quantize_act", "seedb200_gemm_int8", "seedb200_gemv_int8",
     "seedb200_llama_create_int8", "seedb200_llama_int8_load_weight",
     "seedb200_beam_select", "seedb200_llama_beam_generate", "seedb200_llama_reserve_rows",
@@ -68,7 +69,7 @@ class GemmDesc(C.Structure):
                 ("res_mod", C.c_int32), ("res_offset", C.c_int32),
                 ("bn", C.c_int32), ("ctas", C.c_int32),
                 ("ln_stats", C.c_void_p), ("ln_c", C.c_void_p), ("ln_b", C.c_void_p),
-                ("row_moments", C.c_void_p)]
+                ("row_moments", C.c_void_p), ("wg_schedule", C.c_int32)]
 
 
 class GemmInt8Desc(C.Structure):
@@ -318,10 +319,12 @@ def profile_end() -> dict:
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, act: int = ACT_NONE,
          residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, mode: int = 0,
          bn: int = 0, ctas: int = 0, row_group: int = 0, row_stride: int = 0, row_offset: int = 0,
-         res_mod: int = 0, res_offset: int = 0, ln=None, row_moments: Optional[torch.Tensor] = None) -> torch.Tensor:
+         res_mod: int = 0, res_offset: int = 0, ln=None, row_moments: Optional[torch.Tensor] = None,
+         wg_schedule: int = 0) -> torch.Tensor:
     """out = epilogue(a @ w.T); a [M,K], w [N,K] fp16 (nn.Linear layout).  ln = (stats [M,2] fp32, c [N] fp32,
     b [N] fp32) selects the LayerNorm-folded epilogue (w must then be the folded weight of ln_fold_weights).
-    row_moments: float32 [M, N/64, 2] that receives (sum, sum of squares) per 64-column group of the output rows."""
+    row_moments: float32 [M, N/64, 2] that receives (sum, sum of squares) per 64-column group of the output rows.
+    wg_schedule: 0 = the planner's kernel, GEMM_COOPERATIVE / GEMM_PINGPONG force one (same results)."""
     _need_cuda_f16(a, "gemm.a"); _need_cuda_f16(w, "gemm.w")
     M, K = a.shape
     N = w.shape[0]
@@ -339,7 +342,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
     d.act, d.mode = act, mode
     d.row_group, d.row_stride, d.row_offset = row_group, row_stride, row_offset
     d.res_mod, d.res_offset = res_mod, res_offset
-    d.bn, d.ctas = bn, ctas
+    d.bn, d.ctas, d.wg_schedule = bn, ctas, wg_schedule
     if ln is not None:
         stats, cvec, bvec = ln
         for t in (stats, cvec, bvec):
