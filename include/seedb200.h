@@ -300,6 +300,38 @@ int seedb200_sample(const void* logits, int64_t ld, int B, int V, const seedb200
 /* the uniform in (0,1] the sampler draws for (seed, offset + step, row) -- host function, for tests */
 float seedb200_philox_uniform(uint64_t seed, uint64_t offset, uint32_t row);
 
+/* Further generation controls, transformers 4.30.2's logits processors and TopK warper on fp16 logits, as the
+ * reference runs them on CUDA.  Neutral values (all 0, repetition_penalty 1) change nothing and launch nothing.
+ * The processors run first, in this order, on a row whose current length L includes the prompt (S tokens):
+ *   repetition_penalty p   every distinct token t among the row's history (prompt + generated tokens): v = score[t]
+ *                          becomes fp16(v * p) when v < 0, else fp16(v * fp32(1 / p)) -- torch's CUDA division of an
+ *                          fp16 tensor by a Python scalar multiplies by the fp32 reciprocal.  Duplicates count once.
+ *   no_repeat_ngram_size n nothing when L + 1 < n; else for every i <= L - n with x[i : i+n-1] == x[L-n+1 : L],
+ *                          x[i+n-1] is set to -inf
+ *   min_length m           eos is -inf while L < m
+ *   min_new_tokens m       eos is -inf while L - S < m (both length rules need an eos id >= 0)
+ * then the warpers, when sampling: temperature, top_k, top_p.  top_k k keeps every token whose compared value is >=
+ * the k'-th largest, k' = min(max(k, min_keep), V), ties kept (the threshold form of TopP).  Sampling (min_keep 1)
+ * compares the tempered fp16 logit fp16(x * fp32(1 / T)), or x when T == 1 (no temperature warper); TopP then runs
+ * on the kept tokens.  Greedy decoding and beam search apply the processors only.
+ * Beam search / sampling: the processors act on lp = fp16 log_softmax(logits) of each beam row, with that row's own
+ * tokens as history, before s = lp + beam_score; beam sampling compares w = s / T for top_k (min_keep 2), then TopP.
+ * Refused with SEEDB200_ERR_INVALID before any device work: top_k < 0, a repetition_penalty that is not finite and
+ * > 0, or a negative no_repeat_ngram_size / min_length / min_new_tokens.                                          */
+typedef struct seedb200_logits_params {
+  int32_t top_k;                 /* 0 = off */
+  float repetition_penalty;      /* 1 = off */
+  int32_t no_repeat_ngram_size;  /* 0 = off */
+  int32_t min_length;            /* 0 = off */
+  int32_t min_new_tokens;        /* 0 = off */
+} seedb200_logits_params;
+/* seedb200_sample with the controls above; lp NULL is seedb200_sample.  history [B, hist_ld] int64 (device): row b's
+ * first hist_len tokens (prompt_len of them the prompt) are its input ids; needed when a history control is active.
+ * When one is, the processors rewrite the logits rows in place before the selection.  eos_id < 0: none.          */
+int seedb200_sample_processed(void* logits, int64_t ld, int B, int V, const seedb200_sample_params* sp, uint64_t step,
+                              int64_t* tokens_out, void* stream, const seedb200_logits_params* lp,
+                              const int64_t* history, int64_t hist_ld, int hist_len, int prompt_len, int64_t eos_id);
+
 /* Beam search and beam sampling (num_beams > 1), transformers 4.30.2 GenerationMixin.beam_search / beam_sample with
  * BeamSearchScorer(num_beam_hyps_to_keep = 1), the arithmetic the reference pins (requirements.txt:8):
  *   init       beam_scores fp32 = 0 for beam 0 and -1e9 for beams 1..k-1 of every sequence (the prompt is expanded k
@@ -496,6 +528,13 @@ int seedb200_llama_forward_ld(seedb200_llama* llm, const int64_t* input_ids, con
 int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
                             const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id, int use_graph,
                             int64_t* tokens_out, int* n_generated_host, void* stream);
+/* seedb200_llama_generate with the controls of seedb200_logits_params; lp NULL is seedb200_llama_generate.  They live
+ * in device memory like the sampling parameters, so new values replay the captured decode step; a history control
+ * adds one launch per step and its own captured graph. */
+int seedb200_llama_generate_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                      int max_new_tokens, const seedb200_sample_params* sp, int64_t eos_id,
+                                      int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
+                                      void* stream, const seedb200_logits_params* lp);
 /* 1 when the last generate() replayed a captured graph, 0 when it ran eagerly, -1 before any call */
 int seedb200_llama_generate_used_graph(seedb200_llama* llm);
 /* Beam search / beam sampling (see seedb200_beam_params) of prompt_ids [B,S] (device int64): prefill at B cache rows,
@@ -508,6 +547,13 @@ int seedb200_llama_generate_used_graph(seedb200_llama* llm);
 int seedb200_llama_beam_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
                                  const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id, int use_graph,
                                  int64_t* tokens_out, int* n_out_host, float* best_scores_out, void* stream);
+/* seedb200_llama_beam_generate with the controls of seedb200_logits_params; lp NULL is seedb200_llama_beam_generate.
+ * The first call with a history control allocates a [max_batch, max_seq] int32 token table (4 * max_seq bytes per
+ * row), kept until seedb200_llama_reserve_rows reallocates the rows. */
+int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                           int max_new_tokens, const seedb200_beam_params* bp, int64_t eos_id,
+                                           int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
+                                           float* best_scores_out, void* stream, const seedb200_logits_params* lp);
 /* Grows every buffer sized by max_batch (KV caches, activations, int8 workspaces, generation state) to `rows`
  * rows; no-op when rows <= max_batch.  The cache contents and the captured graphs are dropped.  Synchronises the
  * device.  Bytes added per row: see INTEGRATION.md "C4. Beam search".                                           */

@@ -70,7 +70,7 @@ __device__ bool hyps_done(const Hyps& h, const BeamParams& bp, double best, int 
   return h.worst >= best / denom;
 }
 
-__global__ void beam_init_kernel(BeamParams bp, BeamState s) {
+__global__ void beam_init_kernel(BeamParams bp, BeamState s, const long long* prompt) {
   const int rows = bp.B * bp.k;
   const int g = blockIdx.x * blockDim.x + threadIdx.x, n = gridDim.x * blockDim.x;
   if (g == 0) {
@@ -82,15 +82,17 @@ __global__ void beam_init_kernel(BeamParams bp, BeamState s) {
   for (long long e = g; e < (long long)rows * bp.S; e += n) {
     const int b = (int)(e / bp.S), p = (int)(e % bp.S);
     s.slot[(long long)b * s.max_seq + p] = b / bp.k;
+    if (bp.processed) s.tok[(long long)b * s.max_seq + p] = (int)prompt[(long long)(b / bp.k) * bp.S + p];
   }
 }
 
-int beam_init(const BeamState& st, const BeamParams& bp, cudaStream_t stream) {
+int beam_init(const BeamState& st, const BeamParams& bp, const int64_t* prompt, cudaStream_t stream) {
+  SB_REQUIRE(!bp.processed || (st.tok != nullptr && prompt != nullptr), "beam_init: no token table");
   long long work = (long long)bp.B * bp.k * bp.S;
   int blocks = (int)((work + 255) / 256);
   if (blocks < 1) blocks = 1;
   if (blocks > 1024) blocks = 1024;
-  beam_init_kernel<<<blocks, 256, 0, stream>>>(bp, st);
+  beam_init_kernel<<<blocks, 256, 0, stream>>>(bp, st, reinterpret_cast<const long long*>(prompt));
   SB_LAUNCH_CHECK();
   return 0;
 }
@@ -158,6 +160,23 @@ __global__ void __launch_bounds__(256) beam_score_kernel(const BeamState s, int 
     s.slot[(long long)(i * k + j) * s.max_seq + p] = s.slot_tmp[(long long)(i * k + j) * s.max_seq + p];
   }
   if (pos < s.max_seq && tid < k) s.slot[(long long)(i * k + tid) * s.max_seq + pos] = i * k + tid;
+  // the token table the same way (slot_tmp reused): tokens [0, cur_len) from the parent, then the beam's own.  The
+  // flag is loaded here rather than kept live from bp across the scorer, which would add spills to this kernel.
+  if (s.params->processed) {
+    const int nt = cur_len < s.max_seq ? cur_len : s.max_seq, tt = k * nt;
+    __syncthreads();
+    for (int e = tid; e < tt; e += blockDim.x) {
+      const int j = e / nt, p = e - j * nt;
+      s.slot_tmp[(long long)(i * k + j) * s.max_seq + p] = s.tok[(long long)(i * k + s_par[j]) * s.max_seq + p];
+    }
+    __syncthreads();
+    for (int e = tid; e < tt; e += blockDim.x) {
+      const int j = e / nt, p = e - j * nt;
+      s.tok[(long long)(i * k + j) * s.max_seq + p] = s.slot_tmp[(long long)(i * k + j) * s.max_seq + p];
+    }
+    if (cur_len < s.max_seq && tid < k)
+      s.tok[(long long)(i * k + tid) * s.max_seq + cur_len] = (int)s.tokens[i * k + tid];
+  }
   __syncthreads();
   if (tid == 0) {
     __threadfence();

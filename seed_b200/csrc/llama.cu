@@ -19,6 +19,7 @@
 
 #include <map>
 #include <string>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -61,14 +62,16 @@ struct seedb200_llama {
   int* gstate;                    // {cache length, step, arrive counter, valid steps, any-unfinished flag}
   int* gfinished;                 // [max_batch]
   int64_t* gtok;                  // [max_batch] token fed to the next decode forward
-  int64_t* gout;                  // [max_batch, max_seq] generated tokens
+  int64_t* gout;                  // [max_batch, max_seq] each row's tokens: the prompt (kept when a history control
+                                  // reads it), then the generated ones from column S
   __half* glogits;                // [max_batch, vpad]
   sb::GenParams* gparams;         // sampling parameters + eos/pad, read by the sampler at run time
   int* gstate_host;               // pinned mirror of gstate (early-stop polling)
   cudaStream_t gstream;           // private stream the decode step is captured on (the caller's may be the legacy
                                   // default stream, which cannot be captured); replays go to the caller's stream
-  // captured decode units per (batch, beams): beams 0 = the sampler loop; value = (graph, kernels inside one unit)
-  std::map<std::pair<int, int>, std::pair<cudaGraphExec_t, int>> graphs;
+  // captured decode units per (batch, beams, processing launch present): beams 0 = the sampler loop;
+  // value = (graph, kernels inside one unit)
+  std::map<std::tuple<int, int, int>, std::pair<cudaGraphExec_t, int>> graphs;
   sb::BeamState beam;             // beam-search state (rows = batch * beams <= max_batch)
   int used_graph;
   int gen_cache_len;
@@ -256,6 +259,7 @@ static int llama_alloc_rows(seedb200_llama* m, cudaStream_t st) {
   SB_PROPAGATE(llama_alloc(rows, &b.hyp_n, R));
   SB_PROPAGATE(llama_alloc(rows, &b.worst, R));
   SB_PROPAGATE(llama_alloc(rows, &b.done, R));
+  b.tok = nullptr;                 // allocated by the first beam run with a history control
   b.max_seq = c.max_seq;
   return 0;
 }
@@ -497,13 +501,25 @@ __global__ void gen_reset_kernel(GenParams gp, GenParams* dst, int* state, int* 
   if (threadIdx.x < B) finished[threadIdx.x] = 0;
 }
 
-// one unit of the loop: cached forward of the tokens in m->gtok, then the sampler (beams == 0) or the beam candidates
-// and scorer (which also advance the device counters).  Every launch argument is a handle-owned pointer or a
-// constant: the unit can be captured once per (B, beams).
-static int gen_unit(seedb200_llama* m, int B, int beams, cudaStream_t st) {
+// the history processors of the step: on the sampler's rows (history = gout) or on every beam row (history = the
+// token table; beam_ld 0 = the prefill's one row per sequence, which every beam reads)
+static int gen_process(seedb200_llama* m, int B, int beams, int64_t beam_ld, cudaStream_t st) {
+  if (beams == 0)
+    return logits_process<int64_t>(m->glogits, m->vpad, 0, B, 1, m->cfg.vocab, nullptr, &m->gparams->proc, m->gstate,
+                                   m->gout, m->cfg.max_seq, 1, 0, false, st);
+  return logits_process<int>(m->glogits, beam_ld == 0 ? m->vpad : (int64_t)beams * m->vpad, beam_ld, B,
+                             beam_ld == 0 ? 1 : beams, m->cfg.vocab, nullptr, &m->beam.params->proc, m->gstate,
+                             m->beam.tok, m->cfg.max_seq, beams, 0, true, st);
+}
+
+// one unit of the loop: cached forward of the tokens in m->gtok, the history processors when `proc`, then the sampler
+// (beams == 0) or the beam candidates and scorer (which also advance the device counters).  Every launch argument is
+// a handle-owned pointer or a constant: the unit can be captured once per (B, beams, proc).
+static int gen_unit(seedb200_llama* m, int B, int beams, int proc, cudaStream_t st) {
   PdlScope pdl(get_option("decode_pdl") != 0);
   if (beams == 0) {
     SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B, 1, 0, 1, m->glogits, m->vpad, st, m->gstate));
+    if (proc) SB_PROPAGATE(gen_process(m, B, 0, 0, st));
     SB_PROPAGATE(sample(m->glogits, m->vpad, B, m->cfg.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/1,
                         m->gtok, m->gout, m->cfg.max_seq, m->gfinished, st));
     return 0;
@@ -511,6 +527,7 @@ static int gen_unit(seedb200_llama* m, int B, int beams, cudaStream_t st) {
   const int rows = B * beams;
   SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, rows, 1, 0, 1, m->glogits, m->vpad, st, m->gstate,
                              m->beam.slot));
+  if (proc) SB_PROPAGATE(gen_process(m, B, beams, m->vpad, st));
   SB_PROPAGATE(beam_select(m->glogits, (int64_t)beams * m->vpad, m->vpad, B, beams, m->cfg.vocab, m->beam.beam_scores,
                            nullptr, m->beam.params, 0, m->gstate, m->beam.row_stats, m->beam.cand_score,
                            m->beam.cand_idx, st));
@@ -518,12 +535,12 @@ static int gen_unit(seedb200_llama* m, int B, int beams, cudaStream_t st) {
   return 0;
 }
 
-static int gen_capture(seedb200_llama* m, int B, int beams) {
+static int gen_capture(seedb200_llama* m, int B, int beams, int proc) {
   cudaGraph_t graph = nullptr;
   cudaStream_t st = m->gstream;
   SB_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   const int64_t before = seedb200_launch_count();
-  const int s = gen_unit(m, B, beams, st);
+  const int s = gen_unit(m, B, beams, proc, st);
   const int unit = (int)(seedb200_launch_count() - before);
   count_launch(-unit);                        // captured, not executed
   const cudaError_t e = cudaStreamEndCapture(st, &graph);
@@ -545,27 +562,28 @@ static int gen_capture(seedb200_llama* m, int B, int beams) {
     cudaGetLastError();
     return SEEDB200_ERR_CUDA;
   }
-  m->graphs[std::make_pair(B, beams)] = std::make_pair(exec, unit);
+  m->graphs[std::make_tuple(B, beams, proc)] = std::make_pair(exec, unit);
   return 0;
 }
 
-// run `units` decode units (the first eagerly, the rest replayed from the (B, beams) graph when use_graph); with
-// `poll`, the device flag state[poll] is read every 32 units and the loop stops once it is set.  Returns units run.
-static int gen_run_units(seedb200_llama* m, int B, int beams, int units, int use_graph, int poll, cudaStream_t st,
-                         int* done_out) {
+// run `units` decode units (the first eagerly, the rest replayed from the (B, beams, proc) graph when use_graph);
+// with `poll`, the device flag state[poll] is read every 32 units and the loop stops once it is set.  Returns units
+// run.
+static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int units, int use_graph, int poll,
+                         cudaStream_t st, int* done_out) {
   int done = 0;
   m->used_graph = 0;
   if (units > 0) {   // first unit eagerly (also resolves every lazily-set function attribute before a capture)
-    SB_PROPAGATE(gen_unit(m, B, beams, st));
+    SB_PROPAGATE(gen_unit(m, B, beams, proc, st));
     done = 1;
   }
-  const auto key = std::make_pair(B, beams);
+  const auto key = std::make_tuple(B, beams, proc);
   if (units > done && use_graph) {
     if (m->graphs.find(key) == m->graphs.end()) {
-      int s = gen_capture(m, B, beams);
+      int s = gen_capture(m, B, beams, proc);
       if (s != 0 && get_option("decode_pdl") != 0) {   // retry without programmatic launches inside the graph
         seedb200_set_option("decode_pdl", 0);
-        s = gen_capture(m, B, beams);
+        s = gen_capture(m, B, beams, proc);
         seedb200_set_option("decode_pdl", 1);
       }
       if (s != 0) return s;
@@ -582,7 +600,7 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int units, int use
         SB_CHECK_CUDA(cudaGraphLaunch(g.first, st));
         count_launch(g.second);
       } else {
-        SB_PROPAGATE(gen_unit(m, B, beams, st));
+        SB_PROPAGATE(gen_unit(m, B, beams, proc, st));
       }
     }
     done += chunk;
@@ -598,20 +616,28 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int units, int use
 
 static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, int max_new,
                           const seedb200_sample_params* sp, int64_t eos, int64_t pad, int use_graph,
-                          int64_t* tokens_out, int* n_generated_host, cudaStream_t st) {
+                          int64_t* tokens_out, int* n_generated_host, const seedb200_logits_params* lp,
+                          cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
   GenParams gp;
   gp.sp = *sp; gp.eos = eos; gp.pad = pad;
+  gp.proc = logits_proc(lp, eos, S);
+  const int proc = logits_history_active(gp.proc) ? 1 : 0;
   gen_reset_kernel<<<1, 32, 0, st>>>(gp, m->gparams, m->gstate, m->gfinished, S, B);
   SB_LAUNCH_CHECK();
+  // the rows' history: the prompt in gout[:, :S]; the sampler appends from column S
+  if (proc)
+    SB_CHECK_CUDA(cudaMemcpy2DAsync(m->gout, (size_t)c.max_seq * 8, prompt_ids, (size_t)S * 8, (size_t)S * 8, B,
+                                    cudaMemcpyDeviceToDevice, st));
   // prefill: cache rows [0, S), logits of the last position only (what the sampler needs)
   SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, m->vpad, st));
+  if (proc) SB_PROPAGATE(gen_process(m, B, 0, 0, st));
   // token 0 comes from the prefill logits: the step counter advances, the cache length does not
   SB_PROPAGATE(sample(m->glogits, m->vpad, B, c.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/0, m->gtok,
                       m->gout, c.max_seq, m->gfinished, st));
   int done = 0;
   // early stop (only with an eos id): a step ran with every sequence already finished (state[3] < state[1])
-  SB_PROPAGATE(gen_run_units(m, B, 0, max_new - 1, use_graph, eos >= 0 ? 3 : -1, st, &done));
+  SB_PROPAGATE(gen_run_units(m, B, 0, proc, max_new - 1, use_graph, eos >= 0 ? 3 : -1, st, &done));
   int n_valid = done + 1;
   if (eos >= 0) {
     SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -619,7 +645,7 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
     n_valid = m->gstate_host[3];
   }
   if (tokens_out != nullptr)
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)max_new * 8, m->gout, (size_t)c.max_seq * 8, (size_t)n_valid * 8, B,
+    SB_CHECK_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)max_new * 8, m->gout + S, (size_t)c.max_seq * 8, (size_t)n_valid * 8, B,
                                     cudaMemcpyDeviceToDevice, st));
   if (n_generated_host != nullptr) *n_generated_host = n_valid;
   m->gen_cache_len = S + done;     // tokens whose K/V are in the cache
@@ -630,18 +656,22 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
 // then max_new - 1 units of (forward of B * k rows through the lineage table -> candidates -> scorer), then finalize
 static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, int max_new,
                                const seedb200_beam_params* p, int64_t eos, int64_t pad, int use_graph,
-                               int64_t* tokens_out, int* n_out_host, float* best_scores, cudaStream_t st) {
+                               int64_t* tokens_out, int* n_out_host, float* best_scores,
+                               const seedb200_logits_params* lp, cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
   const int k = p->num_beams;
-  const BeamParams bp = beam_params(*p, eos, pad, S, max_new, B);
-  SB_PROPAGATE(beam_init(m->beam, bp, st));
+  const BeamParams bp = beam_params(*p, eos, pad, S, max_new, B, lp);
+  if (bp.processed && m->beam.tok == nullptr)
+    SB_PROPAGATE(llama_alloc(m->row_owned, &m->beam.tok, (size_t)c.max_batch * c.max_seq));
+  SB_PROPAGATE(beam_init(m->beam, bp, prompt_ids, st));
   SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, m->vpad, st));
+  if (bp.processed) SB_PROPAGATE(gen_process(m, B, k, 0, st));
   SB_PROPAGATE(beam_select(m->glogits, m->vpad, 0, B, k, c.vocab, m->beam.beam_scores, nullptr, m->beam.params, 0,
                            m->gstate, m->beam.row_stats, m->beam.cand_score,
                            m->beam.cand_idx, st));
   SB_PROPAGATE(beam_score(m->beam, B, k, c.vocab, /*advance_cache=*/0, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, B, k, max_new - 1, use_graph, eos >= 0 ? 5 : -1, st, &done));
+  SB_PROPAGATE(gen_run_units(m, B, k, bp.processed, max_new - 1, use_graph, eos >= 0 ? 5 : -1, st, &done));
   SB_PROPAGATE(beam_finalize(m->beam, B, tokens_out, max_new, best_scores, st));
   int n_out = 0;
   SB_CHECK_CUDA(cudaMemcpyAsync(&n_out, m->beam.n_out, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -811,6 +841,15 @@ int seedb200_llama_forward(seedb200_llama* llm, const int64_t* input_ids, const 
 int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
                             const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id, int use_graph,
                             int64_t* tokens_out, int* n_generated_host, void* stream) {
+  return seedb200_llama_generate_processed(llm, prompt_ids, B, S, max_new_tokens, sp, eos_id, pad_id, use_graph,
+                                           tokens_out, n_generated_host, stream, nullptr);
+}
+
+int seedb200_llama_generate_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                      int max_new_tokens, const seedb200_sample_params* sp, int64_t eos_id,
+                                      int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
+                                      void* stream, const seedb200_logits_params* lp) {
+  SB_PROPAGATE(sb::logits_params_check("llama_generate", lp));
   SB_REQUIRE(llm && prompt_ids && sp, "llama_generate: null argument");
   SB_REQUIRE(B >= 1 && B <= llm->cfg.max_batch && B <= 4, "llama_generate: batch %d outside [1,%d] (decode GEMV: <= 4 rows)",
              B, llm->cfg.max_batch < 4 ? llm->cfg.max_batch : 4);
@@ -820,7 +859,7 @@ int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int 
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_generate(llm, prompt_ids, B, S, max_new_tokens, sp, eos_id, pad_id, use_graph, tokens_out,
-                            n_generated_host, static_cast<cudaStream_t>(stream));
+                            n_generated_host, lp, static_cast<cudaStream_t>(stream));
 }
 
 int seedb200_llama_generate_used_graph(seedb200_llama* llm) { return llm ? llm->used_graph : -1; }
@@ -828,6 +867,15 @@ int seedb200_llama_generate_used_graph(seedb200_llama* llm) { return llm ? llm->
 int seedb200_llama_beam_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
                                  const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id, int use_graph,
                                  int64_t* tokens_out, int* n_out_host, float* best_scores_out, void* stream) {
+  return seedb200_llama_beam_generate_processed(llm, prompt_ids, B, S, max_new_tokens, bp, eos_id, pad_id, use_graph,
+                                                tokens_out, n_out_host, best_scores_out, stream, nullptr);
+}
+
+int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                           int max_new_tokens, const seedb200_beam_params* bp, int64_t eos_id,
+                                           int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
+                                           float* best_scores_out, void* stream, const seedb200_logits_params* lp) {
+  SB_PROPAGATE(sb::logits_params_check("llama_beam_generate", lp));
   SB_REQUIRE(llm && prompt_ids && bp && tokens_out, "llama_beam_generate: null argument");
   SB_REQUIRE(bp->num_beams >= 1 && bp->num_beams <= sb::BEAM_MAX, "llama_beam_generate: num_beams %d outside [1,%d]",
              bp->num_beams, sb::BEAM_MAX);
@@ -844,7 +892,7 @@ int seedb200_llama_beam_generate(seedb200_llama* llm, const int64_t* prompt_ids,
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_beam_generate(llm, prompt_ids, B, S, max_new_tokens, bp, eos_id, pad_id, use_graph, tokens_out,
-                                 n_out_host, best_scores_out, static_cast<cudaStream_t>(stream));
+                                 n_out_host, best_scores_out, lp, static_cast<cudaStream_t>(stream));
 }
 
 int seedb200_llama_reserve_rows(seedb200_llama* llm, int rows) {

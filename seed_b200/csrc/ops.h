@@ -52,12 +52,38 @@ int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int 
 // slot (optional, device) [B, max_seq] int32: cached key / value p of row b lives in cache row slot[b*max_seq + p]
 // (beam lineage); NULL = row b.  The new token is still appended at row b.
 // sampler.cu
-struct GenParams { seedb200_sample_params sp; long long eos, pad; };
+// logits processors (seedb200_logits_params) with the eos id they mask and the prompt length S: the history of a
+// row is its first L tokens, L = S + state[1] in the device loops (the prompt, then one token per step)
+struct LogitsProc { seedb200_logits_params lp; long long eos; int S; };
+inline LogitsProc logits_proc(const seedb200_logits_params* p, long long eos, int S) {
+  LogitsProc r;
+  r.lp.top_k = 0; r.lp.repetition_penalty = 1.0f; r.lp.no_repeat_ngram_size = 0; r.lp.min_length = 0;
+  r.lp.min_new_tokens = 0;
+  if (p) r.lp = *p;
+  r.eos = eos; r.S = S;
+  return r;
+}
+// a control that reads the history or the length: the processing launch runs only then
+inline bool logits_history_active(const LogitsProc& p) {
+  return p.lp.repetition_penalty != 1.0f || p.lp.no_repeat_ngram_size > 0 ||
+         (p.eos >= 0 && (p.lp.min_length > 0 || p.lp.min_new_tokens > 0));
+}
+int logits_params_check(const char* who, const seedb200_logits_params* p);   // NULL passes
+// out[b, proc.S + step] = token (the device loop keeps the prompt in out[b, 0:S])
+struct GenParams { seedb200_sample_params sp; long long eos, pad; LogitsProc proc; };
 // gp (host, by value) or gp_dev (device, read at run time); state (device, optional) = {cache length, step, arrive,
 // valid steps, flag}: the step index comes from state[1] and the last CTA advances the counters.
 int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, const GenParams* gp_dev, uint64_t step,
            int* state, int advance_cache, int64_t* tokens, int64_t* out, int64_t out_ld, int* finished,
            cudaStream_t stream);
+// the history processors, in place on fp16 rows, one CTA per row.  Row (sequence i, beam j) = logits + i * seq_ld +
+// j * beam_ld, its history = hist + (i * hist_rows + j) * hist_ld, j < beams.  log_softmax: the row holds logits and
+// is first replaced by fp16 log_softmax (beam search).  p (host) or p_dev (device); L = p.S + state[1] when state is
+// given, else hist_len.  Tok = int64 (sampler) or int32 (beam token table).
+template <typename Tok>
+int logits_process(void* logits, int64_t seq_ld, int64_t beam_ld, int B, int beams, int V, const LogitsProc* p,
+                   const LogitsProc* p_dev, const int* state, const Tok* hist, int64_t hist_ld, int hist_rows,
+                   int hist_len, bool log_softmax, cudaStream_t stream);
 // beam search (sampler.cu: candidates; beam.cu: scorer, bookkeeping, finalize)
 constexpr int BEAM_MAX = 8;
 struct BeamParams {                    // read by the beam kernels at run time (graph replay)
@@ -66,12 +92,17 @@ struct BeamParams {                    // read by the beam kernels at run time (
   double length_penalty;
   unsigned long long seed, offset;
   long long eos, pad;
+  LogitsProc proc;                     // top_k (beam sampling) and the history processors
+  int processed;                       // 1: the rows already hold the processed fp16 log_softmax (logits_process)
 };
-inline BeamParams beam_params(const seedb200_beam_params& p, long long eos, long long pad, int S, int max_new, int B) {
+inline BeamParams beam_params(const seedb200_beam_params& p, long long eos, long long pad, int S, int max_new, int B,
+                              const seedb200_logits_params* lp = nullptr) {
   BeamParams b;
   b.k = p.num_beams; b.do_sample = p.do_sample; b.early_stopping = p.early_stopping; b.S = S; b.max_new = max_new;
   b.B = B; b.temperature = p.temperature; b.top_p = p.top_p; b.length_penalty = p.length_penalty;
   b.seed = p.seed; b.offset = p.offset; b.eos = eos; b.pad = pad;
+  b.proc = logits_proc(lp, eos, S);
+  b.processed = logits_history_active(b.proc) ? 1 : 0;
   return b;
 }
 // logits row of (sequence i, beam j) = logits + i * seq_ld + j * beam_ld; -> cand_score / cand_idx [B, 2k]
@@ -99,9 +130,12 @@ struct BeamState {
   double* worst;         // [rows]
   int* done;             // [rows]
   int* n_out;            // [1]
+  int* tok;              // [rows, max_seq] each beam row's tokens (prompt, then its own), or NULL: allocated by
+                         // the first run with a history control and maintained only while params->processed
   int max_seq;
 };
-int beam_init(const BeamState& st, const BeamParams& bp, cudaStream_t stream);
+// prompt [B, S] int64 (device): copied into every beam row of `tok` when bp.processed
+int beam_init(const BeamState& st, const BeamParams& bp, const int64_t* prompt, cudaStream_t stream);
 int beam_score(const BeamState& st, int B, int k, int V, int advance_cache, cudaStream_t stream);
 int beam_finalize(const BeamState& st, int B, int64_t* tokens_out, int64_t ld, float* best_scores, cudaStream_t stream);
 int image_ids_to_tokens(const int64_t* ids, int n, int64_t shift, int64_t boi, int64_t eoi, int64_t* out,

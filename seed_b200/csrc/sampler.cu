@@ -59,7 +59,8 @@ struct SampleArgs {
                                        //     valid steps, any-unfinished flag}, advanced by the last CTA to finish
   int advance_cache;                   // also bump state[0] (a decode forward consumed the previous token)
   long long* tokens;                   // [B] next token per sequence (also the next step's input ids)
-  long long* out; long long out_ld;    // optional [B, out_ld] history: out[b, step] = token
+  long long* out; long long out_ld;    // optional [B, out_ld] history: out[b, gp.proc.S + step] = token (columns
+                                       //     [0, S) hold the prompt when a history control reads it)
   int* finished;                       // optional [B]: sequences that already produced eos emit pad (HF semantics)
   int B;
 };
@@ -96,12 +97,165 @@ __device__ float nucleus_threshold(const Prob& prob, int i0, int i1, float targe
   return __uint_as_float(lo);
 }
 
+// fp16 <-> a 16-bit key in the same order (larger value, larger key; -0 sorts just below +0)
+__device__ __forceinline__ uint32_t half_key(__half h) {
+  const uint32_t u = __half_as_ushort(h);
+  return (u & 0x8000u) ? (~u & 0xFFFFu) : (u | 0x8000u);
+}
+__device__ __forceinline__ float key_half(uint32_t k) {
+  return __half2float(__ushort_as_half((unsigned short)((k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu))));
+}
+
+// the kk-th largest (1-based) of the fp16 values val(i) of the block's elements (this thread: [i0, i1)): two passes of
+// a 256-bin histogram, high byte then low byte.  Every thread returns it.
+template <typename Val>
+__device__ float kth_largest(const Val& val, int i0, int i1, int kk, unsigned* hist, int* sel) {
+  uint32_t prefix = 0u;
+  int rem = kk;
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int b = threadIdx.x; b < 256; b += blockDim.x) hist[b] = 0u;
+    __syncthreads();
+    for (int i = i0; i < i1; ++i) {
+      const uint32_t key = half_key(val(i));
+      if (pass == 0) atomicAdd(&hist[key >> 8], 1u);
+      else if ((key >> 8) == prefix) atomicAdd(&hist[key & 255u], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int r = rem, b = 255;
+      for (; b > 0 && (int)hist[b] < r; --b) r -= (int)hist[b];
+      sel[0] = b; sel[1] = r;
+    }
+    __syncthreads();
+    prefix = pass == 0 ? (uint32_t)sel[0] : (prefix << 8) | (uint32_t)sel[0];
+    rem = sel[1];
+    __syncthreads();
+  }
+  return key_half(prefix);
+}
+
+// ---- history processors (seedb200_logits_params), in place, one CTA per row ------------------------------------
+template <typename Tok>
+struct ProcArgs {
+  __half* logits; long long seq_ld, beam_ld; int V;
+  LogitsProc p; const LogitsProc* p_dev;
+  const int* state;
+  const Tok* hist; long long hist_ld; int hist_rows, hist_len;
+  int log_softmax;
+};
+
+template <typename Tok>
+__global__ void __launch_bounds__(SAMP_THREADS)
+logits_process_kernel(const ProcArgs<Tok> a) {
+  extern __shared__ uint32_t s_seen[];       // one bit per vocabulary id: the row's distinct history tokens
+  __shared__ float red[SAMP_THREADS / 32];
+  const int j = blockIdx.x, sq = blockIdx.y, tid = threadIdx.x;
+  pdl_trigger();
+  pdl_wait();
+  const LogitsProc p = a.p_dev ? *a.p_dev : a.p;
+  const int V = a.V;
+  __half* row = a.logits + (long long)sq * a.seq_ld + (long long)j * a.beam_ld;
+  const Tok* h = a.hist + ((long long)sq * a.hist_rows + j) * a.hist_ld;
+  const int L = a.state ? p.S + a.state[1] : a.hist_len;
+  if (a.log_softmax) {
+    // lp = fp16((x - max) - logZ): beam_row_stats_kernel's arithmetic (same chunks, same reduction order)
+    const int per = (V + SAMP_THREADS - 1) / SAMP_THREADS;
+    const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
+    float m = -INFINITY;
+    for (int i = i0; i < i1; ++i) m = fmaxf(m, __half2float(row[i]));
+    m = warp_max(m);
+    __shared__ float s_m;
+    if ((tid & 31) == 0) red[tid >> 5] = m;
+    __syncthreads();
+    if (tid < 32) {
+      float t = red[tid];
+      t = warp_max(t);
+      if (tid == 0) s_m = t;
+    }
+    __syncthreads();
+    m = s_m;
+    float z = 0.0f;
+    for (int i = i0; i < i1; ++i) z += expf(__half2float(row[i]) - m);
+    const float lz = logf(block_sum(z, red));
+    for (int i = i0; i < i1; ++i) row[i] = __float2half_rn((__half2float(row[i]) - m) - lz);
+  }
+  const int nw = (V + 31) >> 5;
+  const float pen = p.lp.repetition_penalty;
+  if (pen != 1.0f) {
+    for (int w = tid; w < nw; w += SAMP_THREADS) s_seen[w] = 0u;
+    __syncthreads();
+    for (int t = tid; t < L; t += SAMP_THREADS) {
+      const long long tok = (long long)h[t];
+      if (tok >= 0 && tok < V) atomicOr(&s_seen[tok >> 5], 1u << (tok & 31));
+    }
+    __syncthreads();
+    const float inv = 1.0f / pen;            // torch: fp16 tensor / Python scalar = x * fp32 reciprocal
+    for (int w = tid; w < nw; w += SAMP_THREADS) {
+      uint32_t bits = s_seen[w];
+      while (bits) {
+        const int t = (w << 5) + __ffs(bits) - 1;
+        bits &= bits - 1u;
+        const float v = __half2float(row[t]);
+        row[t] = __float2half_rn(v < 0.0f ? v * pen : v * inv);
+      }
+    }
+  }
+  __syncthreads();                           // the bans below overwrite penalised entries
+  const int n = p.lp.no_repeat_ngram_size;
+  if (n > 0 && L + 1 >= n) {
+    for (int i = tid; i <= L - n; i += SAMP_THREADS) {
+      bool match = true;
+      for (int q = 0; q + 1 < n && match; ++q) match = h[i + q] == h[L - n + 1 + q];
+      const long long tok = (long long)h[i + n - 1];
+      if (match && tok >= 0 && tok < V) row[tok] = __float2half_rn(-INFINITY);
+    }
+  }
+  if (tid == 0 && p.eos >= 0 && p.eos < V && (L < p.lp.min_length || L - p.S < p.lp.min_new_tokens))
+    row[p.eos] = __float2half_rn(-INFINITY);
+}
+
+template <typename Tok>
+int logits_process(void* logits, int64_t seq_ld, int64_t beam_ld, int B, int beams, int V, const LogitsProc* p,
+                   const LogitsProc* p_dev, const int* state, const Tok* hist, int64_t hist_ld, int hist_rows,
+                   int hist_len, bool log_softmax, cudaStream_t stream) {
+  const size_t smem = (size_t)((V + 31) >> 5) * 4;
+  SB_REQUIRE(logits && hist && (p || p_dev) && B >= 1 && beams >= 1 && V >= 1 && hist_ld >= 0 && hist_len >= 0,
+             "logits_process: bad arguments");
+  SB_REQUIRE(smem <= 48 * 1024, "logits_process: vocabulary %d above %d", V, 48 * 1024 * 8);
+  ProcArgs<Tok> a;
+  memset(&a, 0, sizeof(a));
+  a.logits = static_cast<__half*>(logits); a.seq_ld = seq_ld; a.beam_ld = beam_ld; a.V = V;
+  if (p) a.p = *p;
+  a.p_dev = p_dev; a.state = state; a.hist = hist; a.hist_ld = hist_ld; a.hist_rows = hist_rows;
+  a.hist_len = hist_len; a.log_softmax = log_softmax ? 1 : 0;
+  SB_CHECK_CUDA(launch_chain(logits_process_kernel<Tok>, dim3(beams, B), dim3(SAMP_THREADS), smem, stream, a));
+  SB_LAUNCH_CHECK();
+  return 0;
+}
+template int logits_process<int64_t>(void*, int64_t, int64_t, int, int, int, const LogitsProc*, const LogitsProc*,
+                                     const int*, const int64_t*, int64_t, int, int, bool, cudaStream_t);
+template int logits_process<int>(void*, int64_t, int64_t, int, int, int, const LogitsProc*, const LogitsProc*,
+                                 const int*, const int*, int64_t, int, int, bool, cudaStream_t);
+
+int logits_params_check(const char* who, const seedb200_logits_params* p) {
+  if (p == nullptr) return 0;
+  SB_REQUIRE(p->top_k >= 0, "%s: top_k %d < 0", who, p->top_k);
+  SB_REQUIRE(isfinite(p->repetition_penalty) && p->repetition_penalty > 0.0f,
+             "%s: repetition_penalty %g must be finite and > 0", who, (double)p->repetition_penalty);
+  SB_REQUIRE(p->no_repeat_ngram_size >= 0 && p->min_length >= 0 && p->min_new_tokens >= 0,
+             "%s: no_repeat_ngram_size %d, min_length %d and min_new_tokens %d must be >= 0", who,
+             p->no_repeat_ngram_size, p->min_length, p->min_new_tokens);
+  return 0;
+}
+
 __global__ void __launch_bounds__(SAMP_THREADS)
 sample_kernel(const SampleArgs a) {
   __shared__ float red[SAMP_THREADS / 32];
   __shared__ float red_v[SAMP_THREADS / 32];
   __shared__ int red_i[SAMP_THREADS / 32];
   __shared__ float scan[SAMP_THREADS];
+  __shared__ unsigned s_hist[256];
+  __shared__ int s_sel[2];
   __shared__ int s_pick;
   const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   pdl_trigger();
@@ -148,7 +302,32 @@ sample_kernel(const SampleArgs a) {
     // p_i = exp((x_i - max) / T)  (unnormalised; TemperatureLogitsWarper then softmax)
     const float inv_t = 1.0f / fmaxf(sp.temperature, 1e-6f);
     const float kk = inv_t * 1.4426950408889634f;
-    auto prob = [&](int i) { return exp2f((__half2float(row[i]) - mx) * kk); };
+    // top_k: keep the tokens whose tempered fp16 logit (HF: fp16 logits / T, skipped at T == 1) is >= the k'-th
+    // largest.  The tempered value is monotone in x, so that is x >= xmin, the least fp16 x whose tempered value
+    // reaches the tempered k'-th largest x (-inf: every token).
+    float xmin = -INFINITY;
+    const int top_k = min(max(gp.proc.lp.top_k, 1), V);
+    if (gp.proc.lp.top_k > 0 && top_k < V) {
+      const float xk = kth_largest([&](int i) { return row[i]; }, i0, i1, top_k, s_hist, s_sel);
+      if (sp.temperature == 1.0f) {
+        xmin = xk;
+      } else {
+        const float inv_tk = 1.0f / sp.temperature;
+        auto tk = [&](float x) { return __half2float(__float2half_rn(x * inv_tk)); };
+        const float kth = tk(xk);
+        uint32_t lo = 0u, hi = half_key(__float2half_rn(xk));      // smallest key with tk(value) >= kth
+        while (lo < hi) {
+          const uint32_t mid = (lo + hi) >> 1;
+          if (tk(key_half(mid)) >= kth) hi = mid; else lo = mid + 1;
+        }
+        xmin = key_half(lo);
+      }
+    }
+    auto prob = [&](int i) {
+      const float x = __half2float(row[i]);
+      const float p = exp2f((x - mx) * kk);
+      return x < xmin ? 0.0f : p;
+    };
     float z = 0.0f;
     for (int i = i0; i < i1; ++i) z += prob(i);
     const float Z = block_sum(z, red);
@@ -195,7 +374,7 @@ sample_kernel(const SampleArgs a) {
       else if (gp.eos >= 0 && tok == gp.eos) a.finished[b] = 1;
     }
     a.tokens[b] = tok;
-    if (a.out != nullptr) a.out[(long long)b * a.out_ld + (long long)step] = tok;
+    if (a.out != nullptr) a.out[(long long)b * a.out_ld + gp.proc.S + (long long)step] = tok;
     if (a.state != nullptr) {
       if (was_unfinished) atomicOr(&a.state[4], 1);
       __threadfence();
@@ -219,7 +398,10 @@ int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, co
   SampleArgs a;
   a.logits = static_cast<const __half*>(logits); a.ld = ld; a.V = V;
   if (gp) a.gp = *gp;
-  else { a.gp.sp.do_sample = 0; a.gp.sp.temperature = 1.0f; a.gp.sp.top_p = 1.0f; a.gp.sp.seed = 0; a.gp.sp.offset = 0; a.gp.eos = -1; a.gp.pad = 0; }
+  else {
+    a.gp.sp.do_sample = 0; a.gp.sp.temperature = 1.0f; a.gp.sp.top_p = 1.0f; a.gp.sp.seed = 0; a.gp.sp.offset = 0;
+    a.gp.eos = -1; a.gp.pad = 0; a.gp.proc = logits_proc(nullptr, -1, 0);
+  }
   a.gp_dev = gp_dev; a.step = step; a.state = state; a.advance_cache = advance_cache;
   a.tokens = reinterpret_cast<long long*>(tokens);
   a.out = reinterpret_cast<long long*>(out); a.out_ld = out_ld;
@@ -240,11 +422,17 @@ struct BeamSelectArgs {
   const float* beam_scores;            // [B*k]
   BeamParams bp; const BeamParams* bp_dev;
   unsigned long long step; const int* state;
-  float* row_stats;                    // [B*k, 5]: max, logZ, beam score, max w, nucleus threshold
+  float* row_stats;                    // [B*k, 5]: max, logZ (0 for processed rows), top-k threshold on w (-inf:
+                                       // none), max w, nucleus threshold; the beam score is read from beam_scores
   float* cand_score; int* cand_idx;    // [B, 2k]
 };
 
 __device__ __forceinline__ bool cand_better(float a, int ia, float b, int ib) { return a > b || (a == b && ia < ib); }
+
+// s = float(fp16 log_softmax(x)) + beam score; a processed row already holds the fp16 log_softmax
+__device__ __forceinline__ float beam_s(bool processed, float x, float mx, float lz, float bs) {
+  return processed ? x + bs : __half2float(__float2half_rn((x - mx) - lz)) + bs;
+}
 
 __device__ __forceinline__ void top2_merge(float& m1, float& m2, float o1, float o2) {
   const float n2 = fmaxf(fminf(m1, o1), fmaxf(m2, o2));
@@ -283,16 +471,32 @@ beam_row_stats_kernel(const BeamSelectArgs a) {
   }
   __syncthreads();
   m1 = red[0]; m2 = red2[0];
-  float z = 0.0f;
-  for (int i = i0; i < i1; ++i) z += expf(__half2float(row[i]) - m1);
-  const float lz = logf(block_sum(z, red));
+  const bool processed = bp.processed != 0;
+  float lz = 0.0f;
+  if (!processed) {
+    float z = 0.0f;
+    for (int i = i0; i < i1; ++i) z += expf(__half2float(row[i]) - m1);
+    lz = logf(block_sum(z, red));
+  }
   const float bsc = a.beam_scores[sq * k + j];
-  // s = float(fp16 log_softmax) + beam score, fp32
-  auto score = [&](float x) { return __half2float(__float2half_rn((x - m1) - lz)) + bsc; };
-  float mxw = 0.0f, thr = 0.0f;
+  // s = float(fp16 log_softmax) + beam score, fp32 (processed rows hold the fp16 log_softmax already)
+  auto score = [&](float x) { return beam_s(processed, x, m1, lz, bsc); };
+  float mxw = 0.0f, thr = 0.0f, wk = -INFINITY;
   if (bp.do_sample != 0) {
     mxw = score(m1) / T;                   // every step is monotone in x: the largest x gives the largest w
-    auto prob = [&](int i) { return exp2f((score(__half2float(row[i])) / T - mxw) * 1.4426950408889634f); };
+    // top_k on w (min_tokens_to_keep 2): w is monotone in the row value, so the k'-th largest w is w(k'-th value)
+    const int top_k = min(max(bp.proc.lp.top_k, 2), V);
+    if (bp.proc.lp.top_k > 0 && top_k < V) {
+      __shared__ unsigned s_hist[256];
+      __shared__ int s_sel[2];
+      wk = score(kth_largest([&](int i) { return row[i]; }, i0, i1, top_k, s_hist, s_sel)) / T;
+    }
+    const bool use_k = wk != -INFINITY;
+    auto prob = [&](int i) {
+      const float w = score(__half2float(row[i])) / T;
+      const float p = exp2f((w - mxw) * 1.4426950408889634f);
+      return (use_k && w < wk) ? 0.0f : p;
+    };
     if (bp.top_p < 1.0f) {
       float zp = 0.0f;
       for (int i = i0; i < i1; ++i) zp += prob(i);
@@ -305,7 +509,7 @@ beam_row_stats_kernel(const BeamSelectArgs a) {
   }
   if (tid == 0) {
     float* o = a.row_stats + (long long)(sq * k + j) * 5;
-    o[0] = m1; o[1] = lz; o[2] = bsc; o[3] = mxw; o[4] = thr;
+    o[0] = m1; o[1] = lz; o[2] = wk; o[3] = mxw; o[4] = thr;
   }
 }
 
@@ -314,7 +518,7 @@ __global__ void __launch_bounds__(SAMP_THREADS)
 beam_select_kernel(const BeamSelectArgs a) {
   __shared__ float red[SAMP_THREADS / 32];
   __shared__ int redi[SAMP_THREADS / 32];
-  __shared__ float s_mx[BEAM_MAX], s_lz[BEAM_MAX], s_bs[BEAM_MAX], s_mxw[BEAM_MAX], s_thr[BEAM_MAX];
+  __shared__ float s_mx[BEAM_MAX], s_lz[BEAM_MAX], s_bs[BEAM_MAX], s_mxw[BEAM_MAX], s_thr[BEAM_MAX], s_wk[BEAM_MAX];
   __shared__ float s_key[2 * BEAM_MAX];
   __shared__ int s_idx[2 * BEAM_MAX];
   const int sq = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -323,15 +527,14 @@ beam_select_kernel(const BeamSelectArgs a) {
   const BeamParams bp = a.bp_dev ? *a.bp_dev : a.bp;
   const unsigned long long step = a.state ? (unsigned long long)a.state[1] : a.step;
   const int k = bp.k, n2 = 2 * k, V = a.V;
-  const bool samp = bp.do_sample != 0;
+  const bool samp = bp.do_sample != 0, processed = bp.processed != 0;
   const float T = bp.temperature;
   auto rowp = [&](int j) { return a.logits + (long long)sq * a.seq_ld + (long long)j * a.beam_ld; };
-  auto score = [&](int j, float x) {      // s = float(fp16 log_softmax) + beam score, fp32
-    return __half2float(__float2half_rn((x - s_mx[j]) - s_lz[j])) + s_bs[j];
-  };
+  auto score = [&](int j, float x) { return beam_s(processed, x, s_mx[j], s_lz[j], s_bs[j]); };
   if (tid < k) {
     const float* st = a.row_stats + (long long)(sq * k + tid) * 5;
-    s_mx[tid] = st[0]; s_lz[tid] = st[1]; s_bs[tid] = st[2]; s_mxw[tid] = st[3]; s_thr[tid] = st[4];
+    s_mx[tid] = st[0]; s_lz[tid] = st[1]; s_wk[tid] = st[2]; s_mxw[tid] = st[3]; s_thr[tid] = st[4];
+    s_bs[tid] = a.beam_scores[sq * k + tid];
   }
   __syncthreads();
   // ---- per-thread best NC candidates, flat index f = j * V + t in increasing order ----
@@ -349,7 +552,7 @@ beam_select_kernel(const BeamSelectArgs a) {
         const float w = sc / T;
         const float p = exp2f((w - s_mxw[j]) * 1.4426950408889634f);
         key = -INFINITY;
-        if (p >= s_thr[j]) {
+        if (p >= s_thr[j] && !(s_wk[j] != -INFINITY && w < s_wk[j])) {
           const float u = philox_open_uniform(bp.seed, bp.offset + step, (uint32_t)sq, (uint32_t)f);
           key = w + (-logf(-logf(u)));
         }
@@ -472,11 +675,28 @@ extern "C" {
 
 int seedb200_sample(const void* logits, int64_t ld, int B, int V, const seedb200_sample_params* sp, uint64_t step,
                     int64_t* tokens_out, void* stream) {
+  return seedb200_sample_processed(const_cast<void*>(logits), ld, B, V, sp, step, tokens_out, stream, nullptr, nullptr,
+                                   0, 0, 0, -1);
+}
+
+int seedb200_sample_processed(void* logits, int64_t ld, int B, int V, const seedb200_sample_params* sp, uint64_t step,
+                              int64_t* tokens_out, void* stream, const seedb200_logits_params* lp,
+                              const int64_t* history, int64_t hist_ld, int hist_len, int prompt_len, int64_t eos_id) {
   SB_REQUIRE(sp != nullptr, "seedb200_sample: null parameters");
+  SB_PROPAGATE(sb::logits_params_check("seedb200_sample_processed", lp));
   sb::GenParams gp;
   gp.sp = *sp; gp.eos = -1; gp.pad = 0;
-  return sb::sample(logits, ld, B, V, &gp, nullptr, step, nullptr, 0, tokens_out, nullptr, 0, nullptr,
-                    static_cast<cudaStream_t>(stream));
+  gp.proc = sb::logits_proc(lp, eos_id, prompt_len);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (sb::logits_history_active(gp.proc)) {
+    SB_REQUIRE(history != nullptr && hist_len >= 0 && hist_ld >= hist_len && prompt_len >= 0 && prompt_len <= hist_len,
+               "seedb200_sample_processed: a history control needs history [B, >= hist_len %d] and prompt_len %d <= it",
+               hist_len, prompt_len);
+    SB_REQUIRE(logits && B >= 1 && V >= 1 && ld >= V, "sample: bad arguments");
+    SB_PROPAGATE(sb::logits_process<int64_t>(logits, ld, 0, B, 1, V, &gp.proc, nullptr, nullptr, history, hist_ld, 1,
+                                             hist_len, false, st));
+  }
+  return sb::sample(logits, ld, B, V, &gp, nullptr, step, nullptr, 0, tokens_out, nullptr, 0, nullptr, st);
 }
 
 float seedb200_philox_uniform(uint64_t seed, uint64_t offset, uint32_t row) {

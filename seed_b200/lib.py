@@ -44,6 +44,7 @@ EXPORTS = [
     "seedb200_llama_lora_merge", "seedb200_llama_replace_weights",
     "seedb200_quantize_4bit", "seedb200_dequantize_4bit", "seedb200_gemv_4bit", "seedb200_llama_create_4bit",
     "seedb200_llama_4bit_load_weight",
+    "seedb200_sample_processed", "seedb200_llama_generate_processed", "seedb200_llama_beam_generate_processed",
 ]
 
 DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
@@ -123,6 +124,27 @@ class BeamParams(C.Structure):
     _fields_ = [("num_beams", C.c_int32), ("do_sample", C.c_int32), ("temperature", C.c_float), ("top_p", C.c_float),
                 ("length_penalty", C.c_double), ("early_stopping", C.c_int32), ("seed", C.c_uint64),
                 ("offset", C.c_uint64)]
+
+
+class LogitsParams(C.Structure):
+    _fields_ = [("top_k", C.c_int32), ("repetition_penalty", C.c_float), ("no_repeat_ngram_size", C.c_int32),
+                ("min_length", C.c_int32), ("min_new_tokens", C.c_int32)]
+
+
+def logits_params(top_k: int = 0, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
+                  min_length: int = 0, min_new_tokens: int = 0) -> Optional[LogitsParams]:
+    """seedb200_logits_params, or None when every control is neutral (the entry points then take their old path).
+    Range checks are the C side's: it refuses bad values before any device work."""
+    p = LogitsParams(int(top_k), float(repetition_penalty), int(no_repeat_ngram_size), int(min_length),
+                     int(min_new_tokens))
+    neutral = (p.top_k == 0 and p.repetition_penalty == 1.0 and p.no_repeat_ngram_size == 0 and p.min_length == 0
+               and p.min_new_tokens == 0)
+    return None if neutral else p
+
+
+def _history_active(lp: Optional[LogitsParams], eos: int) -> bool:
+    return lp is not None and (lp.repetition_penalty != 1.0 or lp.no_repeat_ngram_size > 0
+                               or (eos >= 0 and (lp.min_length > 0 or lp.min_new_tokens > 0)))
 
 
 # early_stopping of transformers' GenerationConfig -> seedb200_beam_params.early_stopping
@@ -254,6 +276,12 @@ def load() -> C.CDLL:
     lib.seedb200_llama_create_4bit.argtypes = [C.POINTER(LlamaConfig), C.POINTER(Tensor), C.c_int, C.c_int,
                                                C.POINTER(C.c_void_p)]
     lib.seedb200_llama_4bit_load_weight.argtypes = [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.c_void_p]
+    lib.seedb200_sample_processed.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.POINTER(SampleParams),
+                                              C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(LogitsParams), C.c_void_p,
+                                              C.c_int64, C.c_int, C.c_int, C.c_int64]
+    lib.seedb200_llama_generate_processed.argtypes = lib.seedb200_llama_generate.argtypes + [C.POINTER(LogitsParams)]
+    lib.seedb200_llama_beam_generate_processed.argtypes = (lib.seedb200_llama_beam_generate.argtypes
+                                                           + [C.POINTER(LogitsParams)])
     _lib = lib
     return lib
 
@@ -875,17 +903,37 @@ def decode_attention_rope(qkv: torch.Tensor, positions: Optional[torch.Tensor], 
 
 
 def sample(logits: torch.Tensor, do_sample: bool = False, temperature: float = 1.0, top_p: float = 1.0,
-           seed: int = 0, offset: int = 0, step: int = 0) -> torch.Tensor:
-    """logits [B, V] fp16 (row stride free) -> next token per row, int64 [B]."""
+           seed: int = 0, offset: int = 0, step: int = 0, history: Optional[torch.Tensor] = None, top_k: int = 0,
+           repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_length: int = 0,
+           min_new_tokens: int = 0, prompt_len: int = 0, eos_token_id: int = -1) -> torch.Tensor:
+    """logits [B, V] fp16 (row stride free) -> next token per row, int64 [B].  The further controls are those of
+    seedb200_logits_params; history [B, L] int64 (device) holds each row's input ids (prompt_len of them the prompt)
+    and is needed by the penalty, n-gram and length controls.  `logits` is left unchanged."""
     _need_cuda_f16(logits, "sample.logits")
     if logits.dim() != 2 or logits.stride(1) != 1:
         raise RuntimeError("sample: logits must be [B, V] with contiguous rows")
     B, V = logits.shape
     out = torch.empty((B,), dtype=torch.int64, device=logits.device)
     sp = SampleParams(int(bool(do_sample)), float(temperature), float(top_p), int(seed), int(offset))
+    lp = logits_params(top_k, repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens)
+    if lp is None:
+        with on(logits.device):
+            check(load().seedb200_sample(logits.data_ptr(), logits.stride(0), B, V, C.byref(sp), int(step),
+                                         out.data_ptr(), stream_ptr(logits.device)), "seedb200_sample")
+        return out
+    hist, hist_len = None, 0
+    if _history_active(lp, int(eos_token_id)):
+        if history is None or history.dtype != torch.int64 or history.device != logits.device or history.dim() != 2 \
+                or history.shape[0] != B:
+            raise RuntimeError(f"sample: these controls need history [B, L] int64 on {logits.device}")
+        hist = history if history.stride(1) == 1 else history.contiguous()
+        hist_len = hist.shape[1]
+        logits = logits.clone()                 # the processors rewrite the rows in place
     with on(logits.device):
-        check(load().seedb200_sample(logits.data_ptr(), logits.stride(0), B, V, C.byref(sp), int(step), out.data_ptr(),
-                                     stream_ptr(logits.device)), "seedb200_sample")
+        check(load().seedb200_sample_processed(logits.data_ptr(), logits.stride(0), B, V, C.byref(sp), int(step),
+                                               out.data_ptr(), stream_ptr(logits.device), C.byref(lp), _p(hist),
+                                               hist.stride(0) if hist is not None else 0, hist_len, int(prompt_len),
+                                               int(eos_token_id)), "seedb200_sample_processed")
     return out
 
 
@@ -1114,29 +1162,34 @@ class Llama:
 
     def generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, do_sample: bool = False,
                  temperature: float = 1.0, top_p: float = 1.0, seed: int = 0, offset: int = 0,
-                 eos_token_id: int = -1, pad_token_id: int = 0, use_graph: bool = True) -> torch.Tensor:
+                 eos_token_id: int = -1, pad_token_id: int = 0, use_graph: bool = True, **controls) -> torch.Tensor:
         """prompt [B,S] int64 (device) -> generated tokens [B, n] (n <= max_new_tokens; shorter only when every
-        sequence hit eos).  Prefill + sampler + cached decode steps, all on the device; see seedb200_llama_generate."""
+        sequence hit eos).  Prefill + sampler + cached decode steps, all on the device; see seedb200_llama_generate.
+        `controls`: the keywords of logits_params (top_k, repetition_penalty, ...)."""
         if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
             raise RuntimeError(f"generate: prompt_ids must be int64 on {self.device}")
         prompt_ids = prompt_ids.contiguous()
         B, S = prompt_ids.shape
         out = torch.empty((B, max_new_tokens), dtype=torch.int64, device=self.device)
         sp = SampleParams(int(bool(do_sample)), float(temperature), float(top_p), int(seed), int(offset))
+        lp = logits_params(**controls)
         n = C.c_int(0)
+        args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(sp), int(eos_token_id),
+                int(pad_token_id), int(bool(use_graph)), out.data_ptr(), C.byref(n), stream_ptr(self.device))
         with on(self.device):
-            check(load().seedb200_llama_generate(self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(sp),
-                                                 int(eos_token_id), int(pad_token_id), int(bool(use_graph)),
-                                                 out.data_ptr(), C.byref(n), stream_ptr(self.device)),
-                  "seedb200_llama_generate")
+            if lp is None:
+                check(load().seedb200_llama_generate(*args), "seedb200_llama_generate")
+            else:
+                check(load().seedb200_llama_generate_processed(*args, C.byref(lp)), "seedb200_llama_generate_processed")
         return out[:, :n.value]
 
     def beam_generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, num_beams: int, do_sample: bool = False,
                       temperature: float = 1.0, top_p: float = 1.0, length_penalty: float = 1.0, early_stopping=False,
                       seed: int = 0, offset: int = 0, eos_token_id: int = -1, pad_token_id: int = 0,
-                      use_graph: bool = True):
+                      use_graph: bool = True, **controls):
         """prompt [B,S] int64 (device) -> (generated tokens [B, n] of the best hypothesis per sequence, fp32 scores [B]);
-        see seedb200_llama_beam_generate.  Needs B * num_beams <= max_batch (reserve_rows)."""
+        see seedb200_llama_beam_generate.  Needs B * num_beams <= max_batch (reserve_rows).  `controls`: the
+        keywords of logits_params."""
         if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
             raise RuntimeError(f"beam_generate: prompt_ids must be int64 on {self.device}")
         prompt_ids = prompt_ids.contiguous()
@@ -1144,12 +1197,17 @@ class Llama:
         out = torch.empty((B, max_new_tokens), dtype=torch.int64, device=self.device)
         scores = torch.empty((B,), dtype=torch.float32, device=self.device)
         bp = beam_params(num_beams, do_sample, temperature, top_p, length_penalty, early_stopping, seed, offset)
+        lp = logits_params(**controls)
         n = C.c_int(0)
+        args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(bp), int(eos_token_id),
+                int(pad_token_id), int(bool(use_graph)), out.data_ptr(), C.byref(n), scores.data_ptr(),
+                stream_ptr(self.device))
         with on(self.device):
-            check(load().seedb200_llama_beam_generate(self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(bp),
-                                                      int(eos_token_id), int(pad_token_id), int(bool(use_graph)),
-                                                      out.data_ptr(), C.byref(n), scores.data_ptr(),
-                                                      stream_ptr(self.device)), "seedb200_llama_beam_generate")
+            if lp is None:
+                check(load().seedb200_llama_beam_generate(*args), "seedb200_llama_beam_generate")
+            else:
+                check(load().seedb200_llama_beam_generate_processed(*args, C.byref(lp)),
+                      "seedb200_llama_beam_generate_processed")
         return out[:, :n.value], scores
 
     def reserve_rows(self, rows: int) -> None:

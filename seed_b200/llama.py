@@ -24,6 +24,7 @@ from __future__ import annotations
 
 import glob
 import json
+import math
 import os
 from typing import List, Optional, Tuple, Union
 
@@ -368,7 +369,24 @@ class LlamaForCausalLM(nn.Module):
 
     # GenerationConfig fields generate() honours, with the defaults used when neither it nor a kwarg sets them
     _GEN_DEFAULTS = {"max_new_tokens": 20, "do_sample": False, "temperature": 1.0, "top_p": 1.0, "num_beams": 1,
-                     "length_penalty": 1.0, "early_stopping": False, "num_return_sequences": 1}
+                     "length_penalty": 1.0, "early_stopping": False, "num_return_sequences": 1,
+                     "top_k": 0, "repetition_penalty": 1.0, "no_repeat_ngram_size": 0, "min_length": 0,
+                     "min_new_tokens": 0}
+
+    @staticmethod
+    def _controls(opts) -> dict:
+        """the logits processors / top_k warper settings, validated as transformers' classes do"""
+        top_k, pen, n = int(opts["top_k"]), opts["repetition_penalty"], int(opts["no_repeat_ngram_size"])
+        min_length, min_new = int(opts["min_length"]), int(opts["min_new_tokens"])
+        if top_k < 0:
+            raise ValueError(f"`top_k` has to be a non-negative integer, but is {top_k}")
+        if not isinstance(pen, (int, float)) or not math.isfinite(pen) or not pen > 0:
+            raise ValueError(f"`repetition_penalty` has to be a strictly positive float, but is {pen}")
+        for name, v in (("no_repeat_ngram_size", n), ("min_length", min_length), ("min_new_tokens", min_new)):
+            if v < 0:
+                raise ValueError(f"`{name}` has to be a non-negative integer, but is {v}")
+        return {"top_k": top_k, "repetition_penalty": float(pen), "no_repeat_ngram_size": n,
+                "min_length": min_length, "min_new_tokens": min_new}
 
     @torch.no_grad()
     def generate(self, input_ids=None, inputs=None, max_new_tokens: Optional[int] = None,
@@ -376,7 +394,9 @@ class LlamaForCausalLM(nn.Module):
                  num_beams: Optional[int] = None, eos_token_id=None, pad_token_id=None, attention_mask=None,
                  generator: Optional[torch.Generator] = None, seed: Optional[int] = None, use_graph: bool = True,
                  device_loop: Optional[bool] = None, generation_config=None, length_penalty: Optional[float] = None,
-                 early_stopping=None, num_return_sequences: Optional[int] = None, **_):
+                 early_stopping=None, num_return_sequences: Optional[int] = None, top_k: Optional[int] = None,
+                 repetition_penalty: Optional[float] = None, no_repeat_ngram_size: Optional[int] = None,
+                 min_length: Optional[int] = None, min_new_tokens: Optional[int] = None, **_):
         """Call pattern of scripts/seed_llama_inference_8B.py:33 (temperature=1.0, num_beams=1, max_new_tokens=512,
         top_p=0.5, do_sample=True); returns [B, S + n_new] like HF generate.
 
@@ -392,11 +412,16 @@ class LlamaForCausalLM(nn.Module):
         "never"); only `num_return_sequences=1`, an unpadded batch and one eos id.  B * num_beams rows must fit the
         handle: a model built with a smaller `max_batch` grows to it first, which drops the KV cache, so
         `past_key_values` returned by earlier forward() calls are no longer valid.
+        `top_k`, `repetition_penalty`, `no_repeat_ngram_size`, `min_length` and `min_new_tokens` act as transformers
+        4.30.2's logits processors and TopK warper, on the device in every path (include/seedb200.h,
+        seedb200_logits_params); the defaults turn them off.  Other generation keywords are ignored.
         `generation_config` (a transformers GenerationConfig) supplies these fields and its eos / pad ids, and
         explicit keyword arguments override it, as in transformers."""
         given = {"max_new_tokens": max_new_tokens, "do_sample": do_sample, "temperature": temperature, "top_p": top_p,
                  "num_beams": num_beams, "length_penalty": length_penalty, "early_stopping": early_stopping,
-                 "num_return_sequences": num_return_sequences}
+                 "num_return_sequences": num_return_sequences, "top_k": top_k,
+                 "repetition_penalty": repetition_penalty, "no_repeat_ngram_size": no_repeat_ngram_size,
+                 "min_length": min_length, "min_new_tokens": min_new_tokens}
         opts = dict(self._GEN_DEFAULTS)
         if generation_config is not None:
             for name in opts:
@@ -411,6 +436,7 @@ class LlamaForCausalLM(nn.Module):
         max_new_tokens, do_sample, temperature, top_p = (int(opts["max_new_tokens"]), bool(opts["do_sample"]),
                                                          float(opts["temperature"]), float(opts["top_p"]))
         num_beams = int(opts["num_beams"])
+        controls = self._controls(opts)
         if int(opts["num_return_sequences"]) != 1:
             raise NotImplementedError("num_return_sequences > 1 is not supported")
         if num_beams < 1:
@@ -430,10 +456,13 @@ class LlamaForCausalLM(nn.Module):
         rng_seed = self._next_seed(generator, seed)
         offset = self._draws
         padded = attention_mask is not None and not bool(attention_mask.to(torch.bool).all())
+        length_rules = controls["min_length"] > 0 or controls["min_new_tokens"] > 0
+        if length_rules and len(eos_list) > 1:
+            raise NotImplementedError("min_length / min_new_tokens with several eos_token_id values are not supported")
         if num_beams > 1:
             return self._beam_generate(input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p,
                                        float(opts["length_penalty"]), opts["early_stopping"], eos_list, pad, padded,
-                                       rng_seed, offset, use_graph)
+                                       rng_seed, offset, use_graph, controls)
         if device_loop is None:
             device_loop = (not padded) and len(eos_list) <= 1 and B <= 4
         if device_loop:
@@ -442,7 +471,7 @@ class LlamaForCausalLM(nn.Module):
             new = self._llm.generate(input_ids, max_new_tokens, do_sample=do_sample, temperature=temperature,
                                      top_p=top_p, seed=rng_seed, offset=offset,
                                      eos_token_id=eos_list[0] if eos_list else -1, pad_token_id=pad,
-                                     use_graph=use_graph)
+                                     use_graph=use_graph, **controls)
             self._draws += max_new_tokens
             self._cache_len, self._cache_batch = 0, 0       # the handle's cache now belongs to that generation
             return torch.cat([input_ids, new], dim=1)
@@ -456,7 +485,8 @@ class LlamaForCausalLM(nn.Module):
                                past_key_values=mi["past_key_values"], use_cache=True, last_logits_only=True)
             past = out.past_key_values
             nxt = L.sample(out.logits[:, -1], do_sample=do_sample, temperature=temperature, top_p=top_p,
-                           seed=rng_seed, offset=offset, step=step)
+                           seed=rng_seed, offset=offset, step=step, history=seq, prompt_len=S,
+                           eos_token_id=eos_list[0] if eos_list else -1, **controls)
             nxt = torch.where(unfinished, nxt, torch.full_like(nxt, pad))
             seq = torch.cat([seq, nxt[:, None]], dim=1)
             if mask is not None:
@@ -469,7 +499,7 @@ class LlamaForCausalLM(nn.Module):
         return seq
 
     def _beam_generate(self, input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p, length_penalty,
-                       early_stopping, eos_list, pad, padded, rng_seed, offset, use_graph):
+                       early_stopping, eos_list, pad, padded, rng_seed, offset, use_graph, controls):
         if num_beams > 8:
             raise ValueError(f"num_beams={num_beams}: at most 8 beams (the scorer runs one CTA per sequence)")
         if padded:
@@ -488,7 +518,7 @@ class LlamaForCausalLM(nn.Module):
                                          temperature=temperature if do_sample else 1.0, top_p=top_p,
                                          length_penalty=length_penalty, early_stopping=early_stopping, seed=rng_seed,
                                          offset=offset, eos_token_id=eos_list[0] if eos_list else -1,
-                                         pad_token_id=pad, use_graph=use_graph)
+                                         pad_token_id=pad, use_graph=use_graph, **controls)
         self._draws += max_new_tokens
         self._cache_len, self._cache_batch = 0, 0
         return torch.cat([input_ids, new], dim=1)
