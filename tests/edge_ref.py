@@ -83,12 +83,24 @@ def act_extra(act, pre):
     return 0.0
 
 
-def in_buffer(t, pad_cols, pad_rows, fill=NAN):
+def in_buffer(t, pad_cols, pad_rows, fill=NAN, dtype=torch.float16):
     """-> (buffer, view): t [r, c] copied into the top-left of an [r + pad_rows, c + pad_cols] buffer of `fill`"""
     r, c = t.shape
-    buf = torch.full((r + pad_rows, c + pad_cols), fill, dtype=torch.float16, device=DEV)
+    buf = torch.full((r + pad_rows, c + pad_cols), fill, dtype=dtype, device=DEV)
     buf[:r, :c] = t
     return buf, buf[:r, :c]
+
+
+def bit_diff(a, b):
+    """"" when the fp16 tensors hold identical bits (any NaN matching any NaN: payloads are not part of any contract),
+    else the number of differing elements and the first of them"""
+    a, b = a.cpu(), b.cpu()
+    na, nb = torch.isnan(a), torch.isnan(b)
+    bad = (na != nb) | (~na & ~nb & (a.view(torch.int16) != b.view(torch.int16)))
+    if not bad.any():
+        return ""
+    i = tuple(int(v) for v in bad.nonzero()[0])
+    return f"{int(bad.sum())}/{bad.numel()} differ; first at {i}: {a[i].item()!r} vs {b[i].item()!r}"
 
 
 def sentinel_buffer(rows, cols):

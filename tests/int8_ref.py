@@ -52,8 +52,11 @@ def quantize_act(a: torch.Tensor, threshold: float = 6.0):
     return q.to(torch.int8), sca, torch.nonzero(cols).flatten()
 
 
-def linear8_parts(a: torch.Tensor, cb: torch.Tensor, scb: torch.Tensor, threshold: float = 6.0) -> torch.Tensor:
-    """y = the fp16 LLM.int8() output of nn.Linear(a) before any residual / gate (see the module docstring)"""
+def linear8_parts(a: torch.Tensor, cb: torch.Tensor, scb: torch.Tensor, threshold: float = 6.0,
+                  skip_outlier: Optional[int] = None) -> torch.Tensor:
+    """y = the fp16 LLM.int8() output of nn.Linear(a) before any residual / gate (see the module docstring).
+    skip_outlier = i leaves the correction term of the i-th outlier column out (a wrong restatement, for negative
+    controls)."""
     ca, sca, O = quantize_act(a, threshold)
     acc = (ca.double() @ cb.double().t()).to(torch.int64)        # exact: |acc| < 2^31
     base = ((acc.float() * DEQUANT) * sca[:, None]) * scb[None, :]
@@ -64,6 +67,8 @@ def linear8_parts(a: torch.Tensor, cb: torch.Tensor, scb: torch.Tensor, threshol
     af = a.float()
     corr = torch.zeros(base.shape, dtype=torch.float32)
     for i, j in enumerate(O.tolist()):                  # ascending, one fp32 rounding per term
+        if i == skip_outlier:
+            continue
         corr = corr + af[:, j:j + 1] * sub[:, i][None, :]
     return (base.float() + corr.half().float()).half()
 
@@ -75,6 +80,25 @@ def silu_gate(y: torch.Tensor) -> torch.Tensor:
     g, u = blk[:, :, 0], blk[:, :, 1]
     s = (g * torch.sigmoid(g)).half().float()
     return (s * u).half().reshape(M, N // 2)
+
+
+def _ulp16(x: torch.Tensor) -> torch.Tensor:
+    """spacing of the fp16 numbers at |x|: 2^-24 throughout the subnormal range"""
+    return 2.0 ** (torch.floor(torch.log2(x.float().abs().clamp(2.0 ** -14, 65504.0))) - 10)
+
+
+def silu_gate_tol(y: torch.Tensor, ref: torch.Tensor) -> torch.Tensor:
+    """elementwise bound on |kernel - silu_gate(y)| for the fp16 gate / up values y (bit-exact by the contract).  The
+    kernels' fp16 s = silu(g) may be one fp16 step from the correctly rounded one (ex2 / rcp approximations), which
+    moves s u by ulp16(s) |u|; out and ref then round s u to fp16 once each, half a step each at a magnitude of at
+    most m = |ref| + ulp16(ref) + ulp16(s) |u|.  So |out - ref| <= ulp16(s) |u| + ulp16(m) (1 % slack on the
+    first term).  ulp16 is the true fp16 spacing, 2^-24 for subnormal s or out."""
+    M, N = y.shape
+    blk = y.float().view(M, N // 256, 2, 128)
+    g, u = blk[:, :, 0].reshape(M, N // 2), blk[:, :, 1].reshape(M, N // 2)
+    s = (g * torch.sigmoid(g)).half().float()
+    step = _ulp16(s) * u.abs()
+    return step * 1.01 + _ulp16(ref.float().abs() + _ulp16(ref) + step)
 
 
 def linear8(a: torch.Tensor, cb: torch.Tensor, scb: torch.Tensor, threshold: float = 6.0,

@@ -127,11 +127,7 @@ def test_silu_gate(lib, M, K, n_out):
         check_guards(buf, G, M, N // 2)
         assert same_bits(o2, out)
     out = out.cpu().float()
-    g = y.float().view(M, N // 256, 2, 128)[:, :, 0].reshape(M, N // 2)
-    u = y.float().view(M, N // 256, 2, 128)[:, :, 1].reshape(M, N // 2)
-    s = (g * torch.sigmoid(g)).half().float()
-    ulp_s = torch.where(s == 0, torch.full_like(s, 2.0 ** -24), 2.0 ** (torch.floor(torch.log2(s.abs())) - 10))
-    tol = ulp_s * u.abs() * 1.01 + 2.0 ** (torch.floor(torch.log2(ref.float().abs().clamp_min(2 ** -24))) - 10)
+    tol = Q.silu_gate_tol(y, ref)
     rf = ref.float()
     assert torch.equal(torch.isnan(out), torch.isnan(rf)) and torch.equal(torch.isinf(out), torch.isinf(rf))
     fin = torch.isfinite(rf)
