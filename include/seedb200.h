@@ -554,6 +554,59 @@ int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* p
                                            int max_new_tokens, const seedb200_beam_params* bp, int64_t eos_id,
                                            int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
                                            float* best_scores_out, void* stream, const seedb200_logits_params* lp);
+/* Contrastive search (generate(penalty_alpha > 0, top_k = k > 1), num_beams 1, no sampling): transformers 4.30.2
+ * GenerationMixin.contrastive_search with _ranking_fast, as the reference runs them on CUDA in fp16.  Per sequence b
+ * and step t, at position p = S + t:
+ *   logits     fp16 [V]: t = 0 the prefill's last-position logits, later the selected candidate's logits of step t-1,
+ *              after the history processors of seedb200_logits_params, and no warpers: top_k is the
+ *              candidate count
+ *   probs      softmax in fp16: fp16(exp(x - max) * fp32(1 / sum)), max and sum in fp32 (torch's CUDA epilogue
+ *              multiplies by the reciprocal; tests/test_contrastive_gpu.py pins it against the installed torch)
+ *   candidates (q_j, id_j), j < k: the k largest probs, descending, ties to the lower token id
+ *   forward    k rows, token id_j at position p, each attending to the prompt + the selected history through the
+ *              lineage table (no KV copies) -> logits_j, h_j = the row's final RMSNorm output (hidden_states[-1])
+ *   context    c_i, i < p: h of position i -- the prefill's rows for i < S, then each step's selected h
+ *   n(x)       fp16(float(x) / float(fp16(sqrt(fp32 sum of float(x)^2))))  (torch's fp16 vector_norm; any sum order)
+ *   cos_ij     fp16(sum_d n(c_i)[d] * n(h_j)[d]), fp32 accumulation in any order (cuBLAS in HF)
+ *   pen_j      max_i cos_ij (a NaN propagates)
+ *   score_j    fp16(fp16(fp32(1 - alpha) * q_j) - fp16(fp32(alpha) * pen_j)); 1 - alpha is computed in double, as
+ *              Python does, then rounded to fp32 (not 1 - fp32(alpha))
+ *   sel        argmax_j score_j, ties to the lower j; the first NaN wins (torch.max)
+ *   token      id_sel, or pad_id once the sequence has finished; the selected candidate's K/V, h and logits carry
+ *              the sequence on either way.  The sequence finishes on eos_id; the loop stops when all have.
+ * The context is stored once per position, already normalised (n depends on its row only), instead of being
+ * renormalised every step: the bits are the same.  top_k in [2, 8]; penalty_alpha finite and > 0.              */
+typedef struct seedb200_contrastive_params {
+  int32_t top_k;          /* k: candidates per step, [2, 8]                                                      */
+  double penalty_alpha;   /* alpha, finite and > 0; double so that fp32(1 - alpha) is the scalar torch uses     */
+} seedb200_contrastive_params;
+/* Contrastive search of prompt_ids [B,S] (device int64): prefill at B rows, the prompt's normalised hidden states
+ * into the context, then max_new_tokens x (history processors when lp has one -> candidates -> one cached forward of
+ * B * k rows through the lineage table -> rank + select).  The step is captured once per (B, k, processors) into a
+ * CUDA graph when use_graph != 0 (contrastive units never replay a sampler or beam graph).  B * k <= max_batch (see
+ * seedb200_llama_reserve_rows); eos_id < 0: no eos.  tokens_out [B, max_new_tokens] int64 (device); *n_generated_host
+ * (may be NULL) receives the valid width.  With an eos id the call synchronises every 32 steps to stop early.
+ * The first call allocates per row: the normalised context (2 * max_seq * hidden bytes), a logits row
+ * (2 * vocab rounded up to 8), and the candidates' probabilities and rank maxima (see INTEGRATION.md C8).  Refused
+ * with SEEDB200_ERR_INVALID before any device work: top_k outside [2, 8], a non-finite or non-positive
+ * penalty_alpha, B * k > max_batch.                                                                              */
+int seedb200_llama_contrastive_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                        int max_new_tokens, const seedb200_contrastive_params* cp, int64_t eos_id,
+                                        int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
+                                        void* stream, const seedb200_logits_params* lp);
+/* The three kernels on their own, for tests.  candidates: logits [B, ld] fp16 (V valid, V >= 8) -> ids_out [B*k]
+ * int64, probs_out [B*k] fp16.  rank: context [B, ctx_ld] fp16 holding ctx_rows normalised rows of `hidden` per
+ * sequence, the first p (>= 1) valid; cand_hidden [B*k, hidden] (raw h_j), cand_probs [B*k] fp16 -> sel_out [B] int32
+ * and scores_out [B*k] fp32 (the fp16 scores; both may be NULL); n(h_sel) is appended at context row p when
+ * p < ctx_rows.  context_init: hidden_states [B*S, hidden] -> context rows [0, S) of each sequence.  hidden % 8 == 0,
+ * 16-byte aligned operands.                                                                                      */
+int seedb200_contrastive_candidates(const void* logits, int64_t ld, int B, int V, int top_k, int64_t* ids_out,
+                                    void* probs_out, void* stream);
+int seedb200_contrastive_rank(void* context, int64_t ctx_ld, int ctx_rows, int p, int hidden, const void* cand_hidden,
+                              const void* cand_probs, int B, const seedb200_contrastive_params* cp, int32_t* sel_out,
+                              float* scores_out, void* stream);
+int seedb200_contrastive_context_init(const void* hidden_states, int B, int S, int hidden, void* context,
+                                      int64_t ctx_ld, void* stream);
 /* Grows every buffer sized by max_batch (KV caches, activations, int8 workspaces, generation state) to `rows`
  * rows; no-op when rows <= max_batch.  The cache contents and the captured graphs are dropped.  Synchronises the
  * device.  Bytes added per row: see INTEGRATION.md "C4. Beam search".                                           */

@@ -69,9 +69,9 @@ struct seedb200_llama {
   int* gstate_host;               // pinned mirror of gstate (early-stop polling)
   cudaStream_t gstream;           // private stream the decode step is captured on (the caller's may be the legacy
                                   // default stream, which cannot be captured); replays go to the caller's stream
-  // captured decode units per (batch, beams, processing launch present): beams 0 = the sampler loop;
-  // value = (graph, kernels inside one unit)
-  std::map<std::tuple<int, int, int>, std::pair<cudaGraphExec_t, int>> graphs;
+  // captured decode units per (batch, beams, processing launch present, contrastive): beams 0 = the sampler loop;
+  // contrastive units use beams = k; value = (graph, kernels inside one unit)
+  std::map<std::tuple<int, int, int, int>, std::pair<cudaGraphExec_t, int>> graphs;
   sb::BeamState beam;             // beam-search state (rows = batch * beams <= max_batch)
   int used_graph;
   int gen_cache_len;
@@ -95,6 +95,13 @@ struct seedb200_llama {
   void* lora_mem;                 // every layer's A and B
   __half* lora_t;                 // [max_batch * max_seq, 3 * r] shrink output (row buffer)
   __half* lora_base;              // [max_batch * max_seq, max(2 ffn, hidden)] base product (row buffer)
+  // ---- contrastive search: row buffers allocated by the first contrastive call ----
+  __half* c_ctx;                  // [max_batch, max_seq, hidden] normalised context of each sequence
+  __half* c_logits;               // [max_batch, vpad] each sequence's logits for the next step
+  __half* c_probs;                // [max_batch] candidates' probabilities
+  float* c_part;                  // [max_batch, CONTRAST_MAX_CTAS, CONTRAST_MAX_K] rank kernel's per-CTA maxima
+  int* c_tickets;                 // [max_batch] rank kernel's arrival counters (zero between launches)
+  sb::ContrastParams* c_params;   // k and the alpha scalars, read at run time (handle-owned)
 };
 
 namespace sb {
@@ -260,6 +267,8 @@ static int llama_alloc_rows(seedb200_llama* m, cudaStream_t st) {
   SB_PROPAGATE(llama_alloc(rows, &b.worst, R));
   SB_PROPAGATE(llama_alloc(rows, &b.done, R));
   b.tok = nullptr;                 // allocated by the first beam run with a history control
+  m->c_ctx = nullptr;              // allocated by the first contrastive run
+  m->c_logits = nullptr; m->c_probs = nullptr; m->c_part = nullptr; m->c_tickets = nullptr;
   b.max_seq = c.max_seq;
   return 0;
 }
@@ -347,6 +356,7 @@ static int llama_build(seedb200_llama* m) {
   SB_PROPAGATE(llama_alloc(m->owned, &m->gparams, 1));
   SB_PROPAGATE(llama_alloc(m->owned, &m->beam.params, 1));
   SB_PROPAGATE(llama_alloc(m->owned, &m->beam.n_out, 1));
+  SB_PROPAGATE(llama_alloc(m->owned, &m->c_params, 1));
   SB_PROPAGATE(llama_alloc_rows(m, st));
   SB_CHECK_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->gstate_host), 8 * sizeof(int)));
   SB_CHECK_CUDA(cudaStreamCreateWithFlags(&m->gstream, cudaStreamNonBlocking));
@@ -512,11 +522,36 @@ static int gen_process(seedb200_llama* m, int B, int beams, int64_t beam_ld, cud
                              m->beam.tok, m->cfg.max_seq, beams, 0, true, st);
 }
 
+// one step of contrastive search at k = beams: the history processors on each sequence's logits when `proc`, the
+// candidates, the forward of B * k candidate rows through the lineage table, then rank + select (which also advances
+// the device counters)
+static int contrastive_unit(seedb200_llama* m, int B, int k, int proc, cudaStream_t st) {
+  const seedb200_llama_config& c = m->cfg;
+  if (proc)
+    SB_PROPAGATE(logits_process<int64_t>(m->c_logits, m->vpad, 0, B, 1, c.vocab, nullptr, &m->gparams->proc,
+                                         m->gstate, m->gout, c.max_seq, 1, 0, false, st));
+  SB_PROPAGATE(contrastive_candidates(m->c_logits, m->vpad, B, c.vocab, nullptr, m->c_params, m->gstate, 0,
+                                      m->beam.slot, c.max_seq, m->gtok, m->c_probs, st));
+  SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B * k, 1, 0, 1, m->glogits, m->vpad, st, m->gstate,
+                             m->beam.slot));
+  ContrastRank r;
+  memset(&r, 0, sizeof(r));
+  r.ctx = m->c_ctx; r.ctx_ld = (int64_t)c.max_seq * c.hidden; r.ctx_rows = c.max_seq; r.H = c.hidden;
+  r.h = m->hn; r.probs = m->c_probs; r.p_dev = m->c_params; r.k = k; r.state = m->gstate;
+  r.part = m->c_part; r.tickets = m->c_tickets; r.G = contrastive_rank_ctas(c.max_seq, B);
+  r.cand_ids = reinterpret_cast<const long long*>(m->gtok); r.cand_logits = m->glogits; r.seq_logits = m->c_logits;
+  r.vpad = m->vpad; r.slot = m->beam.slot; r.max_seq = c.max_seq; r.gp = m->gparams;
+  r.out = reinterpret_cast<long long*>(m->gout); r.out_ld = c.max_seq; r.finished = m->gfinished; r.B = B;
+  return contrastive_rank(r, st);
+}
+
 // one unit of the loop: cached forward of the tokens in m->gtok, the history processors when `proc`, then the sampler
-// (beams == 0) or the beam candidates and scorer (which also advance the device counters).  Every launch argument is
-// a handle-owned pointer or a constant: the unit can be captured once per (B, beams, proc).
-static int gen_unit(seedb200_llama* m, int B, int beams, int proc, cudaStream_t st) {
+// (beams == 0) or the beam candidates and scorer (which also advance the device counters); or, with `contrast`, one
+// contrastive step.  Every launch argument is a handle-owned pointer or a constant: the unit can be captured once per
+// (B, beams, proc, contrast).
+static int gen_unit(seedb200_llama* m, int B, int beams, int proc, int contrast, cudaStream_t st) {
   PdlScope pdl(get_option("decode_pdl") != 0);
+  if (contrast) return contrastive_unit(m, B, beams, proc, st);
   if (beams == 0) {
     SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B, 1, 0, 1, m->glogits, m->vpad, st, m->gstate));
     if (proc) SB_PROPAGATE(gen_process(m, B, 0, 0, st));
@@ -535,12 +570,12 @@ static int gen_unit(seedb200_llama* m, int B, int beams, int proc, cudaStream_t 
   return 0;
 }
 
-static int gen_capture(seedb200_llama* m, int B, int beams, int proc) {
+static int gen_capture(seedb200_llama* m, int B, int beams, int proc, int contrast) {
   cudaGraph_t graph = nullptr;
   cudaStream_t st = m->gstream;
   SB_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   const int64_t before = seedb200_launch_count();
-  const int s = gen_unit(m, B, beams, proc, st);
+  const int s = gen_unit(m, B, beams, proc, contrast, st);
   const int unit = (int)(seedb200_launch_count() - before);
   count_launch(-unit);                        // captured, not executed
   const cudaError_t e = cudaStreamEndCapture(st, &graph);
@@ -562,28 +597,28 @@ static int gen_capture(seedb200_llama* m, int B, int beams, int proc) {
     cudaGetLastError();
     return SEEDB200_ERR_CUDA;
   }
-  m->graphs[std::make_tuple(B, beams, proc)] = std::make_pair(exec, unit);
+  m->graphs[std::make_tuple(B, beams, proc, contrast)] = std::make_pair(exec, unit);
   return 0;
 }
 
-// run `units` decode units (the first eagerly, the rest replayed from the (B, beams, proc) graph when use_graph);
-// with `poll`, the device flag state[poll] is read every 32 units and the loop stops once it is set.  Returns units
-// run.
-static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int units, int use_graph, int poll,
-                         cudaStream_t st, int* done_out) {
+// run `units` decode units (the first eagerly, the rest replayed from the (B, beams, proc, contrast) graph when
+// use_graph); with `poll`, the device flag state[poll] is read every 32 units and the loop stops once it is set.
+// Returns units run.
+static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int contrast, int units, int use_graph,
+                         int poll, cudaStream_t st, int* done_out) {
   int done = 0;
   m->used_graph = 0;
   if (units > 0) {   // first unit eagerly (also resolves every lazily-set function attribute before a capture)
-    SB_PROPAGATE(gen_unit(m, B, beams, proc, st));
+    SB_PROPAGATE(gen_unit(m, B, beams, proc, contrast, st));
     done = 1;
   }
-  const auto key = std::make_tuple(B, beams, proc);
+  const auto key = std::make_tuple(B, beams, proc, contrast);
   if (units > done && use_graph) {
     if (m->graphs.find(key) == m->graphs.end()) {
-      int s = gen_capture(m, B, beams, proc);
+      int s = gen_capture(m, B, beams, proc, contrast);
       if (s != 0 && get_option("decode_pdl") != 0) {   // retry without programmatic launches inside the graph
         seedb200_set_option("decode_pdl", 0);
-        s = gen_capture(m, B, beams, proc);
+        s = gen_capture(m, B, beams, proc, contrast);
         seedb200_set_option("decode_pdl", 1);
       }
       if (s != 0) return s;
@@ -600,7 +635,7 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int unit
         SB_CHECK_CUDA(cudaGraphLaunch(g.first, st));
         count_launch(g.second);
       } else {
-        SB_PROPAGATE(gen_unit(m, B, beams, proc, st));
+        SB_PROPAGATE(gen_unit(m, B, beams, proc, contrast, st));
       }
     }
     done += chunk;
@@ -637,7 +672,7 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
                       m->gout, c.max_seq, m->gfinished, st));
   int done = 0;
   // early stop (only with an eos id): a step ran with every sequence already finished (state[3] < state[1])
-  SB_PROPAGATE(gen_run_units(m, B, 0, proc, max_new - 1, use_graph, eos >= 0 ? 3 : -1, st, &done));
+  SB_PROPAGATE(gen_run_units(m, B, 0, proc, 0, max_new - 1, use_graph, eos >= 0 ? 3 : -1, st, &done));
   int n_valid = done + 1;
   if (eos >= 0) {
     SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -671,13 +706,60 @@ static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int
                            m->beam.cand_idx, st));
   SB_PROPAGATE(beam_score(m->beam, B, k, c.vocab, /*advance_cache=*/0, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, B, k, bp.processed, max_new - 1, use_graph, eos >= 0 ? 5 : -1, st, &done));
+  SB_PROPAGATE(gen_run_units(m, B, k, bp.processed, 0, max_new - 1, use_graph, eos >= 0 ? 5 : -1, st, &done));
   SB_PROPAGATE(beam_finalize(m->beam, B, tokens_out, max_new, best_scores, st));
   int n_out = 0;
   SB_CHECK_CUDA(cudaMemcpyAsync(&n_out, m->beam.n_out, sizeof(int), cudaMemcpyDeviceToHost, st));
   SB_CHECK_CUDA(cudaStreamSynchronize(st));
   if (n_out_host != nullptr) *n_out_host = n_out;
   m->gen_cache_len = 0;            // the cache rows now hold beam lineages, not B plain sequences
+  return 0;
+}
+
+// contrastive search: prefill at B rows (its logits and every prompt row's final hidden state), the normalised prompt
+// into the context, then max_new units of (processors -> candidates -> forward of B * k rows -> rank + select)
+static int llama_contrastive_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, int max_new,
+                                      const seedb200_contrastive_params* cp, int64_t eos, int64_t pad, int use_graph,
+                                      int64_t* tokens_out, int* n_generated_host, const seedb200_logits_params* lp,
+                                      cudaStream_t st) {
+  const seedb200_llama_config& c = m->cfg;
+  const ContrastParams p = contrast_params(*cp);
+  if (m->c_tickets == nullptr) {   // allocated last: a failed first call allocates again
+    const size_t R = (size_t)c.max_batch;
+    SB_PROPAGATE(llama_alloc(m->row_owned, &m->c_ctx, R * c.max_seq * c.hidden));
+    SB_PROPAGATE(llama_alloc(m->row_owned, &m->c_logits, R * m->vpad));
+    SB_PROPAGATE(llama_alloc(m->row_owned, &m->c_probs, R));
+    SB_PROPAGATE(llama_alloc(m->row_owned, &m->c_part, R * CONTRAST_MAX_CTAS * CONTRAST_MAX_K));
+    SB_PROPAGATE(llama_alloc(m->row_owned, &m->c_tickets, R));
+    SB_CHECK_CUDA(cudaMemsetAsync(m->c_tickets, 0, R * sizeof(int), st));   // left zero by every launch
+  }
+  GenParams gp;
+  memset(&gp, 0, sizeof(gp));
+  gp.eos = eos; gp.pad = pad;
+  gp.proc = logits_proc(lp, eos, S);
+  gp.proc.lp.top_k = 0;                           // the candidate count, not a warper
+  const int proc = logits_history_active(gp.proc) ? 1 : 0;
+  gen_reset_kernel<<<1, (B + 31) / 32 * 32, 0, st>>>(gp, m->gparams, m->gstate, m->gfinished, S, B);
+  SB_LAUNCH_CHECK();
+  if (proc)
+    SB_CHECK_CUDA(cudaMemcpy2DAsync(m->gout, (size_t)c.max_seq * 8, prompt_ids, (size_t)S * 8, (size_t)S * 8, B,
+                                    cudaMemcpyDeviceToDevice, st));
+  SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->c_logits, m->vpad, st));
+  SB_PROPAGATE(contrastive_context_init(m->hn, B, S, c.hidden, m->c_ctx, (int64_t)c.max_seq * c.hidden, m->beam.slot,
+                                        p.k, c.max_seq, p, m->c_params, st));
+  int done = 0;
+  SB_PROPAGATE(gen_run_units(m, B, p.k, proc, 1, max_new, use_graph, eos >= 0 ? 3 : -1, st, &done));
+  int n_valid = done;
+  if (eos >= 0) {
+    SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    SB_CHECK_CUDA(cudaStreamSynchronize(st));
+    n_valid = m->gstate_host[3];
+  }
+  if (tokens_out != nullptr && n_valid > 0)
+    SB_CHECK_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)max_new * 8, m->gout + S, (size_t)c.max_seq * 8,
+                                    (size_t)n_valid * 8, B, cudaMemcpyDeviceToDevice, st));
+  if (n_generated_host != nullptr) *n_generated_host = n_valid;
+  m->gen_cache_len = 0;            // the cache rows now hold candidate lineages, not B plain sequences
   return 0;
 }
 
@@ -893,6 +975,32 @@ int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* p
   sb::DeviceGuard guard(llm->device);
   return sb::llama_beam_generate(llm, prompt_ids, B, S, max_new_tokens, bp, eos_id, pad_id, use_graph, tokens_out,
                                  n_out_host, best_scores_out, lp, static_cast<cudaStream_t>(stream));
+}
+
+int seedb200_llama_contrastive_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                        int max_new_tokens, const seedb200_contrastive_params* cp, int64_t eos_id,
+                                        int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
+                                        void* stream, const seedb200_logits_params* lp) {
+  SB_PROPAGATE(sb::contrastive_params_check("llama_contrastive_generate", cp));
+  SB_PROPAGATE(sb::logits_params_check("llama_contrastive_generate", lp));
+  SB_REQUIRE(llm && prompt_ids, "llama_contrastive_generate: null argument");
+  SB_REQUIRE(B >= 1 && B <= 1024 && (int64_t)B * cp->top_k <= llm->cfg.max_batch,
+             "llama_contrastive_generate: batch %d x top_k %d exceeds max_batch %d (seedb200_llama_reserve_rows)", B,
+             cp->top_k, llm->cfg.max_batch);
+  SB_REQUIRE(S >= 1 && max_new_tokens >= 1 && S + max_new_tokens <= llm->cfg.max_seq,
+             "llama_contrastive_generate: prompt %d + %d new tokens exceeds max_seq %d", S, max_new_tokens,
+             llm->cfg.max_seq);
+  SB_REQUIRE(eos_id < llm->cfg.vocab, "llama_contrastive_generate: eos_id %lld outside the vocabulary",
+             (long long)eos_id);
+  SB_REQUIRE(llm->cfg.vocab >= sb::CONTRAST_MAX_K, "llama_contrastive_generate: vocabulary below %d",
+             sb::CONTRAST_MAX_K);
+  SB_REQUIRE((size_t)cp->top_k * llm->cfg.hidden * 2 <= 200 * 1024,
+             "llama_contrastive_generate: top_k %d x hidden %d exceed the rank kernel's shared memory", cp->top_k,
+             llm->cfg.hidden);
+  SB_PROPAGATE(sb::llama_linears_ready(llm));
+  sb::DeviceGuard guard(llm->device);
+  return sb::llama_contrastive_generate(llm, prompt_ids, B, S, max_new_tokens, cp, eos_id, pad_id, use_graph,
+                                        tokens_out, n_generated_host, lp, static_cast<cudaStream_t>(stream));
 }
 
 int seedb200_llama_reserve_rows(seedb200_llama* llm, int rows) {

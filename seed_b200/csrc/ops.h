@@ -2,6 +2,7 @@
 // orchestration in encoder.cu / llama.cu and re-exported 1:1 through the C ABI.
 #pragma once
 
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -140,6 +141,35 @@ int beam_score(const BeamState& st, int B, int k, int V, int advance_cache, cuda
 int beam_finalize(const BeamState& st, int B, int64_t* tokens_out, int64_t ld, float* best_scores, cudaStream_t stream);
 int image_ids_to_tokens(const int64_t* ids, int n, int64_t shift, int64_t boi, int64_t eoi, int64_t* out,
                         int64_t out_stride, cudaStream_t stream);
+// contrastive search (contrastive.cu)
+constexpr int CONTRAST_MAX_K = 8, CONTRAST_MAX_CTAS = 512;
+struct ContrastParams { int k; float c_prob, c_pen; };   // c_prob = fp32(1 - alpha), c_pen = fp32(alpha)
+int contrastive_params_check(const char* who, const seedb200_contrastive_params* cp);   // NULL is refused
+ContrastParams contrast_params(const seedb200_contrastive_params& cp);
+// candidates of B rows (logits + b * ld): ids / probs [B*k]; p (host) or p_dev (device); slot (optional)
+// [B*k, max_seq] gets slot[r, pos] = r with pos = state[0] when state is given
+int contrastive_candidates(const void* logits, int64_t ld, int B, int V, const ContrastParams* p,
+                           const ContrastParams* p_dev, const int* state, int pos, int* slot, int max_seq,
+                           int64_t* ids, void* probs, cudaStream_t stream);
+// one rank + select launch (see RankArgs in contrastive.cu); the loop fields are NULL in the standalone entry point
+struct ContrastRank {
+  __half* ctx; int64_t ctx_ld; int ctx_rows, H;
+  const __half* h; const __half* probs;
+  const ContrastParams* p; const ContrastParams* p_dev; int k;
+  int* state; int pos;
+  float* part; int* tickets; int G;
+  int* sel; float* score;
+  const long long* cand_ids; const __half* cand_logits; __half* seq_logits; int64_t vpad;
+  int* slot; int max_seq;
+  const GenParams* gp; long long* out; int64_t out_ld; int* finished;
+  int B;
+};
+int contrastive_rank_ctas(int max_rows, int B);   // the rank kernel's CTAs per sequence for contexts of max_rows
+int contrastive_rank(const ContrastRank& r, cudaStream_t stream);
+// hidden_states [B*S, H] -> ctx rows [0, S) of each sequence; slot (optional) [B*k, max_seq]: positions < S of every
+// candidate row read the prefill row b; p_out (optional, device) receives p
+int contrastive_context_init(const void* hidden_states, int B, int S, int H, void* ctx, int64_t ctx_ld, int* slot,
+                             int k, int max_seq, const ContrastParams& p, ContrastParams* p_out, cudaStream_t stream);
 int cur_device();
 // LLM.int8() (int8.cu, gemm_wgmma.cu)
 int int8_quantize_weight(const void* W, int64_t ldw, int N, int K, void* CB, void* SCB, cudaStream_t stream);

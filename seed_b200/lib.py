@@ -45,6 +45,8 @@ EXPORTS = [
     "seedb200_quantize_4bit", "seedb200_dequantize_4bit", "seedb200_gemv_4bit", "seedb200_llama_create_4bit",
     "seedb200_llama_4bit_load_weight",
     "seedb200_sample_processed", "seedb200_llama_generate_processed", "seedb200_llama_beam_generate_processed",
+    "seedb200_llama_contrastive_generate", "seedb200_contrastive_candidates", "seedb200_contrastive_rank",
+    "seedb200_contrastive_context_init",
 ]
 
 DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
@@ -129,6 +131,10 @@ class BeamParams(C.Structure):
 class LogitsParams(C.Structure):
     _fields_ = [("top_k", C.c_int32), ("repetition_penalty", C.c_float), ("no_repeat_ngram_size", C.c_int32),
                 ("min_length", C.c_int32), ("min_new_tokens", C.c_int32)]
+
+
+class ContrastiveParams(C.Structure):
+    _fields_ = [("top_k", C.c_int32), ("penalty_alpha", C.c_double)]
 
 
 def logits_params(top_k: int = 0, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
@@ -282,6 +288,16 @@ def load() -> C.CDLL:
     lib.seedb200_llama_generate_processed.argtypes = lib.seedb200_llama_generate.argtypes + [C.POINTER(LogitsParams)]
     lib.seedb200_llama_beam_generate_processed.argtypes = (lib.seedb200_llama_beam_generate.argtypes
                                                            + [C.POINTER(LogitsParams)])
+    lib.seedb200_llama_contrastive_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                        C.POINTER(ContrastiveParams), C.c_int64, C.c_int64, C.c_int,
+                                                        C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(LogitsParams)]
+    lib.seedb200_contrastive_candidates.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p]
+    lib.seedb200_contrastive_rank.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                              C.c_void_p, C.c_int, C.POINTER(ContrastiveParams), C.c_void_p,
+                                              C.c_void_p, C.c_void_p]
+    lib.seedb200_contrastive_context_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64,
+                                                      C.c_void_p]
     _lib = lib
     return lib
 
@@ -937,6 +953,59 @@ def sample(logits: torch.Tensor, do_sample: bool = False, temperature: float = 1
     return out
 
 
+def contrastive_candidates(logits: torch.Tensor, top_k: int):
+    """contrastive search's candidates of each row of logits [B, V] fp16 (row stride free): (ids [B, k] int64,
+    probs [B, k] fp16), the k largest fp16 softmax probabilities, descending, ties to the lower id"""
+    _need_cuda_f16(logits, "contrastive_candidates.logits")
+    if logits.dim() != 2 or logits.stride(1) != 1:
+        raise RuntimeError("contrastive_candidates: logits must be [B, V] with contiguous rows")
+    B, V = logits.shape
+    ids = torch.empty((B, int(top_k)), dtype=torch.int64, device=logits.device)
+    probs = torch.empty((B, int(top_k)), dtype=torch.float16, device=logits.device)
+    with on(logits.device):
+        check(load().seedb200_contrastive_candidates(logits.data_ptr(), logits.stride(0), B, V, int(top_k),
+                                                     ids.data_ptr(), probs.data_ptr(), stream_ptr(logits.device)),
+              "seedb200_contrastive_candidates")
+    return ids, probs
+
+
+def contrastive_rank(context: torch.Tensor, p: int, cand_hidden: torch.Tensor, cand_probs: torch.Tensor,
+                     penalty_alpha: float):
+    """rank + select of B sequences: context [B, rows, H] fp16 (normalised, the first p rows valid; n(h_sel) is written
+    at row p when p < rows), cand_hidden [B, k, H] fp16, cand_probs [B, k] fp16 -> (sel [B] int32, scores [B, k]
+    fp32 holding the fp16 scores)"""
+    for t, n in ((context, "context"), (cand_hidden, "cand_hidden"), (cand_probs, "cand_probs")):
+        _need_cuda_f16(t, "contrastive_rank." + n)
+        if not t.is_contiguous():
+            raise RuntimeError(f"contrastive_rank: {n} must be contiguous")
+    B, rows, H = context.shape
+    k = cand_hidden.shape[1]
+    if tuple(cand_hidden.shape) != (B, k, H) or tuple(cand_probs.shape) != (B, k):
+        raise RuntimeError("contrastive_rank: cand_hidden must be [B, k, H] and cand_probs [B, k]")
+    cp = ContrastiveParams(k, float(penalty_alpha))
+    sel = torch.empty((B,), dtype=torch.int32, device=context.device)
+    scores = torch.empty((B, k), dtype=torch.float32, device=context.device)
+    with on(context.device):
+        check(load().seedb200_contrastive_rank(context.data_ptr(), rows * H, rows, int(p), H, cand_hidden.data_ptr(),
+                                               cand_probs.data_ptr(), B, C.byref(cp), sel.data_ptr(),
+                                               scores.data_ptr(), stream_ptr(context.device)),
+              "seedb200_contrastive_rank")
+    return sel, scores
+
+
+def contrastive_context_init(hidden_states: torch.Tensor, context: torch.Tensor) -> None:
+    """hidden_states [B, S, H] fp16 -> rows [0, S) of context [B, rows, H], normalised"""
+    _need_cuda_f16(hidden_states, "contrastive_context_init.hidden_states")
+    _need_cuda_f16(context, "contrastive_context_init.context")
+    if not (hidden_states.is_contiguous() and context.is_contiguous()):
+        raise RuntimeError("contrastive_context_init: operands must be contiguous")
+    B, S, H = hidden_states.shape
+    with on(context.device):
+        check(load().seedb200_contrastive_context_init(hidden_states.data_ptr(), B, S, H, context.data_ptr(),
+                                                       context.shape[1] * H, stream_ptr(context.device)),
+              "seedb200_contrastive_context_init")
+
+
 def philox_uniform(seed: int, offset: int, row: int) -> float:
     return float(load().seedb200_philox_uniform(int(seed), int(offset), int(row)))
 
@@ -1209,6 +1278,29 @@ class Llama:
                 check(load().seedb200_llama_beam_generate_processed(*args, C.byref(lp)),
                       "seedb200_llama_beam_generate_processed")
         return out[:, :n.value], scores
+
+    def contrastive_generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, top_k: int, penalty_alpha: float,
+                             eos_token_id: int = -1, pad_token_id: int = 0, use_graph: bool = True,
+                             **controls) -> torch.Tensor:
+        """prompt [B,S] int64 (device) -> generated tokens [B, n] of contrastive search (n < max_new_tokens only when
+        every sequence hit eos); see seedb200_llama_contrastive_generate.  Needs B * top_k <= max_batch
+        (reserve_rows).  `controls`: the processor keywords of logits_params (their top_k is not used)."""
+        if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
+            raise RuntimeError(f"contrastive_generate: prompt_ids must be int64 on {self.device}")
+        prompt_ids = prompt_ids.contiguous()
+        B, S = prompt_ids.shape
+        out = torch.empty((B, max_new_tokens), dtype=torch.int64, device=self.device)
+        cp = ContrastiveParams(int(top_k), float(penalty_alpha))
+        lp = logits_params(**dict(controls, top_k=0))
+        n = C.c_int(0)
+        with on(self.device):
+            check(load().seedb200_llama_contrastive_generate(self._h, prompt_ids.data_ptr(), B, S, max_new_tokens,
+                                                             C.byref(cp), int(eos_token_id), int(pad_token_id),
+                                                             int(bool(use_graph)), out.data_ptr(), C.byref(n),
+                                                             stream_ptr(self.device),
+                                                             C.byref(lp) if lp is not None else None),
+                  "seedb200_llama_contrastive_generate")
+        return out[:, :n.value]
 
     def reserve_rows(self, rows: int) -> None:
         """grow every max_batch-sized buffer to `rows` rows (drops the cache contents and the captured graphs)"""

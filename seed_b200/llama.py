@@ -371,7 +371,7 @@ class LlamaForCausalLM(nn.Module):
     _GEN_DEFAULTS = {"max_new_tokens": 20, "do_sample": False, "temperature": 1.0, "top_p": 1.0, "num_beams": 1,
                      "length_penalty": 1.0, "early_stopping": False, "num_return_sequences": 1,
                      "top_k": 0, "repetition_penalty": 1.0, "no_repeat_ngram_size": 0, "min_length": 0,
-                     "min_new_tokens": 0}
+                     "min_new_tokens": 0, "penalty_alpha": None}
 
     @staticmethod
     def _controls(opts) -> dict:
@@ -396,7 +396,8 @@ class LlamaForCausalLM(nn.Module):
                  device_loop: Optional[bool] = None, generation_config=None, length_penalty: Optional[float] = None,
                  early_stopping=None, num_return_sequences: Optional[int] = None, top_k: Optional[int] = None,
                  repetition_penalty: Optional[float] = None, no_repeat_ngram_size: Optional[int] = None,
-                 min_length: Optional[int] = None, min_new_tokens: Optional[int] = None, **_):
+                 min_length: Optional[int] = None, min_new_tokens: Optional[int] = None,
+                 penalty_alpha: Optional[float] = None, **_):
         """Call pattern of scripts/seed_llama_inference_8B.py:33 (temperature=1.0, num_beams=1, max_new_tokens=512,
         top_p=0.5, do_sample=True); returns [B, S + n_new] like HF generate.
 
@@ -415,13 +416,18 @@ class LlamaForCausalLM(nn.Module):
         `top_k`, `repetition_penalty`, `no_repeat_ngram_size`, `min_length` and `min_new_tokens` act as transformers
         4.30.2's logits processors and TopK warper, on the device in every path (include/seedb200.h,
         seedb200_logits_params); the defaults turn them off.  Other generation keywords are ignored.
+        `penalty_alpha` > 0 with `top_k` > 1, `num_beams=1` and `do_sample=False` runs transformers 4.30.2's contrastive
+        search on the device (seedb200_llama_contrastive_generate): `top_k` is then the number of candidates (2..8,
+        and it must be given: transformers' default of 50 would mean 50 cache rows), the processors above still
+        apply, and B * top_k rows must fit the handle, which grows as for beams.  With `num_beams` > 1 or
+        `do_sample=True` penalty_alpha is ignored, as in transformers.
         `generation_config` (a transformers GenerationConfig) supplies these fields and its eos / pad ids, and
         explicit keyword arguments override it, as in transformers."""
         given = {"max_new_tokens": max_new_tokens, "do_sample": do_sample, "temperature": temperature, "top_p": top_p,
                  "num_beams": num_beams, "length_penalty": length_penalty, "early_stopping": early_stopping,
                  "num_return_sequences": num_return_sequences, "top_k": top_k,
                  "repetition_penalty": repetition_penalty, "no_repeat_ngram_size": no_repeat_ngram_size,
-                 "min_length": min_length, "min_new_tokens": min_new_tokens}
+                 "min_length": min_length, "min_new_tokens": min_new_tokens, "penalty_alpha": penalty_alpha}
         opts = dict(self._GEN_DEFAULTS)
         if generation_config is not None:
             for name in opts:
@@ -459,6 +465,15 @@ class LlamaForCausalLM(nn.Module):
         length_rules = controls["min_length"] > 0 or controls["min_new_tokens"] > 0
         if length_rules and len(eos_list) > 1:
             raise NotImplementedError("min_length / min_new_tokens with several eos_token_id values are not supported")
+        alpha = opts["penalty_alpha"]
+        if num_beams == 1 and not do_sample and alpha is not None and alpha > 0:
+            top_k_given = top_k is not None or getattr(generation_config, "top_k", None) is not None
+            if not top_k_given:
+                raise ValueError("penalty_alpha > 0 selects contrastive search, which needs `top_k` (the number of "
+                                 "candidates, 2..8): pass top_k explicitly")
+            if controls["top_k"] > 1:
+                return self._contrastive_generate(input_ids, max_new_tokens, controls["top_k"], float(alpha),
+                                                  eos_list, pad, padded, use_graph, controls)
         if num_beams > 1:
             return self._beam_generate(input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p,
                                        float(opts["length_penalty"]), opts["early_stopping"], eos_list, pad, padded,
@@ -520,6 +535,28 @@ class LlamaForCausalLM(nn.Module):
                                          offset=offset, eos_token_id=eos_list[0] if eos_list else -1,
                                          pad_token_id=pad, use_graph=use_graph, **controls)
         self._draws += max_new_tokens
+        self._cache_len, self._cache_batch = 0, 0
+        return torch.cat([input_ids, new], dim=1)
+
+
+    def _contrastive_generate(self, input_ids, max_new_tokens, top_k, penalty_alpha, eos_list, pad, padded, use_graph,
+                              controls):
+        if top_k > 8:
+            raise ValueError(f"top_k={top_k} with penalty_alpha: contrastive search takes at most 8 candidates")
+        if not math.isfinite(penalty_alpha):
+            raise ValueError(f"penalty_alpha must be finite (got {penalty_alpha})")
+        if padded:
+            raise NotImplementedError("a padding attention_mask is not supported with contrastive search")
+        if len(eos_list) > 1:
+            raise NotImplementedError("several eos_token_id values are not supported with contrastive search")
+        B = input_ids.shape[0]
+        if B * top_k > self.max_batch:
+            self._llm.reserve_rows(B * top_k)            # the cache is reallocated: earlier past_key_values are void
+            self.max_batch = B * top_k
+        new = self._llm.contrastive_generate(input_ids, max_new_tokens, top_k, penalty_alpha,
+                                             eos_token_id=eos_list[0] if eos_list else -1, pad_token_id=pad,
+                                             use_graph=use_graph,
+                                             **{k: v for k, v in controls.items() if k != "top_k"})
         self._cache_len, self._cache_batch = 0, 0
         return torch.cat([input_ids, new], dim=1)
 
