@@ -18,7 +18,7 @@ ORACLE_DIR = os.path.join(REPO, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "libvq_oracle.so")
 
 SOURCES = ["capi.cu", "gemm_wgmma.cu", "attention.cu", "rowwise.cu", "vq.cu", "misc.cu", "sampler.cu", "encoder.cu", "llama.cu", "preprocess.cu", "int8.cu", "beam.cu", "lora.cu", "quant4.cu", "contrastive.cu"]
-HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "int8.cuh"), os.path.join(CSRC, "quant4.cuh"), os.path.join(CSRC, "wgmma.cuh"), os.path.join(CSRC, "ops.h"), os.path.join(REPO, "include", "seedb200.h")]
+HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "int8.cuh"), os.path.join(CSRC, "quant4.cuh"), os.path.join(CSRC, "wgmma.cuh"), os.path.join(CSRC, "select.cuh"), os.path.join(CSRC, "ops.h"), os.path.join(REPO, "include", "seedb200.h")]
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [

@@ -10,6 +10,7 @@
 //                         generated tokens by walking the (token, parent) history back
 #include "common.cuh"
 #include "ops.h"
+#include "select.cuh"
 
 namespace sb {
 
@@ -75,7 +76,7 @@ __global__ void beam_init_kernel(BeamParams bp, BeamState s, const long long* pr
   const int g = blockIdx.x * blockDim.x + threadIdx.x, n = gridDim.x * blockDim.x;
   if (g == 0) {
     *s.params = bp;
-    s.state[0] = bp.S; s.state[1] = 0; s.state[2] = 0; s.state[3] = 0; s.state[4] = 0; s.state[5] = 0;
+    gen_state_reset(s.state, bp.S);
   }
   for (int e = g; e < rows; e += n) s.beam_scores[e] = e % bp.k == 0 ? 0.0f : -1e9f;
   for (int e = g; e < bp.B; e += n) { s.done[e] = 0; s.hyp_n[e] = 0; s.worst[e] = 1e9; }
@@ -104,9 +105,10 @@ __global__ void __launch_bounds__(256) beam_score_kernel(const BeamState s, int 
   pdl_wait();
   const BeamParams bp = *s.params;
   const int k = bp.k, n2 = 2 * k, rows = bp.B * k;
-  const int step = s.state[1];
+  const int step = s.state[GS_STEP];
   const int cur_len = bp.S + step;                        // input_ids.shape[-1] before this step's append
-  const int pos = advance_cache ? s.state[0] + 1 : s.state[0];   // where the next decode step appends
+  const int len = s.state[GS_CACHE_LEN];
+  const int pos = advance_cache ? len + 1 : len;          // where the next decode step appends
   if (tid == 0) {
     float nbs[BEAM_MAX];
     long long ntok[BEAM_MAX];
@@ -178,18 +180,12 @@ __global__ void __launch_bounds__(256) beam_score_kernel(const BeamState s, int 
       s.tok[(long long)(i * k + tid) * s.max_seq + cur_len] = (int)s.tokens[i * k + tid];
   }
   __syncthreads();
-  if (tid == 0) {
-    __threadfence();
-    if (atomicAdd(&s.state[2], 1) == bp.B - 1) {          // last sequence of this step: advance the counters
+  if (tid == 0)
+    step_arrive(s.state, bp.B, step, advance_cache != 0, [&] {
       int all = 1;
       for (int q = 0; q < bp.B; ++q) all &= (__ldcg(s.done + q) != 0);
-      s.state[5] = all;
-      s.state[2] = 0;
-      s.state[1] = step + 1;
-      if (advance_cache) s.state[0] += 1;
-      __threadfence();
-    }
-  }
+      s.state[GS_ALL_DONE] = all;
+    });
 }
 
 int beam_score(const BeamState& st, int B, int k, int V, int advance_cache, cudaStream_t stream) {
@@ -204,7 +200,7 @@ beam_finalize_kernel(const BeamState s, long long* __restrict__ out, long long l
   __shared__ int s_maxlen;
   const int i = threadIdx.x;
   const BeamParams bp = *s.params;
-  const int k = bp.k, rows = bp.B * k, steps = s.state[1];
+  const int k = bp.k, rows = bp.B * k, steps = s.state[GS_STEP];
   if (i == 0) s_maxlen = 0;
   __syncthreads();
   int len = 0, beam = 0, step = -1;

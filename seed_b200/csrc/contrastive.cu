@@ -18,34 +18,18 @@
 
 #include "common.cuh"
 #include "ops.h"
+#include "select.cuh"
 
 namespace sb {
 
-constexpr int CAND_THREADS = 1024;
 constexpr int RANK_THREADS = 256;
 constexpr int RANK_WARPS = RANK_THREADS / 32;
 static_assert(RANK_WARPS >= CONTRAST_MAX_K, "one warp per candidate");
 constexpr int RANK_MIN_ROWS = 16;        // context rows per CTA at least: below that, staging the candidates dominates
 constexpr int RANK_MAX_SMEM = 200 * 1024;   // k * hidden fp16: 8 candidates up to hidden 12800
 
-__device__ __forceinline__ bool prob_better(float a, int ia, float b, int ib) { return a > b || (a == b && ia < ib); }
 // torch.max: NaN propagates
 __device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? __int_as_float(0x7fffffff) : fmaxf(a, b); }
-
-__device__ __forceinline__ float cand_block_reduce(float v, float* red, bool is_max) {
-  v = is_max ? warp_max(v) : warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : (is_max ? -INFINITY : 0.0f);
-  if (warp == 0) {
-    t = is_max ? warp_max(t) : warp_sum(t);
-    if (lane == 0) red[0] = t;
-  }
-  __syncthreads();
-  return red[0];
-}
 
 // n(x) = fp16(float(x) / float(fp16(sqrt(sum of float(x)^2)))), one warp per row of H halves (H % 8 == 0, 16-byte rows)
 __device__ void normalise_row(const __half* __restrict__ src, __half* __restrict__ dst, int H, int lane) {
@@ -77,80 +61,37 @@ __device__ void normalise_row(const __half* __restrict__ src, __half* __restrict
 struct CandArgs {
   const __half* logits; long long ld; int V;
   ContrastParams p; const ContrastParams* p_dev;
-  const int* state; int pos;           // candidates' position p: state[0] when state is given
+  const int* state; int pos;           // candidates' position p: state[GS_CACHE_LEN] when state is given
   int* slot; int max_seq;              // optional lineage table [B*k, max_seq]
   long long* ids; __half* probs;       // [B*k]
 };
 
-__global__ void __launch_bounds__(CAND_THREADS) contrastive_candidates_kernel(const CandArgs a) {
-  __shared__ float red[CAND_THREADS / 32];
-  __shared__ int redi[CAND_THREADS / 32];
+__global__ void __launch_bounds__(SEL_THREADS) contrastive_candidates_kernel(const CandArgs a) {
+  __shared__ float red[SEL_WARPS];
+  __shared__ int redi[SEL_WARPS];
   __shared__ float s_key[CONTRAST_MAX_K];
   __shared__ int s_idx[CONTRAST_MAX_K];
-  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int b = blockIdx.x, tid = threadIdx.x;
   pdl_trigger();
   pdl_wait();
   const int k = a.p_dev ? a.p_dev->k : a.p.k;
   const int V = a.V;
   const __half* row = a.logits + (long long)b * a.ld;
-  const int per = (V + CAND_THREADS - 1) / CAND_THREADS;
+  const int per = (V + SEL_THREADS - 1) / SEL_THREADS;
   const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
   float mx = -INFINITY;
   for (int i = i0; i < i1; ++i) mx = fmaxf(mx, __half2float(row[i]));
-  mx = cand_block_reduce(mx, red, true);
-  float z = 0.0f;
-  for (int i = i0; i < i1; ++i) z += expf(__half2float(row[i]) - mx);
-  const float inv = 1.0f / cand_block_reduce(z, red, false);
+  mx = block_max(mx, red);
+  const float inv = 1.0f / block_exp_sum(row, i0, i1, mx, red);
   // softmax in fp16: torch's CUDA epilogue exp(x - max) * fp32(1 / sum), one rounding
-  float kv[CONTRAST_MAX_K];
-  int ki[CONTRAST_MAX_K];
-#pragma unroll
-  for (int q = 0; q < CONTRAST_MAX_K; ++q) { kv[q] = -INFINITY; ki[q] = 0x7fffffff; }
-  for (int i = i0; i < i1; ++i) {
-    float ck = __half2float(__float2half_rn(expf(__half2float(row[i]) - mx) * inv));
-    int ci = i;
-#pragma unroll
-    for (int q = 0; q < CONTRAST_MAX_K; ++q) {
-      if (prob_better(ck, ci, kv[q], ki[q])) {
-        const float tk = kv[q]; const int ti = ki[q];
-        kv[q] = ck; ki[q] = ci; ck = tk; ci = ti;
-      }
-    }
-  }
-  for (int r = 0; r < k; ++r) {
-    float bk = kv[0];
-    int bi = ki[0];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ok = __shfl_xor_sync(0xffffffffu, bk, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (prob_better(ok, oi, bk, bi)) { bk = ok; bi = oi; }
-    }
-    __syncthreads();
-    if (lane == 0) { red[warp] = bk; redi[warp] = bi; }
-    __syncthreads();
-    if (warp == 0) {
-      bk = red[lane]; bi = redi[lane];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ok = __shfl_xor_sync(0xffffffffu, bk, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (prob_better(ok, oi, bk, bi)) { bk = ok; bi = oi; }
-      }
-      if (lane == 0) { s_key[r] = bk; s_idx[r] = bi; }
-    }
-    __syncthreads();
-    if (ki[0] == s_idx[r] && ki[0] != 0x7fffffff) {
-#pragma unroll
-      for (int q = 0; q + 1 < CONTRAST_MAX_K; ++q) { kv[q] = kv[q + 1]; ki[q] = ki[q + 1]; }
-      kv[CONTRAST_MAX_K - 1] = -INFINITY; ki[CONTRAST_MAX_K - 1] = 0x7fffffff;
-    }
-  }
+  BestList<CONTRAST_MAX_K> best;
+  for (int i = i0; i < i1; ++i) best.insert(__half2float(__float2half_rn(expf(__half2float(row[i]) - mx) * inv)), i);
+  best.pop_rounds(k, red, redi, s_key, s_idx);
   if (tid < k) {
     const int r = b * k + tid;
     a.ids[r] = s_idx[tid];
     a.probs[r] = __float2half_rn(s_key[tid]);
-    const int pos = a.state ? a.state[0] : a.pos;
+    const int pos = a.state ? a.state[GS_CACHE_LEN] : a.pos;
     if (a.slot != nullptr && pos < a.max_seq) a.slot[(long long)r * a.max_seq + pos] = r;
   }
 }
@@ -166,7 +107,7 @@ int contrastive_candidates(const void* logits, int64_t ld, int B, int V, const C
   if (p) a.p = *p;
   a.p_dev = p_dev; a.state = state; a.pos = pos; a.slot = slot; a.max_seq = max_seq;
   a.ids = reinterpret_cast<long long*>(ids); a.probs = static_cast<__half*>(probs);
-  SB_CHECK_CUDA(launch_chain(contrastive_candidates_kernel, dim3(B), dim3(CAND_THREADS), 0, stream, a));
+  SB_CHECK_CUDA(launch_chain(contrastive_candidates_kernel, dim3(B), dim3(SEL_THREADS), 0, stream, a));
   SB_LAUNCH_CHECK();
   return 0;
 }
@@ -179,7 +120,7 @@ struct RankArgs {
   const __half* h;                     // [B*k, H] candidates' final hidden states
   const __half* probs;                 // [B*k]
   ContrastParams p; const ContrastParams* p_dev;
-  int* state; int pos;                 // p = context rows: state[0] when state is given (the loop's counters)
+  int* state; int pos;                 // p = context rows: state[GS_CACHE_LEN] when state is given (the loop's counters)
   float* part; int* tickets; int G;    // [B, G, CONTRAST_MAX_K] per-CTA maxima; [B] arrival counters, left 0
   int* sel; float* score;              // optional [B], [B*k]
   // the generation loop's bookkeeping (state != NULL)
@@ -202,7 +143,7 @@ __global__ void __launch_bounds__(RANK_THREADS) contrastive_rank_kernel(const Ra
   pdl_wait();
   const ContrastParams cp = a.p_dev ? *a.p_dev : a.p;
   const int k = cp.k, H = a.H;
-  const int P = a.state ? a.state[0] : a.pos;
+  const int P = a.state ? a.state[GS_CACHE_LEN] : a.pos;
   const int rpc = max(RANK_MIN_ROWS, (P + a.G - 1) / a.G);
   const int r0 = cta * rpc, r1 = min(P, r0 + rpc);
   const bool active = r0 < r1;
@@ -310,22 +251,10 @@ __global__ void __launch_bounds__(RANK_THREADS) contrastive_rank_kernel(const Ra
   }
   if (tid < k && P < a.max_seq) a.slot[(long long)(b * k + tid) * a.max_seq + P] = r;
   if (tid == 0) {
-    const int step = a.state[1];
-    long long tok = a.cand_ids[r];
-    const bool was_unfinished = a.finished[b] == 0;
-    if (!was_unfinished) tok = a.gp->pad;                    // HF: next * unfinished + pad * (1 - unfinished)
-    else if (a.gp->eos >= 0 && tok == a.gp->eos) a.finished[b] = 1;
-    a.out[(long long)b * a.out_ld + a.gp->proc.S + step] = tok;
-    if (was_unfinished) atomicOr(&a.state[4], 1);
-    __threadfence();
-    if (atomicAdd(&a.state[2], 1) == a.B - 1) {             // last sequence of this step: advance the counters
-      if (atomicOr(&a.state[4], 0) != 0) a.state[3] = step + 1;
-      a.state[4] = 0;
-      a.state[2] = 0;
-      a.state[1] = step + 1;
-      a.state[0] += 1;
-      __threadfence();
-    }
+    const int step = a.state[GS_STEP];
+    bool was_unfinished;
+    emit_token(a.cand_ids[r], b, step, *a.gp, a.finished, a.out, a.out_ld, &was_unfinished);
+    seq_arrive(a.state, a.B, step, true, was_unfinished);
   }
 }
 

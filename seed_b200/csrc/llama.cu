@@ -25,6 +25,7 @@
 
 #include "common.cuh"
 #include "ops.h"
+#include "select.cuh"
 
 namespace sb {
 enum WeightFormat { W_F16, W_INT8, W_4BIT };
@@ -59,7 +60,7 @@ struct seedb200_llama {
   int device;
   // ---- device-resident generation loop (seedb200_llama_generate) ----
   int vpad;                       // logits row stride: vocab rounded up to a multiple of 8
-  int* gstate;                    // {cache length, step, arrive counter, valid steps, any-unfinished flag}
+  int* gstate;                    // [GS_SLOTS] the run's step counters
   int* gfinished;                 // [max_batch]
   int64_t* gtok;                  // [max_batch] token fed to the next decode forward
   int64_t* gout;                  // [max_batch, max_seq] each row's tokens: the prompt (kept when a history control
@@ -352,13 +353,13 @@ static int llama_build(seedb200_llama* m) {
     SB_PROPAGATE(llama_alloc(m->owned, &m->ocount, 1));
   }
   m->vpad = (c.vocab + 7) / 8 * 8;
-  SB_PROPAGATE(llama_alloc(m->owned, &m->gstate, 8));
+  SB_PROPAGATE(llama_alloc(m->owned, &m->gstate, GS_SLOTS));
   SB_PROPAGATE(llama_alloc(m->owned, &m->gparams, 1));
   SB_PROPAGATE(llama_alloc(m->owned, &m->beam.params, 1));
   SB_PROPAGATE(llama_alloc(m->owned, &m->beam.n_out, 1));
   SB_PROPAGATE(llama_alloc(m->owned, &m->c_params, 1));
   SB_PROPAGATE(llama_alloc_rows(m, st));
-  SB_CHECK_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->gstate_host), 8 * sizeof(int)));
+  SB_CHECK_CUDA(cudaMallocHost(reinterpret_cast<void**>(&m->gstate_host), GS_SLOTS * sizeof(int)));
   SB_CHECK_CUDA(cudaStreamCreateWithFlags(&m->gstream, cudaStreamNonBlocking));
   SB_CHECK_CUDA(cudaStreamSynchronize(st));
   return 0;
@@ -506,9 +507,41 @@ static int llama_forward(seedb200_llama* m, const int64_t* input_ids, const void
 __global__ void gen_reset_kernel(GenParams gp, GenParams* dst, int* state, int* finished, int past_len, int B) {
   if (threadIdx.x == 0) {
     *dst = gp;
-    state[0] = past_len; state[1] = 0; state[2] = 0; state[3] = 0; state[4] = 0;
+    gen_state_reset(state, past_len);
   }
   if (threadIdx.x < B) finished[threadIdx.x] = 0;
+}
+
+// the prologue of the sampler and contrastive loops: the parameters and the counters on the device, and the prompt as
+// the rows' history in gout[:, :S] when a history control reads it (the loop appends from column S)
+static int gen_begin(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, const GenParams& gp, cudaStream_t st) {
+  gen_reset_kernel<<<1, (B + 31) / 32 * 32, 0, st>>>(gp, m->gparams, m->gstate, m->gfinished, S, B);
+  SB_LAUNCH_CHECK();
+  if (logits_history_active(gp.proc))
+    SB_CHECK_CUDA(cudaMemcpy2DAsync(m->gout, (size_t)m->cfg.max_seq * 8, prompt_ids, (size_t)S * 8, (size_t)S * 8, B,
+                                    cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+static int gen_state_read(seedb200_llama* m, cudaStream_t st) {
+  SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, GS_SLOTS * sizeof(int), cudaMemcpyDeviceToHost, st));
+  SB_CHECK_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// the epilogue of the sampler and contrastive loops: n_valid steps ran; with an eos id, the steps HF keeps are
+// GS_VALID.  Their tokens go to tokens_out [B, max_new] (optional).
+static int gen_end(seedb200_llama* m, int B, int S, int max_new, int64_t eos, int n_valid, int64_t* tokens_out,
+                   int* n_generated_host, cudaStream_t st) {
+  if (eos >= 0) {
+    SB_PROPAGATE(gen_state_read(m, st));
+    n_valid = m->gstate_host[GS_VALID];
+  }
+  if (tokens_out != nullptr && n_valid > 0)
+    SB_CHECK_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)max_new * 8, m->gout + S, (size_t)m->cfg.max_seq * 8,
+                                    (size_t)n_valid * 8, B, cudaMemcpyDeviceToDevice, st));
+  if (n_generated_host != nullptr) *n_generated_host = n_valid;
+  return 0;
 }
 
 // the history processors of the step: on the sampler's rows (history = gout) or on every beam row (history = the
@@ -601,11 +634,14 @@ static int gen_capture(seedb200_llama* m, int B, int beams, int proc, int contra
   return 0;
 }
 
+// when a loop with an eos id stops early: a step ran with every sequence already finished, or every beam search is done
+enum GenStop { STOP_NEVER, STOP_ALL_FINISHED, STOP_BEAMS_DONE };
+
 // run `units` decode units (the first eagerly, the rest replayed from the (B, beams, proc, contrast) graph when
-// use_graph); with `poll`, the device flag state[poll] is read every 32 units and the loop stops once it is set.
+// use_graph); unless STOP_NEVER, the counters are read every 32 units and the loop ends once `stop` holds.
 // Returns units run.
 static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int contrast, int units, int use_graph,
-                         int poll, cudaStream_t st, int* done_out) {
+                         GenStop stop, cudaStream_t st, int* done_out) {
   int done = 0;
   m->used_graph = 0;
   if (units > 0) {   // first unit eagerly (also resolves every lazily-set function attribute before a capture)
@@ -625,10 +661,10 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int cont
     }
     m->used_graph = 1;
   }
-  bool stop = false;
-  while (done < units && !stop) {
+  bool stopped = false;
+  while (done < units && !stopped) {
     int chunk = units - done;
-    if (poll >= 0 && chunk > 32) chunk = 32;
+    if (stop != STOP_NEVER && chunk > 32) chunk = 32;
     for (int i = 0; i < chunk; ++i) {
       if (m->used_graph) {
         const auto& g = m->graphs[key];
@@ -639,10 +675,10 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int cont
       }
     }
     done += chunk;
-    if (poll >= 0 && done < units) {
-      SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
-      SB_CHECK_CUDA(cudaStreamSynchronize(st));
-      stop = poll == 3 ? m->gstate_host[3] < m->gstate_host[1] : m->gstate_host[poll] != 0;
+    if (stop != STOP_NEVER && done < units) {
+      SB_PROPAGATE(gen_state_read(m, st));
+      const int* g = m->gstate_host;
+      stopped = stop == STOP_ALL_FINISHED ? g[GS_VALID] < g[GS_STEP] : g[GS_ALL_DONE] != 0;
     }
   }
   *done_out = done;
@@ -658,12 +694,7 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
   gp.sp = *sp; gp.eos = eos; gp.pad = pad;
   gp.proc = logits_proc(lp, eos, S);
   const int proc = logits_history_active(gp.proc) ? 1 : 0;
-  gen_reset_kernel<<<1, 32, 0, st>>>(gp, m->gparams, m->gstate, m->gfinished, S, B);
-  SB_LAUNCH_CHECK();
-  // the rows' history: the prompt in gout[:, :S]; the sampler appends from column S
-  if (proc)
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(m->gout, (size_t)c.max_seq * 8, prompt_ids, (size_t)S * 8, (size_t)S * 8, B,
-                                    cudaMemcpyDeviceToDevice, st));
+  SB_PROPAGATE(gen_begin(m, prompt_ids, B, S, gp, st));
   // prefill: cache rows [0, S), logits of the last position only (what the sampler needs)
   SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, m->vpad, st));
   if (proc) SB_PROPAGATE(gen_process(m, B, 0, 0, st));
@@ -671,18 +702,9 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
   SB_PROPAGATE(sample(m->glogits, m->vpad, B, c.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/0, m->gtok,
                       m->gout, c.max_seq, m->gfinished, st));
   int done = 0;
-  // early stop (only with an eos id): a step ran with every sequence already finished (state[3] < state[1])
-  SB_PROPAGATE(gen_run_units(m, B, 0, proc, 0, max_new - 1, use_graph, eos >= 0 ? 3 : -1, st, &done));
-  int n_valid = done + 1;
-  if (eos >= 0) {
-    SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    SB_CHECK_CUDA(cudaStreamSynchronize(st));
-    n_valid = m->gstate_host[3];
-  }
-  if (tokens_out != nullptr)
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)max_new * 8, m->gout + S, (size_t)c.max_seq * 8, (size_t)n_valid * 8, B,
-                                    cudaMemcpyDeviceToDevice, st));
-  if (n_generated_host != nullptr) *n_generated_host = n_valid;
+  SB_PROPAGATE(gen_run_units(m, B, 0, proc, 0, max_new - 1, use_graph, eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st,
+                             &done));
+  SB_PROPAGATE(gen_end(m, B, S, max_new, eos, done + 1, tokens_out, n_generated_host, st));
   m->gen_cache_len = S + done;     // tokens whose K/V are in the cache
   return 0;
 }
@@ -706,7 +728,8 @@ static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int
                            m->beam.cand_idx, st));
   SB_PROPAGATE(beam_score(m->beam, B, k, c.vocab, /*advance_cache=*/0, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, B, k, bp.processed, 0, max_new - 1, use_graph, eos >= 0 ? 5 : -1, st, &done));
+  SB_PROPAGATE(gen_run_units(m, B, k, bp.processed, 0, max_new - 1, use_graph, eos >= 0 ? STOP_BEAMS_DONE : STOP_NEVER,
+                             st, &done));
   SB_PROPAGATE(beam_finalize(m->beam, B, tokens_out, max_new, best_scores, st));
   int n_out = 0;
   SB_CHECK_CUDA(cudaMemcpyAsync(&n_out, m->beam.n_out, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -739,26 +762,14 @@ static int llama_contrastive_generate(seedb200_llama* m, const int64_t* prompt_i
   gp.proc = logits_proc(lp, eos, S);
   gp.proc.lp.top_k = 0;                           // the candidate count, not a warper
   const int proc = logits_history_active(gp.proc) ? 1 : 0;
-  gen_reset_kernel<<<1, (B + 31) / 32 * 32, 0, st>>>(gp, m->gparams, m->gstate, m->gfinished, S, B);
-  SB_LAUNCH_CHECK();
-  if (proc)
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(m->gout, (size_t)c.max_seq * 8, prompt_ids, (size_t)S * 8, (size_t)S * 8, B,
-                                    cudaMemcpyDeviceToDevice, st));
+  SB_PROPAGATE(gen_begin(m, prompt_ids, B, S, gp, st));
   SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->c_logits, m->vpad, st));
   SB_PROPAGATE(contrastive_context_init(m->hn, B, S, c.hidden, m->c_ctx, (int64_t)c.max_seq * c.hidden, m->beam.slot,
                                         p.k, c.max_seq, p, m->c_params, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, B, p.k, proc, 1, max_new, use_graph, eos >= 0 ? 3 : -1, st, &done));
-  int n_valid = done;
-  if (eos >= 0) {
-    SB_CHECK_CUDA(cudaMemcpyAsync(m->gstate_host, m->gstate, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    SB_CHECK_CUDA(cudaStreamSynchronize(st));
-    n_valid = m->gstate_host[3];
-  }
-  if (tokens_out != nullptr && n_valid > 0)
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(tokens_out, (size_t)max_new * 8, m->gout + S, (size_t)c.max_seq * 8,
-                                    (size_t)n_valid * 8, B, cudaMemcpyDeviceToDevice, st));
-  if (n_generated_host != nullptr) *n_generated_host = n_valid;
+  SB_PROPAGATE(gen_run_units(m, B, p.k, proc, 1, max_new, use_graph, eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st,
+                             &done));
+  SB_PROPAGATE(gen_end(m, B, S, max_new, eos, done, tokens_out, n_generated_host, st));
   m->gen_cache_len = 0;            // the cache rows now hold candidate lineages, not B plain sequences
   return 0;
 }
@@ -780,6 +791,15 @@ static int llama_linears_ready(const seedb200_llama* m) {
                   (int)(i / 7), kLinear[i % 7].name);
       return SEEDB200_ERR_INVALID;
     }
+  return 0;
+}
+
+// the checks the three generation entry points share, reported under `who`
+static int gen_args_check(const char* who, const seedb200_llama* m, const int64_t* prompt_ids, const void* params,
+                          int S, int max_new) {
+  SB_REQUIRE(m && prompt_ids && params, "%s: null argument", who);
+  SB_REQUIRE(S >= 1 && max_new >= 1 && S + max_new <= m->cfg.max_seq, "%s: prompt %d + %d new tokens exceeds max_seq %d",
+             who, S, max_new, m->cfg.max_seq);
   return 0;
 }
 
@@ -932,11 +952,9 @@ int seedb200_llama_generate_processed(seedb200_llama* llm, const int64_t* prompt
                                       int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
                                       void* stream, const seedb200_logits_params* lp) {
   SB_PROPAGATE(sb::logits_params_check("llama_generate", lp));
-  SB_REQUIRE(llm && prompt_ids && sp, "llama_generate: null argument");
+  SB_PROPAGATE(sb::gen_args_check("llama_generate", llm, prompt_ids, sp, S, max_new_tokens));
   SB_REQUIRE(B >= 1 && B <= llm->cfg.max_batch && B <= 4, "llama_generate: batch %d outside [1,%d] (decode GEMV: <= 4 rows)",
              B, llm->cfg.max_batch < 4 ? llm->cfg.max_batch : 4);
-  SB_REQUIRE(S >= 1 && max_new_tokens >= 1 && S + max_new_tokens <= llm->cfg.max_seq,
-             "llama_generate: prompt %d + %d new tokens exceeds max_seq %d", S, max_new_tokens, llm->cfg.max_seq);
   SB_REQUIRE(!sp->do_sample || (sp->temperature > 0.0f && sp->top_p > 0.0f), "llama_generate: temperature and top_p must be > 0");
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
@@ -958,14 +976,13 @@ int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* p
                                            int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
                                            float* best_scores_out, void* stream, const seedb200_logits_params* lp) {
   SB_PROPAGATE(sb::logits_params_check("llama_beam_generate", lp));
-  SB_REQUIRE(llm && prompt_ids && bp && tokens_out, "llama_beam_generate: null argument");
+  SB_PROPAGATE(sb::gen_args_check("llama_beam_generate", llm, prompt_ids, bp, S, max_new_tokens));
+  SB_REQUIRE(tokens_out != nullptr, "llama_beam_generate: null argument");
   SB_REQUIRE(bp->num_beams >= 1 && bp->num_beams <= sb::BEAM_MAX, "llama_beam_generate: num_beams %d outside [1,%d]",
              bp->num_beams, sb::BEAM_MAX);
   SB_REQUIRE(B >= 1 && (int64_t)B * bp->num_beams <= llm->cfg.max_batch,
              "llama_beam_generate: batch %d x %d beams exceeds max_batch %d (seedb200_llama_reserve_rows)", B,
              bp->num_beams, llm->cfg.max_batch);
-  SB_REQUIRE(S >= 1 && max_new_tokens >= 1 && S + max_new_tokens <= llm->cfg.max_seq,
-             "llama_beam_generate: prompt %d + %d new tokens exceeds max_seq %d", S, max_new_tokens, llm->cfg.max_seq);
   SB_REQUIRE(!bp->do_sample || (bp->temperature > 0.0f && bp->top_p > 0.0f),
              "llama_beam_generate: temperature and top_p must be > 0 when sampling");
   SB_REQUIRE(bp->early_stopping >= 0 && bp->early_stopping <= 2, "llama_beam_generate: early_stopping %d not in {0,1,2}",
@@ -983,13 +1000,10 @@ int seedb200_llama_contrastive_generate(seedb200_llama* llm, const int64_t* prom
                                         void* stream, const seedb200_logits_params* lp) {
   SB_PROPAGATE(sb::contrastive_params_check("llama_contrastive_generate", cp));
   SB_PROPAGATE(sb::logits_params_check("llama_contrastive_generate", lp));
-  SB_REQUIRE(llm && prompt_ids, "llama_contrastive_generate: null argument");
+  SB_PROPAGATE(sb::gen_args_check("llama_contrastive_generate", llm, prompt_ids, cp, S, max_new_tokens));
   SB_REQUIRE(B >= 1 && B <= 1024 && (int64_t)B * cp->top_k <= llm->cfg.max_batch,
              "llama_contrastive_generate: batch %d x top_k %d exceeds max_batch %d (seedb200_llama_reserve_rows)", B,
              cp->top_k, llm->cfg.max_batch);
-  SB_REQUIRE(S >= 1 && max_new_tokens >= 1 && S + max_new_tokens <= llm->cfg.max_seq,
-             "llama_contrastive_generate: prompt %d + %d new tokens exceeds max_seq %d", S, max_new_tokens,
-             llm->cfg.max_seq);
   SB_REQUIRE(eos_id < llm->cfg.vocab, "llama_contrastive_generate: eos_id %lld outside the vocabulary",
              (long long)eos_id);
   SB_REQUIRE(llm->cfg.vocab >= sb::CONTRAST_MAX_K, "llama_contrastive_generate: vocabulary below %d",

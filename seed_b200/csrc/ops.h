@@ -52,9 +52,21 @@ int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int 
                           float scale, cudaStream_t stream, const int* dyn = nullptr, const int* slot = nullptr);
 // slot (optional, device) [B, max_seq] int32: cached key / value p of row b lives in cache row slot[b*max_seq + p]
 // (beam lineage); NULL = row b.  The new token is still appended at row b.
+// The device counters of a generation run: int[GS_SLOTS], one array per LLaMA handle.  Every kernel of a decode unit
+// reads them at run time, which is what lets one captured graph replay every step.  The run's first launch
+// (gen_reset_kernel, beam_init_kernel) sets GS_CACHE_LEN to the prompt length and zeroes the other slots; after that
+// they change only through the arrival at the end of each step (step_arrive / seq_arrive in select.cuh).
+//   GS_CACHE_LEN   K/V positions in the cache
+//   GS_STEP        the step being generated
+//   GS_ARRIVE      sequences that have ended the current step
+//   GS_VALID       steps HF keeps: last step with an unfinished sequence + 1 (sampler and contrastive loops)
+//   GS_UNFINISHED  some sequence was unfinished at the current step (sampler and contrastive loops)
+//   GS_ALL_DONE    every sequence's beam search is done (beam loop)
+enum GenSlot { GS_CACHE_LEN, GS_STEP, GS_ARRIVE, GS_VALID, GS_UNFINISHED, GS_ALL_DONE, GS_SLOTS };
+static_assert(GS_CACHE_LEN == 0, "the decode forward reads the cache length as dyn[0]");
 // sampler.cu
 // logits processors (seedb200_logits_params) with the eos id they mask and the prompt length S: the history of a
-// row is its first L tokens, L = S + state[1] in the device loops (the prompt, then one token per step)
+// row is its first L tokens, L = S + state[GS_STEP] in the device loops (the prompt, then one token per step)
 struct LogitsProc { seedb200_logits_params lp; long long eos; int S; };
 inline LogitsProc logits_proc(const seedb200_logits_params* p, long long eos, int S) {
   LogitsProc r;
@@ -72,15 +84,15 @@ inline bool logits_history_active(const LogitsProc& p) {
 int logits_params_check(const char* who, const seedb200_logits_params* p);   // NULL passes
 // out[b, proc.S + step] = token (the device loop keeps the prompt in out[b, 0:S])
 struct GenParams { seedb200_sample_params sp; long long eos, pad; LogitsProc proc; };
-// gp (host, by value) or gp_dev (device, read at run time); state (device, optional) = {cache length, step, arrive,
-// valid steps, flag}: the step index comes from state[1] and the last CTA advances the counters.
+// gp (host, by value) or gp_dev (device, read at run time); state (device, optional): the GenSlot counters, which
+// give the step and which the last CTA advances.
 int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, const GenParams* gp_dev, uint64_t step,
            int* state, int advance_cache, int64_t* tokens, int64_t* out, int64_t out_ld, int* finished,
            cudaStream_t stream);
 // the history processors, in place on fp16 rows, one CTA per row.  Row (sequence i, beam j) = logits + i * seq_ld +
 // j * beam_ld, its history = hist + (i * hist_rows + j) * hist_ld, j < beams.  log_softmax: the row holds logits and
-// is first replaced by fp16 log_softmax (beam search).  p (host) or p_dev (device); L = p.S + state[1] when state is
-// given, else hist_len.  Tok = int64 (sampler) or int32 (beam token table).
+// is first replaced by fp16 log_softmax (beam search).  p (host) or p_dev (device); L = p.S + state[GS_STEP] when
+// state is given, else hist_len.  Tok = int64 (sampler) or int32 (beam token table).
 template <typename Tok>
 int logits_process(void* logits, int64_t seq_ld, int64_t beam_ld, int B, int beams, int V, const LogitsProc* p,
                    const LogitsProc* p_dev, const int* state, const Tok* hist, int64_t hist_ld, int hist_rows,
@@ -113,7 +125,7 @@ int beam_select(const void* logits, int64_t seq_ld, int64_t beam_ld, int B, int 
 // the device state of one beam-search run (rows = B * k <= max_batch; hyps: k per sequence)
 struct BeamState {
   BeamParams* params;
-  int* state;            // {cache length, step, arrive counter, -, -, all sequences done}
+  int* state;            // the GenSlot counters
   float* beam_scores;    // [rows]
   float* row_stats;      // [rows, 5] per-row statistics of the candidate kernel
   float* cand_score;     // [rows * 2]
@@ -147,7 +159,7 @@ struct ContrastParams { int k; float c_prob, c_pen; };   // c_prob = fp32(1 - al
 int contrastive_params_check(const char* who, const seedb200_contrastive_params* cp);   // NULL is refused
 ContrastParams contrast_params(const seedb200_contrastive_params& cp);
 // candidates of B rows (logits + b * ld): ids / probs [B*k]; p (host) or p_dev (device); slot (optional)
-// [B*k, max_seq] gets slot[r, pos] = r with pos = state[0] when state is given
+// [B*k, max_seq] gets slot[r, pos] = r with pos = state[GS_CACHE_LEN] when state is given
 int contrastive_candidates(const void* logits, int64_t ld, int B, int V, const ContrastParams* p,
                            const ContrastParams* p_dev, const int* state, int pos, int* slot, int max_seq,
                            int64_t* ids, void* probs, cudaStream_t stream);

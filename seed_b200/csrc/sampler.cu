@@ -15,10 +15,9 @@
 
 #include "common.cuh"
 #include "ops.h"
+#include "select.cuh"
 
 namespace sb {
-
-constexpr int SAMP_THREADS = 1024;
 
 // ---- Philox4x32-10 (Salmon et al., SC'11) -- same constants as cuRAND / torch's Philox -----------------------------
 __host__ __device__ inline void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
@@ -55,30 +54,15 @@ struct SampleArgs {
   GenParams gp;                        // sampling parameters + eos/pad by value, or ...
   const GenParams* gp_dev;             // ... read from device memory when non-null (graph replay)
   unsigned long long step;             // Philox offset of this call = sp.offset + step, or ...
-  int* state;                          // ... state[1] when non-null: device counters {cache length, step, arrive,
-                                       //     valid steps, any-unfinished flag}, advanced by the last CTA to finish
-  int advance_cache;                   // also bump state[0] (a decode forward consumed the previous token)
+  int* state;                          // ... state[GS_STEP] when non-null: the GenSlot counters, advanced by the last
+                                       //     CTA to finish
+  int advance_cache;                   // also bump the cache length (a decode forward consumed the previous token)
   long long* tokens;                   // [B] next token per sequence (also the next step's input ids)
   long long* out; long long out_ld;    // optional [B, out_ld] history: out[b, gp.proc.S + step] = token (columns
                                        //     [0, S) hold the prompt when a history control reads it)
   int* finished;                       // optional [B]: sequences that already produced eos emit pad (HF semantics)
   int B;
 };
-
-__device__ __forceinline__ float block_sum(float v, float* red) {
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  float t = (threadIdx.x < SAMP_THREADS / 32) ? red[threadIdx.x] : 0.0f;
-  if (warp == 0) {
-    t = warp_sum(t);
-    if (lane == 0) red[0] = t;
-  }
-  __syncthreads();
-  return red[0];
-}
 
 // nucleus threshold (TopPLogitsWarper in threshold form): the smallest t with mass{p > t} < target, found by bisection
 // over the float bit pattern of p in (0, 1] (31 block reductions); kept = {p >= t}.  prob(i) is this thread's p_i over
@@ -145,10 +129,10 @@ struct ProcArgs {
 };
 
 template <typename Tok>
-__global__ void __launch_bounds__(SAMP_THREADS)
+__global__ void __launch_bounds__(SEL_THREADS)
 logits_process_kernel(const ProcArgs<Tok> a) {
   extern __shared__ uint32_t s_seen[];       // one bit per vocabulary id: the row's distinct history tokens
-  __shared__ float red[SAMP_THREADS / 32];
+  __shared__ float red[SEL_WARPS];
   const int j = blockIdx.x, sq = blockIdx.y, tid = threadIdx.x;
   pdl_trigger();
   pdl_wait();
@@ -156,41 +140,29 @@ logits_process_kernel(const ProcArgs<Tok> a) {
   const int V = a.V;
   __half* row = a.logits + (long long)sq * a.seq_ld + (long long)j * a.beam_ld;
   const Tok* h = a.hist + ((long long)sq * a.hist_rows + j) * a.hist_ld;
-  const int L = a.state ? p.S + a.state[1] : a.hist_len;
+  const int L = a.state ? p.S + a.state[GS_STEP] : a.hist_len;
   if (a.log_softmax) {
     // lp = fp16((x - max) - logZ): beam_row_stats_kernel's arithmetic (same chunks, same reduction order)
-    const int per = (V + SAMP_THREADS - 1) / SAMP_THREADS;
+    const int per = (V + SEL_THREADS - 1) / SEL_THREADS;
     const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
     float m = -INFINITY;
     for (int i = i0; i < i1; ++i) m = fmaxf(m, __half2float(row[i]));
-    m = warp_max(m);
-    __shared__ float s_m;
-    if ((tid & 31) == 0) red[tid >> 5] = m;
-    __syncthreads();
-    if (tid < 32) {
-      float t = red[tid];
-      t = warp_max(t);
-      if (tid == 0) s_m = t;
-    }
-    __syncthreads();
-    m = s_m;
-    float z = 0.0f;
-    for (int i = i0; i < i1; ++i) z += expf(__half2float(row[i]) - m);
-    const float lz = logf(block_sum(z, red));
+    m = block_max(m, red);
+    const float lz = logf(block_exp_sum(row, i0, i1, m, red));
     for (int i = i0; i < i1; ++i) row[i] = __float2half_rn((__half2float(row[i]) - m) - lz);
   }
   const int nw = (V + 31) >> 5;
   const float pen = p.lp.repetition_penalty;
   if (pen != 1.0f) {
-    for (int w = tid; w < nw; w += SAMP_THREADS) s_seen[w] = 0u;
+    for (int w = tid; w < nw; w += SEL_THREADS) s_seen[w] = 0u;
     __syncthreads();
-    for (int t = tid; t < L; t += SAMP_THREADS) {
+    for (int t = tid; t < L; t += SEL_THREADS) {
       const long long tok = (long long)h[t];
       if (tok >= 0 && tok < V) atomicOr(&s_seen[tok >> 5], 1u << (tok & 31));
     }
     __syncthreads();
     const float inv = 1.0f / pen;            // torch: fp16 tensor / Python scalar = x * fp32 reciprocal
-    for (int w = tid; w < nw; w += SAMP_THREADS) {
+    for (int w = tid; w < nw; w += SEL_THREADS) {
       uint32_t bits = s_seen[w];
       while (bits) {
         const int t = (w << 5) + __ffs(bits) - 1;
@@ -203,7 +175,7 @@ logits_process_kernel(const ProcArgs<Tok> a) {
   __syncthreads();                           // the bans below overwrite penalised entries
   const int n = p.lp.no_repeat_ngram_size;
   if (n > 0 && L + 1 >= n) {
-    for (int i = tid; i <= L - n; i += SAMP_THREADS) {
+    for (int i = tid; i <= L - n; i += SEL_THREADS) {
       bool match = true;
       for (int q = 0; q + 1 < n && match; ++q) match = h[i + q] == h[L - n + 1 + q];
       const long long tok = (long long)h[i + n - 1];
@@ -228,7 +200,7 @@ int logits_process(void* logits, int64_t seq_ld, int64_t beam_ld, int B, int bea
   if (p) a.p = *p;
   a.p_dev = p_dev; a.state = state; a.hist = hist; a.hist_ld = hist_ld; a.hist_rows = hist_rows;
   a.hist_len = hist_len; a.log_softmax = log_softmax ? 1 : 0;
-  SB_CHECK_CUDA(launch_chain(logits_process_kernel<Tok>, dim3(beams, B), dim3(SAMP_THREADS), smem, stream, a));
+  SB_CHECK_CUDA(launch_chain(logits_process_kernel<Tok>, dim3(beams, B), dim3(SEL_THREADS), smem, stream, a));
   SB_LAUNCH_CHECK();
   return 0;
 }
@@ -248,53 +220,34 @@ int logits_params_check(const char* who, const seedb200_logits_params* p) {
   return 0;
 }
 
-__global__ void __launch_bounds__(SAMP_THREADS)
+__global__ void __launch_bounds__(SEL_THREADS)
 sample_kernel(const SampleArgs a) {
-  __shared__ float red[SAMP_THREADS / 32];
-  __shared__ float red_v[SAMP_THREADS / 32];
-  __shared__ int red_i[SAMP_THREADS / 32];
-  __shared__ float scan[SAMP_THREADS];
+  __shared__ float red[SEL_WARPS];
+  __shared__ int red_i[SEL_WARPS];
+  __shared__ float scan[SEL_THREADS];
   __shared__ unsigned s_hist[256];
   __shared__ int s_sel[2];
   __shared__ int s_pick;
-  const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int b = blockIdx.x, tid = threadIdx.x;
   pdl_trigger();
   pdl_wait();
   const GenParams gp = a.gp_dev ? *a.gp_dev : a.gp;
   const seedb200_sample_params sp = gp.sp;
-  const unsigned long long step = a.state ? (unsigned long long)a.state[1] : a.step;
+  const unsigned long long step = a.state ? (unsigned long long)a.state[GS_STEP] : a.step;
   const __half* row = a.logits + (long long)b * a.ld;
   const int V = a.V;
   // contiguous chunk per thread (the CDF inversion below walks tokens in index order)
-  const int per = (V + SAMP_THREADS - 1) / SAMP_THREADS;
+  const int per = (V + SEL_THREADS - 1) / SEL_THREADS;
   const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
 
   // ---- argmax (ties -> lowest index), also the softmax max ----
   float mx = -INFINITY; int mi = 0x7fffffff;
   for (int i = i0; i < i1; ++i) {
     const float x = __half2float(row[i]);
-    if (x > mx || (x == mx && i < mi)) { mx = x; mi = i; }
+    if (key_better(x, i, mx, mi)) { mx = x; mi = i; }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, mx, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, mi, o);
-    if (ov > mx || (ov == mx && oi < mi)) { mx = ov; mi = oi; }
-  }
-  if (lane == 0) { red_v[warp] = mx; red_i[warp] = mi; }
-  __syncthreads();
-  if (warp == 0) {
-    mx = red_v[lane]; mi = red_i[lane];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ov = __shfl_xor_sync(0xffffffffu, mx, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, mi, o);
-      if (ov > mx || (ov == mx && oi < mi)) { mx = ov; mi = oi; }
-    }
-    if (lane == 0) { red_v[0] = mx; red_i[0] = mi; }
-  }
-  __syncthreads();
-  mx = red_v[0]; mi = red_i[0];
+  block_best(mx, mi, red, red_i, &red[0], &red_i[0]);
+  mx = red[0]; mi = red_i[0];
   if (mi == 0x7fffffff) mi = 0;
   int pick = mi;
 
@@ -340,13 +293,13 @@ sample_kernel(const SampleArgs a) {
     scan[tid] = k;
     __syncthreads();
     // inclusive scan of the 1024 per-thread masses (Hillis-Steele in shared memory)
-    for (int o = 1; o < SAMP_THREADS; o <<= 1) {
+    for (int o = 1; o < SEL_THREADS; o <<= 1) {
       const float add = tid >= o ? scan[tid - o] : 0.0f;
       __syncthreads();
       scan[tid] += add;
       __syncthreads();
     }
-    const float K = scan[SAMP_THREADS - 1];
+    const float K = scan[SEL_THREADS - 1];
     const float u = philox_uniform(sp.seed, sp.offset + step, (uint32_t)b) * K;     // (0, K]
     if (tid == 0) s_pick = -1;
     __syncthreads();
@@ -366,27 +319,9 @@ sample_kernel(const SampleArgs a) {
   }
 
   if (tid == 0) {
-    long long tok = pick;
-    bool was_unfinished = true;
-    if (a.finished != nullptr) {
-      was_unfinished = a.finished[b] == 0;
-      if (!was_unfinished) tok = gp.pad;                       // HF: next_tokens * unfinished + pad * (1 - unfinished)
-      else if (gp.eos >= 0 && tok == gp.eos) a.finished[b] = 1;
-    }
-    a.tokens[b] = tok;
-    if (a.out != nullptr) a.out[(long long)b * a.out_ld + gp.proc.S + (long long)step] = tok;
-    if (a.state != nullptr) {
-      if (was_unfinished) atomicOr(&a.state[4], 1);
-      __threadfence();
-      if (atomicAdd(&a.state[2], 1) == a.B - 1) {       // last sequence of this step: publish the new position
-        if (atomicOr(&a.state[4], 0) != 0) a.state[3] = (int)step + 1;   // steps HF would have kept (it stops once all finished)
-        a.state[4] = 0;
-        a.state[2] = 0;
-        a.state[1] = (int)step + 1;
-        if (a.advance_cache) a.state[0] += 1;
-        __threadfence();
-      }
-    }
+    bool was_unfinished;
+    a.tokens[b] = emit_token(pick, b, (long long)step, gp, a.finished, a.out, a.out_ld, &was_unfinished);
+    if (a.state != nullptr) seq_arrive(a.state, a.B, (int)step, a.advance_cache != 0, was_unfinished);
   }
 }
 
@@ -406,7 +341,7 @@ int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, co
   a.tokens = reinterpret_cast<long long*>(tokens);
   a.out = reinterpret_cast<long long*>(out); a.out_ld = out_ld;
   a.finished = finished; a.B = B;
-  SB_CHECK_CUDA(launch_chain(sample_kernel, dim3(B), dim3(SAMP_THREADS), 0, stream, a));
+  SB_CHECK_CUDA(launch_chain(sample_kernel, dim3(B), dim3(SEL_THREADS), 0, stream, a));
   SB_LAUNCH_CHECK();
   return 0;
 }
@@ -427,8 +362,6 @@ struct BeamSelectArgs {
   float* cand_score; int* cand_idx;    // [B, 2k]
 };
 
-__device__ __forceinline__ bool cand_better(float a, int ia, float b, int ib) { return a > b || (a == b && ia < ib); }
-
 // s = float(fp16 log_softmax(x)) + beam score; a processed row already holds the fp16 log_softmax
 __device__ __forceinline__ float beam_s(bool processed, float x, float mx, float lz, float bs) {
   return processed ? x + bs : __half2float(__float2half_rn((x - mx) - lz)) + bs;
@@ -441,10 +374,10 @@ __device__ __forceinline__ void top2_merge(float& m1, float& m2, float o1, float
 }
 
 // one CTA per (beam row j, sequence i): the row's statistics, so that the k rows of a sequence run on k SMs
-__global__ void __launch_bounds__(SAMP_THREADS)
+__global__ void __launch_bounds__(SEL_THREADS)
 beam_row_stats_kernel(const BeamSelectArgs a) {
-  __shared__ float red[SAMP_THREADS / 32];
-  __shared__ float red2[SAMP_THREADS / 32];
+  __shared__ float red[SEL_WARPS];
+  __shared__ float red2[SEL_WARPS];
   const int j = blockIdx.x, sq = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   pdl_trigger();
   pdl_wait();
@@ -452,7 +385,7 @@ beam_row_stats_kernel(const BeamSelectArgs a) {
   const int k = bp.k, V = a.V;
   if (j >= k) return;
   const float T = bp.temperature;
-  const int per = (V + SAMP_THREADS - 1) / SAMP_THREADS;
+  const int per = (V + SEL_THREADS - 1) / SEL_THREADS;
   const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
   const __half* row = a.logits + (long long)sq * a.seq_ld + (long long)j * a.beam_ld;
   float m1 = -INFINITY, m2 = -INFINITY;
@@ -473,11 +406,7 @@ beam_row_stats_kernel(const BeamSelectArgs a) {
   m1 = red[0]; m2 = red2[0];
   const bool processed = bp.processed != 0;
   float lz = 0.0f;
-  if (!processed) {
-    float z = 0.0f;
-    for (int i = i0; i < i1; ++i) z += expf(__half2float(row[i]) - m1);
-    lz = logf(block_sum(z, red));
-  }
+  if (!processed) lz = logf(block_exp_sum(row, i0, i1, m1, red));
   const float bsc = a.beam_scores[sq * k + j];
   // s = float(fp16 log_softmax) + beam score, fp32 (processed rows hold the fp16 log_softmax already)
   auto score = [&](float x) { return beam_s(processed, x, m1, lz, bsc); };
@@ -514,18 +443,18 @@ beam_row_stats_kernel(const BeamSelectArgs a) {
 }
 
 template <int NC>
-__global__ void __launch_bounds__(SAMP_THREADS)
+__global__ void __launch_bounds__(SEL_THREADS)
 beam_select_kernel(const BeamSelectArgs a) {
-  __shared__ float red[SAMP_THREADS / 32];
-  __shared__ int redi[SAMP_THREADS / 32];
+  __shared__ float red[SEL_WARPS];
+  __shared__ int redi[SEL_WARPS];
   __shared__ float s_mx[BEAM_MAX], s_lz[BEAM_MAX], s_bs[BEAM_MAX], s_mxw[BEAM_MAX], s_thr[BEAM_MAX], s_wk[BEAM_MAX];
   __shared__ float s_key[2 * BEAM_MAX];
   __shared__ int s_idx[2 * BEAM_MAX];
-  const int sq = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int sq = blockIdx.x, tid = threadIdx.x;
   pdl_trigger();
   pdl_wait();
   const BeamParams bp = a.bp_dev ? *a.bp_dev : a.bp;
-  const unsigned long long step = a.state ? (unsigned long long)a.state[1] : a.step;
+  const unsigned long long step = a.state ? (unsigned long long)a.state[GS_STEP] : a.step;
   const int k = bp.k, n2 = 2 * k, V = a.V;
   const bool samp = bp.do_sample != 0, processed = bp.processed != 0;
   const float T = bp.temperature;
@@ -538,13 +467,10 @@ beam_select_kernel(const BeamSelectArgs a) {
   }
   __syncthreads();
   // ---- per-thread best NC candidates, flat index f = j * V + t in increasing order ----
-  float kv[NC];
-  int ki[NC];
-#pragma unroll
-  for (int q = 0; q < NC; ++q) { kv[q] = -INFINITY; ki[q] = 0x7fffffff; }
+  BestList<NC> best;
   for (int j = 0; j < k; ++j) {
     const __half* row = rowp(j);
-    for (int t = tid; t < V; t += SAMP_THREADS) {
+    for (int t = tid; t < V; t += SEL_THREADS) {
       const float sc = score(j, __half2float(row[t]));
       const int f = j * V + t;
       float key = sc;
@@ -557,47 +483,10 @@ beam_select_kernel(const BeamSelectArgs a) {
           key = w + (-logf(-logf(u)));
         }
       }
-      float ck = key;
-      int ci = f;
-#pragma unroll
-      for (int q = 0; q < NC; ++q) {
-        if (cand_better(ck, ci, kv[q], ki[q])) {
-          const float tk = kv[q]; const int ti = ki[q];
-          kv[q] = ck; ki[q] = ci; ck = tk; ci = ti;
-        }
-      }
+      best.insert(key, f);
     }
   }
-  // ---- 2k rounds: the best head of all threads wins and is popped ----
-  for (int r = 0; r < n2; ++r) {
-    float bk = kv[0];
-    int bi = ki[0];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const float ok = __shfl_xor_sync(0xffffffffu, bk, o);
-      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (cand_better(ok, oi, bk, bi)) { bk = ok; bi = oi; }
-    }
-    __syncthreads();
-    if (lane == 0) { red[warp] = bk; redi[warp] = bi; }
-    __syncthreads();
-    if (warp == 0) {
-      bk = red[lane]; bi = redi[lane];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ok = __shfl_xor_sync(0xffffffffu, bk, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (cand_better(ok, oi, bk, bi)) { bk = ok; bi = oi; }
-      }
-      if (lane == 0) { s_key[r] = bk; s_idx[r] = bi; }
-    }
-    __syncthreads();
-    if (ki[0] == s_idx[r] && ki[0] != 0x7fffffff) {
-#pragma unroll
-      for (int q = 0; q + 1 < NC; ++q) { kv[q] = kv[q + 1]; ki[q] = ki[q + 1]; }
-      kv[NC - 1] = -INFINITY; ki[NC - 1] = 0x7fffffff;
-    }
-  }
+  best.pop_rounds(n2, red, redi, s_key, s_idx);     // 2k rounds: the best head of all threads wins and is popped
   if (tid != 0) return;
   // the scorer receives s (greedy) or w (sampling), the draws sorted by w descending, ties to the lowest index
   float sc[2 * BEAM_MAX];
@@ -609,7 +498,7 @@ beam_select_kernel(const BeamSelectArgs a) {
     const float v = score(j, __half2float(rowp(j)[f - j * V]));
     float w = samp ? v / T : v;
     int q = r;
-    while (q > 0 && cand_better(w, f, sc[q - 1], ix[q - 1])) { sc[q] = sc[q - 1]; ix[q] = ix[q - 1]; --q; }
+    while (q > 0 && key_better(w, f, sc[q - 1], ix[q - 1])) { sc[q] = sc[q - 1]; ix[q] = ix[q - 1]; --q; }
     sc[q] = w; ix[q] = f;
   }
   for (int r = 0; r < n2; ++r) {
@@ -637,11 +526,11 @@ int beam_select(const void* logits, int64_t seq_ld, int64_t beam_ld, int B, int 
   if (bp) a.bp = *bp;
   a.bp_dev = bp_dev; a.step = step; a.state = state; a.row_stats = row_stats;
   a.cand_score = cand_score; a.cand_idx = cand_idx;
-  SB_CHECK_CUDA(launch_chain(beam_row_stats_kernel, dim3(k, B), dim3(SAMP_THREADS), 0, stream, a));
+  SB_CHECK_CUDA(launch_chain(beam_row_stats_kernel, dim3(k, B), dim3(SEL_THREADS), 0, stream, a));
   SB_LAUNCH_CHECK();
   const int n2 = 2 * k;
   auto kern = n2 <= 4 ? beam_select_kernel<4> : (n2 <= 8 ? beam_select_kernel<8> : beam_select_kernel<16>);
-  SB_CHECK_CUDA(launch_chain(kern, dim3(B), dim3(SAMP_THREADS), 0, stream, a));
+  SB_CHECK_CUDA(launch_chain(kern, dim3(B), dim3(SEL_THREADS), 0, stream, a));
   SB_LAUNCH_CHECK();
   return 0;
 }
