@@ -524,7 +524,8 @@ int seedb200_llama_forward_ld(seedb200_llama* llm, const int64_t* input_ids, con
  * launches eagerly.  Sequences that emitted eos_id (>= 0) produce pad_id afterwards (HF semantics).  With an
  * eos_id the call synchronises the stream every 32 steps to stop early once every sequence has finished;
  * without one it only enqueues.  tokens_out [B, max_new_tokens] int64 (device); *n_generated_host (may be NULL)
- * receives the number of valid columns.  Returns an error when B > 4 (the decode step uses the <= 4-row GEMV). */
+ * receives the number of valid columns.  B <= max_batch (see seedb200_llama_reserve_rows); a call is
+ * seedb200_llama_generate_n with num_return_sequences = 1. */
 int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
                             const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id, int use_graph,
                             int64_t* tokens_out, int* n_generated_host, void* stream);
@@ -535,6 +536,22 @@ int seedb200_llama_generate_processed(seedb200_llama* llm, const int64_t* prompt
                                       int max_new_tokens, const seedb200_sample_params* sp, int64_t eos_id,
                                       int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
                                       void* stream, const seedb200_logits_params* lp);
+/* num_return_sequences = n samples per prompt (transformers 4.30.2 generate(do_sample=True, num_return_sequences=n),
+ * which expands the inputs n times): R = B * n rows, prompt-major, row b * n + j is sample j of prompt b.  Each
+ * prompt is prefilled once, at cache row b; row r reads prompt r / n's K/V through the lineage table and appends its
+ * own from position S on, so the prompt's K/V are written once per prompt.  Every row samples on its own: Philox row
+ * r, its own eos / pad state and its own history for the controls, so the tokens equal those of a call on
+ * prompt_ids.repeat_interleave(n, 0) with n = 1.  n = 1 issues the launches of seedb200_llama_generate.
+ * tokens_out [R, max_new_tokens].  Refused with SEEDB200_ERR_INVALID before any device work: n < 1, R > max_batch,
+ * R > 1024.  With n > 1 the cache rows hold lineages afterwards (as after beam search).                            */
+int seedb200_llama_generate_n(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                              int num_return_sequences, const seedb200_sample_params* sp, int64_t eos_id,
+                              int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream);
+int seedb200_llama_generate_n_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                        int max_new_tokens, int num_return_sequences,
+                                        const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id,
+                                        int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream,
+                                        const seedb200_logits_params* lp);
 /* 1 when the last generate() replayed a captured graph, 0 when it ran eagerly, -1 before any call */
 int seedb200_llama_generate_used_graph(seedb200_llama* llm);
 /* Beam search / beam sampling (see seedb200_beam_params) of prompt_ids [B,S] (device int64): prefill at B cache rows,
@@ -554,6 +571,24 @@ int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* p
                                            int max_new_tokens, const seedb200_beam_params* bp, int64_t eos_id,
                                            int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
                                            float* best_scores_out, void* stream, const seedb200_logits_params* lp);
+/* Beam sampling with num_return_sequences = n, as transformers 4.30.2 runs it: BeamSearchScorer(batch_size = B * n,
+ * num_beams = k) keeping one hypothesis per search, and inputs expanded k * n times.  So each prompt gets n
+ * independent beam-sample searches and each returns its best hypothesis; n may exceed k.  (Later transformers
+ * releases return the top n hypotheses of one search instead; that is not what this computes.)  Search g = b * n + j
+ * (prompt-major) reads prompt b, prefilled once at cache row b, through the lineage table, and draws from Philox
+ * sequence g, so the tokens equal those of a call on prompt_ids.repeat_interleave(n, 0) with n = 1.
+ * tokens_out [B * n, max_new_tokens], best_scores_out [B * n].  B * n * k <= max_batch.  Refused with
+ * SEEDB200_ERR_INVALID before any device work: n < 1, n > 1 with bp->do_sample == 0 (beam search keeps refusing it),
+ * rows above max_batch, B * n > 1024.  n = 1 is seedb200_llama_beam_generate{,_processed}.                       */
+int seedb200_llama_beam_generate_n(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                                   int num_return_sequences, const seedb200_beam_params* bp, int64_t eos_id,
+                                   int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
+                                   float* best_scores_out, void* stream);
+int seedb200_llama_beam_generate_n_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                             int max_new_tokens, int num_return_sequences,
+                                             const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id,
+                                             int use_graph, int64_t* tokens_out, int* n_out_host,
+                                             float* best_scores_out, void* stream, const seedb200_logits_params* lp);
 /* Contrastive search (generate(penalty_alpha > 0, top_k = k > 1), num_beams 1, no sampling): transformers 4.30.2
  * GenerationMixin.contrastive_search with _ranking_fast, as the reference runs them on CUDA in fp16.  Per sequence b
  * and step t, at position p = S + t:

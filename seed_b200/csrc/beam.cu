@@ -2,7 +2,8 @@
 // BeamSearchScorer.process / BeamHypotheses / finalize, stated in include/seedb200.h next to seedb200_beam_params).
 //
 //   beam_init_kernel      beam scores (0 / -1e9), hypotheses, counters, and the lineage table of the prompt: every beam
-//                         of sequence i reads cache row i for positions < S (the prompt is prefilled once, at B rows)
+//                         of sequence i reads cache row i / gpp for positions < S (each prompt is prefilled once, and
+//                         gpp = num_return_sequences sequences search it)
 //   beam_score_kernel     one CTA per sequence: thread 0 walks the 2k candidates (process + is_done), then the CTA
 //                         gathers the parents' lineage rows and points position `pos` of every beam at its own row,
 //                         where the next decode step appends its K/V
@@ -81,9 +82,9 @@ __global__ void beam_init_kernel(BeamParams bp, BeamState s, const long long* pr
   for (int e = g; e < rows; e += n) s.beam_scores[e] = e % bp.k == 0 ? 0.0f : -1e9f;
   for (int e = g; e < bp.B; e += n) { s.done[e] = 0; s.hyp_n[e] = 0; s.worst[e] = 1e9; }
   for (long long e = g; e < (long long)rows * bp.S; e += n) {
-    const int b = (int)(e / bp.S), p = (int)(e % bp.S);
-    s.slot[(long long)b * s.max_seq + p] = b / bp.k;
-    if (bp.processed) s.tok[(long long)b * s.max_seq + p] = (int)prompt[(long long)(b / bp.k) * bp.S + p];
+    const int b = (int)(e / bp.S), p = (int)(e % bp.S), row = b / bp.k / bp.gpp;
+    s.slot[(long long)b * s.max_seq + p] = row;
+    if (bp.processed) s.tok[(long long)b * s.max_seq + p] = (int)prompt[(long long)row * bp.S + p];
   }
 }
 

@@ -70,7 +70,7 @@ struct seedb200_llama {
   int* gstate_host;               // pinned mirror of gstate (early-stop polling)
   cudaStream_t gstream;           // private stream the decode step is captured on (the caller's may be the legacy
                                   // default stream, which cannot be captured); replays go to the caller's stream
-  // captured decode units per (batch, beams, processing launch present, contrastive): beams 0 = the sampler loop;
+  // captured decode units per (batch, beams, processing launch present, unit kind): beams 0 = the sampler loop;
   // contrastive units use beams = k; value = (graph, kernels inside one unit)
   std::map<std::tuple<int, int, int, int>, std::pair<cudaGraphExec_t, int>> graphs;
   sb::BeamState beam;             // beam-search state (rows = batch * beams <= max_batch)
@@ -512,13 +512,37 @@ __global__ void gen_reset_kernel(GenParams gp, GenParams* dst, int* state, int* 
   if (threadIdx.x < B) finished[threadIdx.x] = 0;
 }
 
+// the lineage table of R = B * n sampling rows that share B prompts (num_return_sequences = n): row r reads prompt
+// row r / n for positions < S and its own row from S on.  Sampling rows never change parent, so it is written once.
+__global__ void sample_lineage_kernel(int* slot, int R, int n, int S, int max_seq) {
+  const long long total = (long long)R * max_seq;
+  for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const int r = (int)(e / max_seq), p = (int)(e - (long long)r * max_seq);
+    slot[e] = p < S ? r / n : r;
+  }
+}
+
 // the prologue of the sampler and contrastive loops: the parameters and the counters on the device, and the prompt as
-// the rows' history in gout[:, :S] when a history control reads it (the loop appends from column S)
-static int gen_begin(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, const GenParams& gp, cudaStream_t st) {
-  gen_reset_kernel<<<1, (B + 31) / 32 * 32, 0, st>>>(gp, m->gparams, m->gstate, m->gfinished, S, B);
+// the rows' history in gout[:, :S] when a history control reads it (the loop appends from column S).  B prompts,
+// n rows each: row r's history starts with prompt r / n.
+static int gen_begin(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, const GenParams& gp, cudaStream_t st,
+                     int n = 1) {
+  const int R = B * n;
+  gen_reset_kernel<<<1, (R + 31) / 32 * 32, 0, st>>>(gp, m->gparams, m->gstate, m->gfinished, S, R);
   SB_LAUNCH_CHECK();
   if (logits_history_active(gp.proc))
-    SB_CHECK_CUDA(cudaMemcpy2DAsync(m->gout, (size_t)m->cfg.max_seq * 8, prompt_ids, (size_t)S * 8, (size_t)S * 8, B,
+    for (int j = 0; j < n; ++j)
+      SB_CHECK_CUDA(cudaMemcpy2DAsync(m->gout + (size_t)j * m->cfg.max_seq, (size_t)n * m->cfg.max_seq * 8, prompt_ids,
+                                      (size_t)S * 8, (size_t)S * 8, B, cudaMemcpyDeviceToDevice, st));
+  return 0;
+}
+
+// the prefill wrote prompt b's logits to glogits row b * n (rows n apart); copy it to rows b * n + 1 .. b * n + n - 1,
+// so that the first step of every row (or beam group) reads its prompt's logits as if the prompt had been expanded
+static int gen_spread_logits(seedb200_llama* m, int B, int n, cudaStream_t st) {
+  const size_t row = (size_t)m->vpad * 2, pitch = (size_t)n * row;
+  for (int j = 1; j < n; ++j)
+    SB_CHECK_CUDA(cudaMemcpy2DAsync(m->glogits + (size_t)j * m->vpad, pitch, m->glogits, pitch, row, B,
                                     cudaMemcpyDeviceToDevice, st));
   return 0;
 }
@@ -578,15 +602,20 @@ static int contrastive_unit(seedb200_llama* m, int B, int k, int proc, cudaStrea
   return contrastive_rank(r, st);
 }
 
+// what a decode unit runs, part of its graph key: the sampler or beam step, a contrastive step, or the sampler step
+// whose rows share their prompts through the lineage table
+enum UnitKind { UNIT_PLAIN, UNIT_CONTRASTIVE, UNIT_SHARED };
+
 // one unit of the loop: cached forward of the tokens in m->gtok, the history processors when `proc`, then the sampler
-// (beams == 0) or the beam candidates and scorer (which also advance the device counters); or, with `contrast`, one
-// contrastive step.  Every launch argument is a handle-owned pointer or a constant: the unit can be captured once per
-// (B, beams, proc, contrast).
-static int gen_unit(seedb200_llama* m, int B, int beams, int proc, int contrast, cudaStream_t st) {
+// (beams == 0) or the beam candidates and scorer (which also advance the device counters); or one contrastive step.
+// Sampler rows of UNIT_SHARED read their prompt through the lineage table (num_return_sequences > 1).  Every launch
+// argument is a handle-owned pointer or a constant: the unit can be captured once per (B, beams, proc, kind).
+static int gen_unit(seedb200_llama* m, int B, int beams, int proc, int kind, cudaStream_t st) {
   PdlScope pdl(get_option("decode_pdl") != 0);
-  if (contrast) return contrastive_unit(m, B, beams, proc, st);
+  if (kind == UNIT_CONTRASTIVE) return contrastive_unit(m, B, beams, proc, st);
   if (beams == 0) {
-    SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B, 1, 0, 1, m->glogits, m->vpad, st, m->gstate));
+    SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B, 1, 0, 1, m->glogits, m->vpad, st, m->gstate,
+                               kind == UNIT_SHARED ? m->beam.slot : nullptr));
     if (proc) SB_PROPAGATE(gen_process(m, B, 0, 0, st));
     SB_PROPAGATE(sample(m->glogits, m->vpad, B, m->cfg.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/1,
                         m->gtok, m->gout, m->cfg.max_seq, m->gfinished, st));
@@ -603,12 +632,12 @@ static int gen_unit(seedb200_llama* m, int B, int beams, int proc, int contrast,
   return 0;
 }
 
-static int gen_capture(seedb200_llama* m, int B, int beams, int proc, int contrast) {
+static int gen_capture(seedb200_llama* m, int B, int beams, int proc, int kind) {
   cudaGraph_t graph = nullptr;
   cudaStream_t st = m->gstream;
   SB_CHECK_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
   const int64_t before = seedb200_launch_count();
-  const int s = gen_unit(m, B, beams, proc, contrast, st);
+  const int s = gen_unit(m, B, beams, proc, kind, st);
   const int unit = (int)(seedb200_launch_count() - before);
   count_launch(-unit);                        // captured, not executed
   const cudaError_t e = cudaStreamEndCapture(st, &graph);
@@ -630,31 +659,31 @@ static int gen_capture(seedb200_llama* m, int B, int beams, int proc, int contra
     cudaGetLastError();
     return SEEDB200_ERR_CUDA;
   }
-  m->graphs[std::make_tuple(B, beams, proc, contrast)] = std::make_pair(exec, unit);
+  m->graphs[std::make_tuple(B, beams, proc, kind)] = std::make_pair(exec, unit);
   return 0;
 }
 
 // when a loop with an eos id stops early: a step ran with every sequence already finished, or every beam search is done
 enum GenStop { STOP_NEVER, STOP_ALL_FINISHED, STOP_BEAMS_DONE };
 
-// run `units` decode units (the first eagerly, the rest replayed from the (B, beams, proc, contrast) graph when
+// run `units` decode units (the first eagerly, the rest replayed from the (B, beams, proc, kind) graph when
 // use_graph); unless STOP_NEVER, the counters are read every 32 units and the loop ends once `stop` holds.
 // Returns units run.
-static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int contrast, int units, int use_graph,
+static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int kind, int units, int use_graph,
                          GenStop stop, cudaStream_t st, int* done_out) {
   int done = 0;
   m->used_graph = 0;
   if (units > 0) {   // first unit eagerly (also resolves every lazily-set function attribute before a capture)
-    SB_PROPAGATE(gen_unit(m, B, beams, proc, contrast, st));
+    SB_PROPAGATE(gen_unit(m, B, beams, proc, kind, st));
     done = 1;
   }
-  const auto key = std::make_tuple(B, beams, proc, contrast);
+  const auto key = std::make_tuple(B, beams, proc, kind);
   if (units > done && use_graph) {
     if (m->graphs.find(key) == m->graphs.end()) {
-      int s = gen_capture(m, B, beams, proc, contrast);
+      int s = gen_capture(m, B, beams, proc, kind);
       if (s != 0 && get_option("decode_pdl") != 0) {   // retry without programmatic launches inside the graph
         seedb200_set_option("decode_pdl", 0);
-        s = gen_capture(m, B, beams, proc, contrast);
+        s = gen_capture(m, B, beams, proc, kind);
         seedb200_set_option("decode_pdl", 1);
       }
       if (s != 0) return s;
@@ -671,7 +700,7 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int cont
         SB_CHECK_CUDA(cudaGraphLaunch(g.first, st));
         count_launch(g.second);
       } else {
-        SB_PROPAGATE(gen_unit(m, B, beams, proc, contrast, st));
+        SB_PROPAGATE(gen_unit(m, B, beams, proc, kind, st));
       }
     }
     done += chunk;
@@ -685,52 +714,63 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int cont
   return 0;
 }
 
-static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, int max_new,
+// B prompts, n = num_return_sequences rows each (R = B * n, prompt-major): the prompts are prefilled once, row r reads
+// prompt r / n's K/V through the lineage table and samples from Philox row r
+static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int n, int S, int max_new,
                           const seedb200_sample_params* sp, int64_t eos, int64_t pad, int use_graph,
                           int64_t* tokens_out, int* n_generated_host, const seedb200_logits_params* lp,
                           cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
+  const int R = B * n;
   GenParams gp;
   gp.sp = *sp; gp.eos = eos; gp.pad = pad;
   gp.proc = logits_proc(lp, eos, S);
   const int proc = logits_history_active(gp.proc) ? 1 : 0;
-  SB_PROPAGATE(gen_begin(m, prompt_ids, B, S, gp, st));
+  SB_PROPAGATE(gen_begin(m, prompt_ids, B, S, gp, st, n));
+  if (n > 1) {
+    const long long blocks = ((long long)R * c.max_seq + 255) / 256;
+    sample_lineage_kernel<<<blocks < 1024 ? (int)blocks : 1024, 256, 0, st>>>(m->beam.slot, R, n, S, c.max_seq);
+    SB_LAUNCH_CHECK();
+  }
   // prefill: cache rows [0, S), logits of the last position only (what the sampler needs)
-  SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, m->vpad, st));
-  if (proc) SB_PROPAGATE(gen_process(m, B, 0, 0, st));
+  SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, (int64_t)n * m->vpad, st));
+  SB_PROPAGATE(gen_spread_logits(m, B, n, st));
+  if (proc) SB_PROPAGATE(gen_process(m, R, 0, 0, st));
   // token 0 comes from the prefill logits: the step counter advances, the cache length does not
-  SB_PROPAGATE(sample(m->glogits, m->vpad, B, c.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/0, m->gtok,
+  SB_PROPAGATE(sample(m->glogits, m->vpad, R, c.vocab, nullptr, m->gparams, 0, m->gstate, /*advance_cache=*/0, m->gtok,
                       m->gout, c.max_seq, m->gfinished, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, B, 0, proc, 0, max_new - 1, use_graph, eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st,
-                             &done));
-  SB_PROPAGATE(gen_end(m, B, S, max_new, eos, done + 1, tokens_out, n_generated_host, st));
-  m->gen_cache_len = S + done;     // tokens whose K/V are in the cache
+  SB_PROPAGATE(gen_run_units(m, R, 0, proc, n > 1 ? UNIT_SHARED : UNIT_PLAIN, max_new - 1, use_graph,
+                             eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st, &done));
+  SB_PROPAGATE(gen_end(m, R, S, max_new, eos, done + 1, tokens_out, n_generated_host, st));
+  m->gen_cache_len = n > 1 ? 0 : S + done;   // tokens whose K/V are in the cache; with n > 1 the rows hold lineages
   return 0;
 }
 
 // beam search: prefill at B rows, candidates + scorer from the prefill logits (every beam reads its sequence's row),
-// then max_new - 1 units of (forward of B * k rows through the lineage table -> candidates -> scorer), then finalize
-static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, int max_new,
+// then max_new - 1 units of (forward of G * k rows through the lineage table -> candidates -> scorer), then finalize.
+// G = B * n sequences (num_return_sequences = n, beam sampling only): sequence g searches prompt g / n on its own.
+static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int n, int S, int max_new,
                                const seedb200_beam_params* p, int64_t eos, int64_t pad, int use_graph,
                                int64_t* tokens_out, int* n_out_host, float* best_scores,
                                const seedb200_logits_params* lp, cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
-  const int k = p->num_beams;
-  const BeamParams bp = beam_params(*p, eos, pad, S, max_new, B, lp);
+  const int k = p->num_beams, G = B * n;
+  const BeamParams bp = beam_params(*p, eos, pad, S, max_new, G, lp, n);
   if (bp.processed && m->beam.tok == nullptr)
     SB_PROPAGATE(llama_alloc(m->row_owned, &m->beam.tok, (size_t)c.max_batch * c.max_seq));
   SB_PROPAGATE(beam_init(m->beam, bp, prompt_ids, st));
-  SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, m->vpad, st));
-  if (bp.processed) SB_PROPAGATE(gen_process(m, B, k, 0, st));
-  SB_PROPAGATE(beam_select(m->glogits, m->vpad, 0, B, k, c.vocab, m->beam.beam_scores, nullptr, m->beam.params, 0,
+  SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->glogits, (int64_t)n * m->vpad, st));
+  SB_PROPAGATE(gen_spread_logits(m, B, n, st));
+  if (bp.processed) SB_PROPAGATE(gen_process(m, G, k, 0, st));
+  SB_PROPAGATE(beam_select(m->glogits, m->vpad, 0, G, k, c.vocab, m->beam.beam_scores, nullptr, m->beam.params, 0,
                            m->gstate, m->beam.row_stats, m->beam.cand_score,
                            m->beam.cand_idx, st));
-  SB_PROPAGATE(beam_score(m->beam, B, k, c.vocab, /*advance_cache=*/0, st));
+  SB_PROPAGATE(beam_score(m->beam, G, k, c.vocab, /*advance_cache=*/0, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, B, k, bp.processed, 0, max_new - 1, use_graph, eos >= 0 ? STOP_BEAMS_DONE : STOP_NEVER,
-                             st, &done));
-  SB_PROPAGATE(beam_finalize(m->beam, B, tokens_out, max_new, best_scores, st));
+  SB_PROPAGATE(gen_run_units(m, G, k, bp.processed, UNIT_PLAIN, max_new - 1, use_graph,
+                             eos >= 0 ? STOP_BEAMS_DONE : STOP_NEVER, st, &done));
+  SB_PROPAGATE(beam_finalize(m->beam, G, tokens_out, max_new, best_scores, st));
   int n_out = 0;
   SB_CHECK_CUDA(cudaMemcpyAsync(&n_out, m->beam.n_out, sizeof(int), cudaMemcpyDeviceToHost, st));
   SB_CHECK_CUDA(cudaStreamSynchronize(st));
@@ -767,8 +807,8 @@ static int llama_contrastive_generate(seedb200_llama* m, const int64_t* prompt_i
   SB_PROPAGATE(contrastive_context_init(m->hn, B, S, c.hidden, m->c_ctx, (int64_t)c.max_seq * c.hidden, m->beam.slot,
                                         p.k, c.max_seq, p, m->c_params, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, B, p.k, proc, 1, max_new, use_graph, eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st,
-                             &done));
+  SB_PROPAGATE(gen_run_units(m, B, p.k, proc, UNIT_CONTRASTIVE, max_new, use_graph,
+                             eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st, &done));
   SB_PROPAGATE(gen_end(m, B, S, max_new, eos, done, tokens_out, n_generated_host, st));
   m->gen_cache_len = 0;            // the cache rows now hold candidate lineages, not B plain sequences
   return 0;
@@ -943,22 +983,42 @@ int seedb200_llama_forward(seedb200_llama* llm, const int64_t* input_ids, const 
 int seedb200_llama_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
                             const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id, int use_graph,
                             int64_t* tokens_out, int* n_generated_host, void* stream) {
-  return seedb200_llama_generate_processed(llm, prompt_ids, B, S, max_new_tokens, sp, eos_id, pad_id, use_graph,
-                                           tokens_out, n_generated_host, stream, nullptr);
+  return seedb200_llama_generate_n_processed(llm, prompt_ids, B, S, max_new_tokens, 1, sp, eos_id, pad_id, use_graph,
+                                             tokens_out, n_generated_host, stream, nullptr);
 }
 
 int seedb200_llama_generate_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
                                       int max_new_tokens, const seedb200_sample_params* sp, int64_t eos_id,
                                       int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
                                       void* stream, const seedb200_logits_params* lp) {
+  return seedb200_llama_generate_n_processed(llm, prompt_ids, B, S, max_new_tokens, 1, sp, eos_id, pad_id, use_graph,
+                                             tokens_out, n_generated_host, stream, lp);
+}
+
+int seedb200_llama_generate_n(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                              int num_return_sequences, const seedb200_sample_params* sp, int64_t eos_id,
+                              int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream) {
+  return seedb200_llama_generate_n_processed(llm, prompt_ids, B, S, max_new_tokens, num_return_sequences, sp, eos_id,
+                                             pad_id, use_graph, tokens_out, n_generated_host, stream, nullptr);
+}
+
+int seedb200_llama_generate_n_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                        int max_new_tokens, int num_return_sequences,
+                                        const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id,
+                                        int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream,
+                                        const seedb200_logits_params* lp) {
+  const int n = num_return_sequences;
+  SB_REQUIRE(n >= 1, "llama_generate: num_return_sequences %d < 1", n);
   SB_PROPAGATE(sb::logits_params_check("llama_generate", lp));
   SB_PROPAGATE(sb::gen_args_check("llama_generate", llm, prompt_ids, sp, S, max_new_tokens));
-  SB_REQUIRE(B >= 1 && B <= llm->cfg.max_batch && B <= 4, "llama_generate: batch %d outside [1,%d] (decode GEMV: <= 4 rows)",
-             B, llm->cfg.max_batch < 4 ? llm->cfg.max_batch : 4);
+  SB_REQUIRE(B >= 1 && (int64_t)B * n <= llm->cfg.max_batch,
+             "llama_generate: batch %d x %d sequences exceeds max_batch %d (seedb200_llama_reserve_rows)", B, n,
+             llm->cfg.max_batch);
+  SB_REQUIRE((int64_t)B * n <= 1024, "llama_generate: batch %d x %d sequences above 1024 rows", B, n);
   SB_REQUIRE(!sp->do_sample || (sp->temperature > 0.0f && sp->top_p > 0.0f), "llama_generate: temperature and top_p must be > 0");
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
-  return sb::llama_generate(llm, prompt_ids, B, S, max_new_tokens, sp, eos_id, pad_id, use_graph, tokens_out,
+  return sb::llama_generate(llm, prompt_ids, B, n, S, max_new_tokens, sp, eos_id, pad_id, use_graph, tokens_out,
                             n_generated_host, lp, static_cast<cudaStream_t>(stream));
 }
 
@@ -967,22 +1027,45 @@ int seedb200_llama_generate_used_graph(seedb200_llama* llm) { return llm ? llm->
 int seedb200_llama_beam_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
                                  const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id, int use_graph,
                                  int64_t* tokens_out, int* n_out_host, float* best_scores_out, void* stream) {
-  return seedb200_llama_beam_generate_processed(llm, prompt_ids, B, S, max_new_tokens, bp, eos_id, pad_id, use_graph,
-                                                tokens_out, n_out_host, best_scores_out, stream, nullptr);
+  return seedb200_llama_beam_generate_n_processed(llm, prompt_ids, B, S, max_new_tokens, 1, bp, eos_id, pad_id,
+                                                  use_graph, tokens_out, n_out_host, best_scores_out, stream, nullptr);
 }
 
 int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
                                            int max_new_tokens, const seedb200_beam_params* bp, int64_t eos_id,
                                            int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
                                            float* best_scores_out, void* stream, const seedb200_logits_params* lp) {
+  return seedb200_llama_beam_generate_n_processed(llm, prompt_ids, B, S, max_new_tokens, 1, bp, eos_id, pad_id,
+                                                  use_graph, tokens_out, n_out_host, best_scores_out, stream, lp);
+}
+
+int seedb200_llama_beam_generate_n(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                                   int num_return_sequences, const seedb200_beam_params* bp, int64_t eos_id,
+                                   int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
+                                   float* best_scores_out, void* stream) {
+  return seedb200_llama_beam_generate_n_processed(llm, prompt_ids, B, S, max_new_tokens, num_return_sequences, bp,
+                                                  eos_id, pad_id, use_graph, tokens_out, n_out_host, best_scores_out,
+                                                  stream, nullptr);
+}
+
+int seedb200_llama_beam_generate_n_processed(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                             int max_new_tokens, int num_return_sequences,
+                                             const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id,
+                                             int use_graph, int64_t* tokens_out, int* n_out_host,
+                                             float* best_scores_out, void* stream, const seedb200_logits_params* lp) {
+  const int n = num_return_sequences;
+  SB_REQUIRE(n >= 1, "llama_beam_generate: num_return_sequences %d < 1", n);
+  SB_REQUIRE(n == 1 || bp == nullptr || bp->do_sample,
+             "llama_beam_generate: num_return_sequences %d > 1 needs beam sampling (do_sample)", n);
   SB_PROPAGATE(sb::logits_params_check("llama_beam_generate", lp));
   SB_PROPAGATE(sb::gen_args_check("llama_beam_generate", llm, prompt_ids, bp, S, max_new_tokens));
   SB_REQUIRE(tokens_out != nullptr, "llama_beam_generate: null argument");
   SB_REQUIRE(bp->num_beams >= 1 && bp->num_beams <= sb::BEAM_MAX, "llama_beam_generate: num_beams %d outside [1,%d]",
              bp->num_beams, sb::BEAM_MAX);
-  SB_REQUIRE(B >= 1 && (int64_t)B * bp->num_beams <= llm->cfg.max_batch,
-             "llama_beam_generate: batch %d x %d beams exceeds max_batch %d (seedb200_llama_reserve_rows)", B,
-             bp->num_beams, llm->cfg.max_batch);
+  SB_REQUIRE(B >= 1 && (int64_t)B * n * bp->num_beams <= llm->cfg.max_batch,
+             "llama_beam_generate: batch %d x %d sequences x %d beams exceeds max_batch %d (seedb200_llama_reserve_rows)",
+             B, n, bp->num_beams, llm->cfg.max_batch);
+  SB_REQUIRE((int64_t)B * n <= 1024, "llama_beam_generate: batch %d x %d sequences above 1024", B, n);
   SB_REQUIRE(!bp->do_sample || (bp->temperature > 0.0f && bp->top_p > 0.0f),
              "llama_beam_generate: temperature and top_p must be > 0 when sampling");
   SB_REQUIRE(bp->early_stopping >= 0 && bp->early_stopping <= 2, "llama_beam_generate: early_stopping %d not in {0,1,2}",
@@ -990,7 +1073,7 @@ int seedb200_llama_beam_generate_processed(seedb200_llama* llm, const int64_t* p
   SB_REQUIRE(eos_id < llm->cfg.vocab, "llama_beam_generate: eos_id %lld outside the vocabulary", (long long)eos_id);
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
-  return sb::llama_beam_generate(llm, prompt_ids, B, S, max_new_tokens, bp, eos_id, pad_id, use_graph, tokens_out,
+  return sb::llama_beam_generate(llm, prompt_ids, B, n, S, max_new_tokens, bp, eos_id, pad_id, use_graph, tokens_out,
                                  n_out_host, best_scores_out, lp, static_cast<cudaStream_t>(stream));
 }
 

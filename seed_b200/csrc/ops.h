@@ -101,6 +101,7 @@ int logits_process(void* logits, int64_t seq_ld, int64_t beam_ld, int B, int bea
 constexpr int BEAM_MAX = 8;
 struct BeamParams {                    // read by the beam kernels at run time (graph replay)
   int k, do_sample, early_stopping, S, max_new, B;
+  int gpp;                             // sequences per prompt: sequence i searches prompt row i / gpp
   float temperature, top_p;
   double length_penalty;
   unsigned long long seed, offset;
@@ -109,10 +110,10 @@ struct BeamParams {                    // read by the beam kernels at run time (
   int processed;                       // 1: the rows already hold the processed fp16 log_softmax (logits_process)
 };
 inline BeamParams beam_params(const seedb200_beam_params& p, long long eos, long long pad, int S, int max_new, int B,
-                              const seedb200_logits_params* lp = nullptr) {
+                              const seedb200_logits_params* lp = nullptr, int gpp = 1) {
   BeamParams b;
   b.k = p.num_beams; b.do_sample = p.do_sample; b.early_stopping = p.early_stopping; b.S = S; b.max_new = max_new;
-  b.B = B; b.temperature = p.temperature; b.top_p = p.top_p; b.length_penalty = p.length_penalty;
+  b.B = B; b.gpp = gpp; b.temperature = p.temperature; b.top_p = p.top_p; b.length_penalty = p.length_penalty;
   b.seed = p.seed; b.offset = p.offset; b.eos = eos; b.pad = pad;
   b.proc = logits_proc(lp, eos, S);
   b.processed = logits_history_active(b.proc) ? 1 : 0;
@@ -147,7 +148,8 @@ struct BeamState {
                          // the first run with a history control and maintained only while params->processed
   int max_seq;
 };
-// prompt [B, S] int64 (device): copied into every beam row of `tok` when bp.processed
+// prompt [B / bp.gpp, S] int64 (device): prompt row i / gpp is the prefix of every beam of sequence i, in the lineage
+// table and (when bp.processed) in `tok`
 int beam_init(const BeamState& st, const BeamParams& bp, const int64_t* prompt, cudaStream_t stream);
 int beam_score(const BeamState& st, int B, int k, int V, int advance_cache, cudaStream_t stream);
 int beam_finalize(const BeamState& st, int B, int64_t* tokens_out, int64_t ld, float* best_scores, cudaStream_t stream);

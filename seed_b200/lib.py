@@ -47,6 +47,8 @@ EXPORTS = [
     "seedb200_sample_processed", "seedb200_llama_generate_processed", "seedb200_llama_beam_generate_processed",
     "seedb200_llama_contrastive_generate", "seedb200_contrastive_candidates", "seedb200_contrastive_rank",
     "seedb200_contrastive_context_init",
+    "seedb200_llama_generate_n", "seedb200_llama_generate_n_processed", "seedb200_llama_beam_generate_n",
+    "seedb200_llama_beam_generate_n_processed",
 ]
 
 DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
@@ -291,6 +293,13 @@ def load() -> C.CDLL:
     lib.seedb200_llama_contrastive_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                                         C.POINTER(ContrastiveParams), C.c_int64, C.c_int64, C.c_int,
                                                         C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(LogitsParams)]
+    lib.seedb200_llama_generate_n.argtypes = (lib.seedb200_llama_generate.argtypes[:5] + [C.c_int]
+                                              + lib.seedb200_llama_generate.argtypes[5:])
+    lib.seedb200_llama_generate_n_processed.argtypes = lib.seedb200_llama_generate_n.argtypes + [C.POINTER(LogitsParams)]
+    lib.seedb200_llama_beam_generate_n.argtypes = (lib.seedb200_llama_beam_generate.argtypes[:5] + [C.c_int]
+                                                   + lib.seedb200_llama_beam_generate.argtypes[5:])
+    lib.seedb200_llama_beam_generate_n_processed.argtypes = (lib.seedb200_llama_beam_generate_n.argtypes
+                                                             + [C.POINTER(LogitsParams)])
     lib.seedb200_contrastive_candidates.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                                     C.c_void_p, C.c_void_p]
     lib.seedb200_contrastive_rank.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
@@ -1231,52 +1240,59 @@ class Llama:
 
     def generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, do_sample: bool = False,
                  temperature: float = 1.0, top_p: float = 1.0, seed: int = 0, offset: int = 0,
-                 eos_token_id: int = -1, pad_token_id: int = 0, use_graph: bool = True, **controls) -> torch.Tensor:
-        """prompt [B,S] int64 (device) -> generated tokens [B, n] (n <= max_new_tokens; shorter only when every
-        sequence hit eos).  Prefill + sampler + cached decode steps, all on the device; see seedb200_llama_generate.
-        `controls`: the keywords of logits_params (top_k, repetition_penalty, ...)."""
+                 eos_token_id: int = -1, pad_token_id: int = 0, use_graph: bool = True,
+                 num_return_sequences: int = 1, **controls) -> torch.Tensor:
+        """prompt [B,S] int64 (device) -> generated tokens [B * num_return_sequences, n] (n <= max_new_tokens; shorter
+        only when every row hit eos), row b * num_return_sequences + j being sample j of prompt b.  Prefill + sampler
+        + cached decode steps, all on the device; see seedb200_llama_generate_n.  Needs B * num_return_sequences <=
+        max_batch (reserve_rows).  `controls`: the keywords of logits_params (top_k, repetition_penalty, ...)."""
         if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
             raise RuntimeError(f"generate: prompt_ids must be int64 on {self.device}")
         prompt_ids = prompt_ids.contiguous()
         B, S = prompt_ids.shape
-        out = torch.empty((B, max_new_tokens), dtype=torch.int64, device=self.device)
+        rs = int(num_return_sequences)
+        out = torch.empty((B * max(rs, 1), max_new_tokens), dtype=torch.int64, device=self.device)
         sp = SampleParams(int(bool(do_sample)), float(temperature), float(top_p), int(seed), int(offset))
         lp = logits_params(**controls)
         n = C.c_int(0)
-        args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(sp), int(eos_token_id),
+        args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, rs, C.byref(sp), int(eos_token_id),
                 int(pad_token_id), int(bool(use_graph)), out.data_ptr(), C.byref(n), stream_ptr(self.device))
         with on(self.device):
             if lp is None:
-                check(load().seedb200_llama_generate(*args), "seedb200_llama_generate")
+                check(load().seedb200_llama_generate_n(*args), "seedb200_llama_generate_n")
             else:
-                check(load().seedb200_llama_generate_processed(*args, C.byref(lp)), "seedb200_llama_generate_processed")
+                check(load().seedb200_llama_generate_n_processed(*args, C.byref(lp)),
+                      "seedb200_llama_generate_n_processed")
         return out[:, :n.value]
 
     def beam_generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, num_beams: int, do_sample: bool = False,
                       temperature: float = 1.0, top_p: float = 1.0, length_penalty: float = 1.0, early_stopping=False,
                       seed: int = 0, offset: int = 0, eos_token_id: int = -1, pad_token_id: int = 0,
-                      use_graph: bool = True, **controls):
-        """prompt [B,S] int64 (device) -> (generated tokens [B, n] of the best hypothesis per sequence, fp32 scores [B]);
-        see seedb200_llama_beam_generate.  Needs B * num_beams <= max_batch (reserve_rows).  `controls`: the
-        keywords of logits_params."""
+                      use_graph: bool = True, num_return_sequences: int = 1, **controls):
+        """prompt [B,S] int64 (device) -> (generated tokens [G, n] of the best hypothesis per search, fp32 scores [G]),
+        G = B * num_return_sequences independent searches, prompt-major (beam sampling only when
+        num_return_sequences > 1); see seedb200_llama_beam_generate_n.  Needs G * num_beams <= max_batch
+        (reserve_rows).  `controls`: the keywords of logits_params."""
         if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
             raise RuntimeError(f"beam_generate: prompt_ids must be int64 on {self.device}")
         prompt_ids = prompt_ids.contiguous()
         B, S = prompt_ids.shape
-        out = torch.empty((B, max_new_tokens), dtype=torch.int64, device=self.device)
-        scores = torch.empty((B,), dtype=torch.float32, device=self.device)
+        rs = int(num_return_sequences)
+        G = B * max(rs, 1)
+        out = torch.empty((G, max_new_tokens), dtype=torch.int64, device=self.device)
+        scores = torch.empty((G,), dtype=torch.float32, device=self.device)
         bp = beam_params(num_beams, do_sample, temperature, top_p, length_penalty, early_stopping, seed, offset)
         lp = logits_params(**controls)
         n = C.c_int(0)
-        args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(bp), int(eos_token_id),
+        args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, rs, C.byref(bp), int(eos_token_id),
                 int(pad_token_id), int(bool(use_graph)), out.data_ptr(), C.byref(n), scores.data_ptr(),
                 stream_ptr(self.device))
         with on(self.device):
             if lp is None:
-                check(load().seedb200_llama_beam_generate(*args), "seedb200_llama_beam_generate")
+                check(load().seedb200_llama_beam_generate_n(*args), "seedb200_llama_beam_generate_n")
             else:
-                check(load().seedb200_llama_beam_generate_processed(*args, C.byref(lp)),
-                      "seedb200_llama_beam_generate_processed")
+                check(load().seedb200_llama_beam_generate_n_processed(*args, C.byref(lp)),
+                      "seedb200_llama_beam_generate_n_processed")
         return out[:, :n.value], scores
 
     def contrastive_generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, top_k: int, penalty_alpha: float,

@@ -410,9 +410,16 @@ class LlamaForCausalLM(nn.Module):
 
         `num_beams` > 1 runs transformers 4.30.2's beam search (`do_sample=False`) or beam sampling (`do_sample=True`)
         on the device (seedb200_llama_beam_generate), with `length_penalty` and `early_stopping` (False / True /
-        "never"); only `num_return_sequences=1`, an unpadded batch and one eos id.  B * num_beams rows must fit the
-        handle: a model built with a smaller `max_batch` grows to it first, which drops the KV cache, so
-        `past_key_values` returned by earlier forward() calls are no longer valid.
+        "never"); only an unpadded batch and one eos id.  B * num_beams rows must fit the handle: a model built with a
+        smaller `max_batch` grows to it first, which drops the KV cache, so `past_key_values` returned by earlier
+        forward() calls are no longer valid.
+        `num_return_sequences` = n > 1 needs `do_sample=True` and returns [B * n, ...], prompt-major (row b * n + j is
+        candidate j of prompt b), as transformers 4.30.2 does.  Sampling runs B * n rows in one device call
+        (seedb200_llama_generate_n) that prefills each prompt once; beam sampling runs n independent searches per
+        prompt, each returning its best hypothesis (seedb200_llama_beam_generate_n).  Both equal, token for token, the
+        same call on `input_ids.repeat_interleave(n, 0)`, and grow the handle to B * n (times num_beams) rows as beams
+        do.  With a padded mask or several eos ids the expanded batch runs through the per-token loop below.  Greedy,
+        beam and contrastive search refuse n > 1.
         `top_k`, `repetition_penalty`, `no_repeat_ngram_size`, `min_length` and `min_new_tokens` act as transformers
         4.30.2's logits processors and TopK warper, on the device in every path (include/seedb200.h,
         seedb200_logits_params); the defaults turn them off.  Other generation keywords are ignored.
@@ -443,8 +450,12 @@ class LlamaForCausalLM(nn.Module):
                                                          float(opts["temperature"]), float(opts["top_p"]))
         num_beams = int(opts["num_beams"])
         controls = self._controls(opts)
-        if int(opts["num_return_sequences"]) != 1:
-            raise NotImplementedError("num_return_sequences > 1 is not supported")
+        n_ret = int(opts["num_return_sequences"])
+        if n_ret < 1:
+            raise ValueError(f"num_return_sequences must be >= 1 (got {n_ret})")
+        if n_ret > 1 and not do_sample:
+            raise NotImplementedError("num_return_sequences > 1 is supported with do_sample=True (sampling and beam "
+                                      "sampling) only, not with greedy, beam or contrastive search")
         if num_beams < 1:
             raise ValueError(f"num_beams must be >= 1 (got {num_beams})")
         if input_ids is None:
@@ -477,20 +488,26 @@ class LlamaForCausalLM(nn.Module):
         if num_beams > 1:
             return self._beam_generate(input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p,
                                        float(opts["length_penalty"]), opts["early_stopping"], eos_list, pad, padded,
-                                       rng_seed, offset, use_graph, controls)
+                                       rng_seed, offset, use_graph, controls, n_ret)
         if device_loop is None:
-            device_loop = (not padded) and len(eos_list) <= 1 and B <= 4
+            device_loop = (not padded) and len(eos_list) <= 1 and (B <= 4 or n_ret > 1)
         if device_loop:
-            if padded or len(eos_list) > 1 or B > 4:
-                raise ValueError("device_loop needs an unpadded batch of <= 4 sequences and at most one eos id")
+            if padded or len(eos_list) > 1:
+                raise ValueError("device_loop needs an unpadded batch and at most one eos id")
+            self._reserve(B * n_ret)
             new = self._llm.generate(input_ids, max_new_tokens, do_sample=do_sample, temperature=temperature,
                                      top_p=top_p, seed=rng_seed, offset=offset,
                                      eos_token_id=eos_list[0] if eos_list else -1, pad_token_id=pad,
-                                     use_graph=use_graph, **controls)
+                                     use_graph=use_graph, num_return_sequences=n_ret, **controls)
             self._draws += max_new_tokens
             self._cache_len, self._cache_batch = 0, 0       # the handle's cache now belongs to that generation
-            return torch.cat([input_ids, new], dim=1)
+            return torch.cat([input_ids.repeat_interleave(n_ret, 0), new], dim=1)
         # ---- HF-shaped loop (padding masks, several eos ids): one forward per token from Python ----
+        if n_ret > 1:   # transformers' _expand_inputs_for_generation: every prompt n_ret times, prompt-major
+            input_ids = input_ids.repeat_interleave(n_ret, 0)
+            attention_mask = attention_mask.repeat_interleave(n_ret, 0) if attention_mask is not None else None
+            B = input_ids.shape[0]
+            self._reserve(B)
         mask = attention_mask.to(self._device) if attention_mask is not None else None
         seq, past = input_ids, None
         unfinished = torch.ones(B, dtype=torch.bool, device=self._device)
@@ -513,8 +530,14 @@ class LlamaForCausalLM(nn.Module):
         self._draws += max_new_tokens
         return seq
 
+    def _reserve(self, rows):
+        """grow the handle to `rows` rows; the cache is reallocated, so earlier past_key_values are void"""
+        if rows > self.max_batch:
+            self._llm.reserve_rows(rows)
+            self.max_batch = rows
+
     def _beam_generate(self, input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p, length_penalty,
-                       early_stopping, eos_list, pad, padded, rng_seed, offset, use_graph, controls):
+                       early_stopping, eos_list, pad, padded, rng_seed, offset, use_graph, controls, n_ret=1):
         if num_beams > 8:
             raise ValueError(f"num_beams={num_beams}: at most 8 beams (the scorer runs one CTA per sequence)")
         if padded:
@@ -526,17 +549,16 @@ class LlamaForCausalLM(nn.Module):
         if do_sample and temperature <= 0.0:
             raise ValueError(f"temperature must be > 0 when sampling (got {temperature})")
         B = input_ids.shape[0]
-        if B * num_beams > self.max_batch:
-            self._llm.reserve_rows(B * num_beams)       # the cache is reallocated: earlier past_key_values are void
-            self.max_batch = B * num_beams
+        self._reserve(B * n_ret * num_beams)
         new, _ = self._llm.beam_generate(input_ids, max_new_tokens, num_beams, do_sample=do_sample,
                                          temperature=temperature if do_sample else 1.0, top_p=top_p,
                                          length_penalty=length_penalty, early_stopping=early_stopping, seed=rng_seed,
                                          offset=offset, eos_token_id=eos_list[0] if eos_list else -1,
-                                         pad_token_id=pad, use_graph=use_graph, **controls)
+                                         pad_token_id=pad, use_graph=use_graph, num_return_sequences=n_ret,
+                                         **controls)
         self._draws += max_new_tokens
         self._cache_len, self._cache_batch = 0, 0
-        return torch.cat([input_ids, new], dim=1)
+        return torch.cat([input_ids.repeat_interleave(n_ret, 0), new], dim=1)
 
 
     def _contrastive_generate(self, input_ids, max_new_tokens, top_k, penalty_alpha, eos_list, pad, padded, use_graph,
@@ -549,10 +571,7 @@ class LlamaForCausalLM(nn.Module):
             raise NotImplementedError("a padding attention_mask is not supported with contrastive search")
         if len(eos_list) > 1:
             raise NotImplementedError("several eos_token_id values are not supported with contrastive search")
-        B = input_ids.shape[0]
-        if B * top_k > self.max_batch:
-            self._llm.reserve_rows(B * top_k)            # the cache is reallocated: earlier past_key_values are void
-            self.max_batch = B * top_k
+        self._reserve(input_ids.shape[0] * top_k)
         new = self._llm.contrastive_generate(input_ids, max_new_tokens, top_k, penalty_alpha,
                                              eos_token_id=eos_list[0] if eos_list else -1, pad_token_id=pad,
                                              use_graph=use_graph,
