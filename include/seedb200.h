@@ -331,6 +331,14 @@ typedef struct seedb200_logits_params {
 int seedb200_sample_processed(void* logits, int64_t ld, int B, int V, const seedb200_sample_params* sp, uint64_t step,
                               int64_t* tokens_out, void* stream, const seedb200_logits_params* lp,
                               const int64_t* history, int64_t hist_ld, int hist_len, int prompt_len, int64_t eos_id);
+/* seedb200_sample_processed that also writes each row's generation score (see seedb200_gen_outputs) to
+ * scores_out + b * scores_ld (fp16 [B, scores_ld], V valid columns); scores_out NULL is seedb200_sample_processed.
+ * Refused with SEEDB200_ERR_INVALID before any device work: scores_ld < V or not a multiple of 8, or a base that is
+ * not 16-byte aligned. */
+int seedb200_sample_scores(void* logits, int64_t ld, int B, int V, const seedb200_sample_params* sp, uint64_t step,
+                           int64_t* tokens_out, void* stream, const seedb200_logits_params* lp,
+                           const int64_t* history, int64_t hist_ld, int hist_len, int prompt_len, int64_t eos_id,
+                           void* scores_out, int64_t scores_ld);
 
 /* Beam search and beam sampling (num_beams > 1), transformers 4.30.2 GenerationMixin.beam_search / beam_sample with
  * BeamSearchScorer(num_beam_hyps_to_keep = 1), the arithmetic the reference pins (requirements.txt:8):
@@ -552,6 +560,48 @@ int seedb200_llama_generate_n_processed(seedb200_llama* llm, const int64_t* prom
                                         const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id,
                                         int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream,
                                         const seedb200_logits_params* lp);
+/* Generation scores, transformers 4.30.2 generate(output_scores=True, return_dict_in_generate=True): one fp16 row of
+ * V scores per generated row and step, written by the kernel that already holds the row (no extra pass).  The row of
+ * step t and row r is scores + (t * R + r) * scores_pitch (halves), R the call's row count; the caller allocates
+ * max_new_tokens * R * scores_pitch halves.  What a row holds:
+ *   greedy     the processed logits: the controls of seedb200_logits_params other than top_k, no warpers
+ *              (4.30.2 greedy_search: next_tokens_scores = logits_processor(input_ids, next_token_logits))
+ *   sampling   the warped row (4.30.2 sample: next_token_scores = logits_warper(...)): fp16(x * fp32(1 / T)), or x
+ *              when T == 1, on the tokens the draw kept (top_k, then top_p, in the threshold form of
+ *              seedb200_sample) and -inf elsewhere
+ *   contrastive the processed logits the candidates are taken from (4.30.2 contrastive_search:
+ *              scores += (logit_for_next_step,), no warpers)
+ *   beam search   (4.30.2 beam_search: scores += (next_token_scores_processed,)) R = G * k beam rows, row g * k + j:
+ *              lp = fp16((x - max) - logZ) of beam j, the processors applied, before the beam score is added.  At step
+ *              0 the k rows of a search are identical (every beam reads the prefill's row).
+ *   beam sampling (4.30.2 beam_sample: scores += (logits_warper(input_ids, next_token_scores_processed),)) the warpers
+ *              on the processed lp row without the beam score: v = fp16(lp * fp32(1 / T)) (lp when T == 1), TopK keeps
+ *              v >= the k'-th largest, k' = min(max(top_k, 2), V), TopP keeps p = exp(v - max v) >= its threshold, at
+ *              least the two largest (min_tokens_to_keep = 2); removed tokens are -inf.  This is not the w = s / T the
+ *              draws use; it costs one more launch per step.
+ * n_steps_out receives the number of entries transformers returns.  Sampling, greedy and contrastive: the valid width
+ * of tokens_out (the loop stops once every row has finished).  Beams: the number of BeamSearchScorer.process calls, the
+ * step at which every search became done + 1, or max_new_tokens; the device records that step, and it may exceed the
+ * valid width.  Rows of later steps may hold scores of steps the early-stop poll ran past; they are not counted.
+ * beam_indices (beam entry point only, optional; NULL elsewhere): int64 [G, S + max_new_tokens], row g written in
+ * full: entry t is the flat beam row in [0, G * k) whose scores row produced token t of the returned hypothesis (4.30.2
+ * BeamSearchScorer: beam_indices[beam_idx] + (beam_idx,)); a hypothesis closed by an eos candidate has one entry more,
+ * the eos step's parent row; -1 after that.
+ * Refused with SEEDB200_ERR_INVALID before any device work: a NULL scores, a scores_pitch < V or not a multiple of 8,
+ * a base that is not 16-byte aligned, a non-NULL beam_indices outside the beam entry point.  The pointers reach the
+ * captured decode step through the device-resident parameters each call rewrites (GenParams, BeamParams), so
+ * consecutive calls may pass different buffers. */
+typedef struct seedb200_gen_outputs {
+  void* scores;              /* fp16, device */
+  int64_t scores_pitch;      /* halves between rows, >= V, a multiple of 8 */
+  int64_t* beam_indices;     /* beams: int64 [G, S + max_new_tokens] (device), optional, and NULL elsewhere */
+  int32_t n_steps_out;       /* written by the call */
+} seedb200_gen_outputs;
+/* seedb200_llama_generate_n_processed with optional outputs (NULL: none, the launches of the call without them). */
+int seedb200_llama_generate_ex(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                               int num_return_sequences, const seedb200_sample_params* sp, int64_t eos_id,
+                               int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream,
+                               const seedb200_logits_params* lp, seedb200_gen_outputs* outputs);
 /* 1 when the last generate() replayed a captured graph, 0 when it ran eagerly, -1 before any call */
 int seedb200_llama_generate_used_graph(seedb200_llama* llm);
 /* Beam search / beam sampling (see seedb200_beam_params) of prompt_ids [B,S] (device int64): prefill at B cache rows,
@@ -589,6 +639,14 @@ int seedb200_llama_beam_generate_n_processed(seedb200_llama* llm, const int64_t*
                                              const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id,
                                              int use_graph, int64_t* tokens_out, int* n_out_host,
                                              float* best_scores_out, void* stream, const seedb200_logits_params* lp);
+/* seedb200_llama_beam_generate_n_processed with optional outputs (seedb200_gen_outputs; NULL: none, the launches of
+ * the call without them).  R = B * n * k beam rows; best_scores_out holds transformers' sequences_scores.  With
+ * outputs and bp->do_sample the decode step has one more launch (the warp of the scores rows) and its own graph. */
+int seedb200_llama_beam_generate_ex(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                                    int num_return_sequences, const seedb200_beam_params* bp, int64_t eos_id,
+                                    int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
+                                    float* best_scores_out, void* stream, const seedb200_logits_params* lp,
+                                    seedb200_gen_outputs* outputs);
 /* Contrastive search (generate(penalty_alpha > 0, top_k = k > 1), num_beams 1, no sampling): transformers 4.30.2
  * GenerationMixin.contrastive_search with _ranking_fast, as the reference runs them on CUDA in fp16.  Per sequence b
  * and step t, at position p = S + t:
@@ -629,6 +687,13 @@ int seedb200_llama_contrastive_generate(seedb200_llama* llm, const int64_t* prom
                                         int max_new_tokens, const seedb200_contrastive_params* cp, int64_t eos_id,
                                         int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
                                         void* stream, const seedb200_logits_params* lp);
+/* seedb200_llama_contrastive_generate with optional outputs (seedb200_gen_outputs; NULL: none, the launches of the
+ * call without them).  R = B rows.  The candidates kernel copies each step's row; no launch is added. */
+int seedb200_llama_contrastive_generate_ex(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                           int max_new_tokens, const seedb200_contrastive_params* cp, int64_t eos_id,
+                                           int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
+                                           void* stream, const seedb200_logits_params* lp,
+                                           seedb200_gen_outputs* outputs);
 /* The three kernels on their own, for tests.  candidates: logits [B, ld] fp16 (V valid, V >= 8) -> ids_out [B*k]
  * int64, probs_out [B*k] fp16.  rank: context [B, ctx_ld] fp16 holding ctx_rows normalised rows of `hidden` per
  * sequence, the first p (>= 1) valid; cand_hidden [B*k, hidden] (raw h_j), cand_probs [B*k] fp16 -> sel_out [B] int32

@@ -186,6 +186,8 @@ __global__ void __launch_bounds__(256) beam_score_kernel(const BeamState s, int 
       int all = 1;
       for (int q = 0; q < bp.B; ++q) all &= (__ldcg(s.done + q) != 0);
       s.state[GS_ALL_DONE] = all;
+      // the steps transformers records: its loop ends after the step at which every search is done
+      if (all && s.state[GS_VALID] == 0) s.state[GS_VALID] = step + 1;
     });
 }
 
@@ -222,10 +224,20 @@ beam_finalize_kernel(const BeamState s, long long* __restrict__ out, long long l
   if (i == 0) *s.n_out = width - bp.S;
   if (i >= bp.B) return;
   long long* row = out + (long long)i * ld;
+  // beam_indices (4.30.2 BeamSearchScorer: beam_indices[beam_idx] + (beam_idx,)): entry t is the flat beam row whose
+  // scores produced token t.  A hypothesis closed by an eos candidate (added before the last step, unlike the running
+  // beams added above) has one entry more: the eos step's parent row.  Then -1 to the end of the row.
+  long long* bi = bp.beam_indices ? bp.beam_indices + (long long)i * bp.bi_ld : nullptr;
+  if (bi != nullptr) {
+    const bool eos_hyp = step + 1 < steps;
+    for (int c = step + 1 + (eos_hyp ? 1 : 0); c < bp.bi_ld; ++c) bi[c] = -1;
+    if (eos_hyp) bi[step + 1] = i * k + beam;
+  }
   for (int t = step; t >= 0; --t) {
     const int b = i * k + beam;
     row[t] = s.hist_tok[(long long)t * rows + b];
     beam = s.hist_par[(long long)t * rows + b];
+    if (bi != nullptr) bi[t] = i * k + beam;
   }
   for (int c = len - bp.S; c < bp.max_new; ++c)
     row[c] = (c == len - bp.S && len < width && bp.eos >= 0) ? bp.eos : bp.pad;

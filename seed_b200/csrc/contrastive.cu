@@ -64,6 +64,8 @@ struct CandArgs {
   const int* state; int pos;           // candidates' position p: state[GS_CACHE_LEN] when state is given
   int* slot; int max_seq;              // optional lineage table [B*k, max_seq]
   long long* ids; __half* probs;       // [B*k]
+  const GenParams* gp_dev;             // optional (with state): the loop's parameters, whose scores buffer receives
+                                       // the row the candidates are taken from
 };
 
 __global__ void __launch_bounds__(SEL_THREADS) contrastive_candidates_kernel(const CandArgs a) {
@@ -79,6 +81,12 @@ __global__ void __launch_bounds__(SEL_THREADS) contrastive_candidates_kernel(con
   const __half* row = a.logits + (long long)b * a.ld;
   const int per = (V + SEL_THREADS - 1) / SEL_THREADS;
   const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
+  // contrastive_search's scores (4.30.2 generation/utils.py: scores += (logit_for_next_step,)): the processed row
+  if (a.gp_dev != nullptr && a.state != nullptr && a.gp_dev->scores != nullptr) {
+    __half* srow = a.gp_dev->scores + (long long)a.state[GS_STEP] * a.gp_dev->scores_step +
+                   (long long)b * a.gp_dev->scores_pitch;
+    for (int i = tid; i < V; i += SEL_THREADS) srow[i] = row[i];
+  }
   float mx = -INFINITY;
   for (int i = i0; i < i1; ++i) mx = fmaxf(mx, __half2float(row[i]));
   mx = block_max(mx, red);
@@ -98,7 +106,7 @@ __global__ void __launch_bounds__(SEL_THREADS) contrastive_candidates_kernel(con
 
 int contrastive_candidates(const void* logits, int64_t ld, int B, int V, const ContrastParams* p,
                            const ContrastParams* p_dev, const int* state, int pos, int* slot, int max_seq,
-                           int64_t* ids, void* probs, cudaStream_t stream) {
+                           int64_t* ids, void* probs, cudaStream_t stream, const GenParams* gp_dev) {
   SB_REQUIRE(logits && ids && probs && (p || p_dev) && B >= 1 && V >= CONTRAST_MAX_K && ld >= V,
              "contrastive_candidates: bad arguments (B %d, V %d >= %d, ld %lld)", B, V, CONTRAST_MAX_K, (long long)ld);
   CandArgs a;
@@ -107,6 +115,7 @@ int contrastive_candidates(const void* logits, int64_t ld, int B, int V, const C
   if (p) a.p = *p;
   a.p_dev = p_dev; a.state = state; a.pos = pos; a.slot = slot; a.max_seq = max_seq;
   a.ids = reinterpret_cast<long long*>(ids); a.probs = static_cast<__half*>(probs);
+  a.gp_dev = gp_dev;
   SB_CHECK_CUDA(launch_chain(contrastive_candidates_kernel, dim3(B), dim3(SEL_THREADS), 0, stream, a));
   SB_LAUNCH_CHECK();
   return 0;

@@ -588,7 +588,7 @@ static int contrastive_unit(seedb200_llama* m, int B, int k, int proc, cudaStrea
     SB_PROPAGATE(logits_process<int64_t>(m->c_logits, m->vpad, 0, B, 1, c.vocab, nullptr, &m->gparams->proc,
                                          m->gstate, m->gout, c.max_seq, 1, 0, false, st));
   SB_PROPAGATE(contrastive_candidates(m->c_logits, m->vpad, B, c.vocab, nullptr, m->c_params, m->gstate, 0,
-                                      m->beam.slot, c.max_seq, m->gtok, m->c_probs, st));
+                                      m->beam.slot, c.max_seq, m->gtok, m->c_probs, st, m->gparams));
   SB_PROPAGATE(llama_forward(m, m->gtok, nullptr, nullptr, B * k, 1, 0, 1, m->glogits, m->vpad, st, m->gstate,
                              m->beam.slot));
   ContrastRank r;
@@ -602,9 +602,9 @@ static int contrastive_unit(seedb200_llama* m, int B, int k, int proc, cudaStrea
   return contrastive_rank(r, st);
 }
 
-// what a decode unit runs, part of its graph key: the sampler or beam step, a contrastive step, or the sampler step
-// whose rows share their prompts through the lineage table
-enum UnitKind { UNIT_PLAIN, UNIT_CONTRASTIVE, UNIT_SHARED };
+// what a decode unit runs, part of its graph key: the sampler or beam step, a contrastive step, the sampler step
+// whose rows share their prompts through the lineage table, or the beam step that also warps beam sampling's scores
+enum UnitKind { UNIT_PLAIN, UNIT_CONTRASTIVE, UNIT_SHARED, UNIT_BEAM_WARP };
 
 // one unit of the loop: cached forward of the tokens in m->gtok, the history processors when `proc`, then the sampler
 // (beams == 0) or the beam candidates and scorer (which also advance the device counters); or one contrastive step.
@@ -627,7 +627,7 @@ static int gen_unit(seedb200_llama* m, int B, int beams, int proc, int kind, cud
   if (proc) SB_PROPAGATE(gen_process(m, B, beams, m->vpad, st));
   SB_PROPAGATE(beam_select(m->glogits, (int64_t)beams * m->vpad, m->vpad, B, beams, m->cfg.vocab, m->beam.beam_scores,
                            nullptr, m->beam.params, 0, m->gstate, m->beam.row_stats, m->beam.cand_score,
-                           m->beam.cand_idx, st));
+                           m->beam.cand_idx, st, kind == UNIT_BEAM_WARP));
   SB_PROPAGATE(beam_score(m->beam, B, beams, m->cfg.vocab, /*advance_cache=*/1, st));
   return 0;
 }
@@ -719,12 +719,15 @@ static int gen_run_units(seedb200_llama* m, int B, int beams, int proc, int kind
 static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int n, int S, int max_new,
                           const seedb200_sample_params* sp, int64_t eos, int64_t pad, int use_graph,
                           int64_t* tokens_out, int* n_generated_host, const seedb200_logits_params* lp,
-                          cudaStream_t st) {
+                          seedb200_gen_outputs* outputs, cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
   const int R = B * n;
   GenParams gp;
   gp.sp = *sp; gp.eos = eos; gp.pad = pad;
   gp.proc = logits_proc(lp, eos, S);
+  gp.scores = outputs ? static_cast<__half*>(outputs->scores) : nullptr;
+  gp.scores_pitch = outputs ? outputs->scores_pitch : 0;
+  gp.scores_step = (long long)R * gp.scores_pitch;
   const int proc = logits_history_active(gp.proc) ? 1 : 0;
   SB_PROPAGATE(gen_begin(m, prompt_ids, B, S, gp, st, n));
   if (n > 1) {
@@ -742,7 +745,10 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
   int done = 0;
   SB_PROPAGATE(gen_run_units(m, R, 0, proc, n > 1 ? UNIT_SHARED : UNIT_PLAIN, max_new - 1, use_graph,
                              eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st, &done));
-  SB_PROPAGATE(gen_end(m, R, S, max_new, eos, done + 1, tokens_out, n_generated_host, st));
+  int n_valid = 0;
+  SB_PROPAGATE(gen_end(m, R, S, max_new, eos, done + 1, tokens_out, &n_valid, st));
+  if (n_generated_host != nullptr) *n_generated_host = n_valid;
+  if (outputs != nullptr) outputs->n_steps_out = n_valid;
   m->gen_cache_len = n > 1 ? 0 : S + done;   // tokens whose K/V are in the cache; with n > 1 the rows hold lineages
   return 0;
 }
@@ -753,10 +759,18 @@ static int llama_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, i
 static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int n, int S, int max_new,
                                const seedb200_beam_params* p, int64_t eos, int64_t pad, int use_graph,
                                int64_t* tokens_out, int* n_out_host, float* best_scores,
-                               const seedb200_logits_params* lp, cudaStream_t st) {
+                               const seedb200_logits_params* lp, seedb200_gen_outputs* outputs, cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
   const int k = p->num_beams, G = B * n;
-  const BeamParams bp = beam_params(*p, eos, pad, S, max_new, G, lp, n);
+  BeamParams bp = beam_params(*p, eos, pad, S, max_new, G, lp, n);
+  if (outputs != nullptr) {
+    bp.scores = static_cast<__half*>(outputs->scores);
+    bp.scores_pitch = outputs->scores_pitch;
+    bp.scores_step = (long long)G * k * outputs->scores_pitch;
+    bp.beam_indices = reinterpret_cast<long long*>(outputs->beam_indices);
+    bp.bi_ld = S + max_new;
+  }
+  const bool warp = outputs != nullptr && bp.do_sample;   // beam sampling's scores: one more launch per step
   if (bp.processed && m->beam.tok == nullptr)
     SB_PROPAGATE(llama_alloc(m->row_owned, &m->beam.tok, (size_t)c.max_batch * c.max_seq));
   SB_PROPAGATE(beam_init(m->beam, bp, prompt_ids, st));
@@ -765,16 +779,20 @@ static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int
   if (bp.processed) SB_PROPAGATE(gen_process(m, G, k, 0, st));
   SB_PROPAGATE(beam_select(m->glogits, m->vpad, 0, G, k, c.vocab, m->beam.beam_scores, nullptr, m->beam.params, 0,
                            m->gstate, m->beam.row_stats, m->beam.cand_score,
-                           m->beam.cand_idx, st));
+                           m->beam.cand_idx, st, warp));
   SB_PROPAGATE(beam_score(m->beam, G, k, c.vocab, /*advance_cache=*/0, st));
   int done = 0;
-  SB_PROPAGATE(gen_run_units(m, G, k, bp.processed, UNIT_PLAIN, max_new - 1, use_graph,
+  SB_PROPAGATE(gen_run_units(m, G, k, bp.processed, warp ? UNIT_BEAM_WARP : UNIT_PLAIN, max_new - 1, use_graph,
                              eos >= 0 ? STOP_BEAMS_DONE : STOP_NEVER, st, &done));
   SB_PROPAGATE(beam_finalize(m->beam, G, tokens_out, max_new, best_scores, st));
   int n_out = 0;
   SB_CHECK_CUDA(cudaMemcpyAsync(&n_out, m->beam.n_out, sizeof(int), cudaMemcpyDeviceToHost, st));
   SB_CHECK_CUDA(cudaStreamSynchronize(st));
   if (n_out_host != nullptr) *n_out_host = n_out;
+  if (outputs != nullptr) {   // transformers' process() calls: through the step every search became done, else all
+    SB_PROPAGATE(gen_state_read(m, st));
+    outputs->n_steps_out = m->gstate_host[GS_VALID] != 0 ? m->gstate_host[GS_VALID] : done + 1;
+  }
   m->gen_cache_len = 0;            // the cache rows now hold beam lineages, not B plain sequences
   return 0;
 }
@@ -784,7 +802,7 @@ static int llama_beam_generate(seedb200_llama* m, const int64_t* prompt_ids, int
 static int llama_contrastive_generate(seedb200_llama* m, const int64_t* prompt_ids, int B, int S, int max_new,
                                       const seedb200_contrastive_params* cp, int64_t eos, int64_t pad, int use_graph,
                                       int64_t* tokens_out, int* n_generated_host, const seedb200_logits_params* lp,
-                                      cudaStream_t st) {
+                                      seedb200_gen_outputs* outputs, cudaStream_t st) {
   const seedb200_llama_config& c = m->cfg;
   const ContrastParams p = contrast_params(*cp);
   if (m->c_tickets == nullptr) {   // allocated last: a failed first call allocates again
@@ -801,6 +819,11 @@ static int llama_contrastive_generate(seedb200_llama* m, const int64_t* prompt_i
   gp.eos = eos; gp.pad = pad;
   gp.proc = logits_proc(lp, eos, S);
   gp.proc.lp.top_k = 0;                           // the candidate count, not a warper
+  if (outputs != nullptr) {
+    gp.scores = static_cast<__half*>(outputs->scores);
+    gp.scores_pitch = outputs->scores_pitch;
+    gp.scores_step = (long long)B * outputs->scores_pitch;
+  }
   const int proc = logits_history_active(gp.proc) ? 1 : 0;
   SB_PROPAGATE(gen_begin(m, prompt_ids, B, S, gp, st));
   SB_PROPAGATE(llama_forward(m, prompt_ids, nullptr, nullptr, B, S, 0, 1, m->c_logits, m->vpad, st));
@@ -809,7 +832,10 @@ static int llama_contrastive_generate(seedb200_llama* m, const int64_t* prompt_i
   int done = 0;
   SB_PROPAGATE(gen_run_units(m, B, p.k, proc, UNIT_CONTRASTIVE, max_new, use_graph,
                              eos >= 0 ? STOP_ALL_FINISHED : STOP_NEVER, st, &done));
-  SB_PROPAGATE(gen_end(m, B, S, max_new, eos, done, tokens_out, n_generated_host, st));
+  int n_valid = 0;
+  SB_PROPAGATE(gen_end(m, B, S, max_new, eos, done, tokens_out, &n_valid, st));
+  if (n_generated_host != nullptr) *n_generated_host = n_valid;
+  if (outputs != nullptr) outputs->n_steps_out = n_valid;
   m->gen_cache_len = 0;            // the cache rows now hold candidate lineages, not B plain sequences
   return 0;
 }
@@ -840,6 +866,19 @@ static int gen_args_check(const char* who, const seedb200_llama* m, const int64_
   SB_REQUIRE(m && prompt_ids && params, "%s: null argument", who);
   SB_REQUIRE(S >= 1 && max_new >= 1 && S + max_new <= m->cfg.max_seq, "%s: prompt %d + %d new tokens exceeds max_seq %d",
              who, S, max_new, m->cfg.max_seq);
+  return 0;
+}
+
+// seedb200_gen_outputs (NULL passes): a scores buffer of 16-byte aligned rows a multiple of 8 halves apart;
+// beam_indices only for beam search (optional there).  The pitch is checked against the vocabulary once the handle
+// has been.
+static int gen_outputs_check(const char* who, const seedb200_gen_outputs* o, bool beams = false) {
+  if (o == nullptr) return 0;
+  SB_REQUIRE(o->scores != nullptr && (uintptr_t)o->scores % 16 == 0,
+             "%s: outputs.scores must be a 16-byte aligned device pointer", who);
+  SB_REQUIRE(o->scores_pitch > 0 && o->scores_pitch % 8 == 0,
+             "%s: outputs.scores_pitch %lld must be a positive multiple of 8", who, (long long)o->scores_pitch);
+  SB_REQUIRE(beams || o->beam_indices == nullptr, "%s: outputs.beam_indices is written by beam search only", who);
   return 0;
 }
 
@@ -1007,8 +1046,17 @@ int seedb200_llama_generate_n_processed(seedb200_llama* llm, const int64_t* prom
                                         const seedb200_sample_params* sp, int64_t eos_id, int64_t pad_id,
                                         int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream,
                                         const seedb200_logits_params* lp) {
+  return seedb200_llama_generate_ex(llm, prompt_ids, B, S, max_new_tokens, num_return_sequences, sp, eos_id, pad_id,
+                                    use_graph, tokens_out, n_generated_host, stream, lp, nullptr);
+}
+
+int seedb200_llama_generate_ex(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                               int num_return_sequences, const seedb200_sample_params* sp, int64_t eos_id,
+                               int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host, void* stream,
+                               const seedb200_logits_params* lp, seedb200_gen_outputs* outputs) {
   const int n = num_return_sequences;
   SB_REQUIRE(n >= 1, "llama_generate: num_return_sequences %d < 1", n);
+  SB_PROPAGATE(sb::gen_outputs_check("llama_generate", outputs));
   SB_PROPAGATE(sb::logits_params_check("llama_generate", lp));
   SB_PROPAGATE(sb::gen_args_check("llama_generate", llm, prompt_ids, sp, S, max_new_tokens));
   SB_REQUIRE(B >= 1 && (int64_t)B * n <= llm->cfg.max_batch,
@@ -1016,10 +1064,13 @@ int seedb200_llama_generate_n_processed(seedb200_llama* llm, const int64_t* prom
              llm->cfg.max_batch);
   SB_REQUIRE((int64_t)B * n <= 1024, "llama_generate: batch %d x %d sequences above 1024 rows", B, n);
   SB_REQUIRE(!sp->do_sample || (sp->temperature > 0.0f && sp->top_p > 0.0f), "llama_generate: temperature and top_p must be > 0");
+  SB_REQUIRE(outputs == nullptr || outputs->scores_pitch >= llm->cfg.vocab,
+             "llama_generate: outputs.scores_pitch %lld below the vocabulary %d", (long long)outputs->scores_pitch,
+             llm->cfg.vocab);
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_generate(llm, prompt_ids, B, n, S, max_new_tokens, sp, eos_id, pad_id, use_graph, tokens_out,
-                            n_generated_host, lp, static_cast<cudaStream_t>(stream));
+                            n_generated_host, lp, outputs, static_cast<cudaStream_t>(stream));
 }
 
 int seedb200_llama_generate_used_graph(seedb200_llama* llm) { return llm ? llm->used_graph : -1; }
@@ -1053,8 +1104,19 @@ int seedb200_llama_beam_generate_n_processed(seedb200_llama* llm, const int64_t*
                                              const seedb200_beam_params* bp, int64_t eos_id, int64_t pad_id,
                                              int use_graph, int64_t* tokens_out, int* n_out_host,
                                              float* best_scores_out, void* stream, const seedb200_logits_params* lp) {
+  return seedb200_llama_beam_generate_ex(llm, prompt_ids, B, S, max_new_tokens, num_return_sequences, bp, eos_id,
+                                         pad_id, use_graph, tokens_out, n_out_host, best_scores_out, stream, lp,
+                                         nullptr);
+}
+
+int seedb200_llama_beam_generate_ex(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S, int max_new_tokens,
+                                    int num_return_sequences, const seedb200_beam_params* bp, int64_t eos_id,
+                                    int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_out_host,
+                                    float* best_scores_out, void* stream, const seedb200_logits_params* lp,
+                                    seedb200_gen_outputs* outputs) {
   const int n = num_return_sequences;
   SB_REQUIRE(n >= 1, "llama_beam_generate: num_return_sequences %d < 1", n);
+  SB_PROPAGATE(sb::gen_outputs_check("llama_beam_generate", outputs, /*beams=*/true));
   SB_REQUIRE(n == 1 || bp == nullptr || bp->do_sample,
              "llama_beam_generate: num_return_sequences %d > 1 needs beam sampling (do_sample)", n);
   SB_PROPAGATE(sb::logits_params_check("llama_beam_generate", lp));
@@ -1071,16 +1133,29 @@ int seedb200_llama_beam_generate_n_processed(seedb200_llama* llm, const int64_t*
   SB_REQUIRE(bp->early_stopping >= 0 && bp->early_stopping <= 2, "llama_beam_generate: early_stopping %d not in {0,1,2}",
              bp->early_stopping);
   SB_REQUIRE(eos_id < llm->cfg.vocab, "llama_beam_generate: eos_id %lld outside the vocabulary", (long long)eos_id);
+  SB_REQUIRE(outputs == nullptr || outputs->scores_pitch >= llm->cfg.vocab,
+             "llama_beam_generate: outputs.scores_pitch %lld below the vocabulary %d", (long long)outputs->scores_pitch,
+             llm->cfg.vocab);
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_beam_generate(llm, prompt_ids, B, n, S, max_new_tokens, bp, eos_id, pad_id, use_graph, tokens_out,
-                                 n_out_host, best_scores_out, lp, static_cast<cudaStream_t>(stream));
+                                 n_out_host, best_scores_out, lp, outputs, static_cast<cudaStream_t>(stream));
 }
 
 int seedb200_llama_contrastive_generate(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
                                         int max_new_tokens, const seedb200_contrastive_params* cp, int64_t eos_id,
                                         int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
                                         void* stream, const seedb200_logits_params* lp) {
+  return seedb200_llama_contrastive_generate_ex(llm, prompt_ids, B, S, max_new_tokens, cp, eos_id, pad_id, use_graph,
+                                                tokens_out, n_generated_host, stream, lp, nullptr);
+}
+
+int seedb200_llama_contrastive_generate_ex(seedb200_llama* llm, const int64_t* prompt_ids, int B, int S,
+                                           int max_new_tokens, const seedb200_contrastive_params* cp, int64_t eos_id,
+                                           int64_t pad_id, int use_graph, int64_t* tokens_out, int* n_generated_host,
+                                           void* stream, const seedb200_logits_params* lp,
+                                           seedb200_gen_outputs* outputs) {
+  SB_PROPAGATE(sb::gen_outputs_check("llama_contrastive_generate", outputs));
   SB_PROPAGATE(sb::contrastive_params_check("llama_contrastive_generate", cp));
   SB_PROPAGATE(sb::logits_params_check("llama_contrastive_generate", lp));
   SB_PROPAGATE(sb::gen_args_check("llama_contrastive_generate", llm, prompt_ids, cp, S, max_new_tokens));
@@ -1091,13 +1166,16 @@ int seedb200_llama_contrastive_generate(seedb200_llama* llm, const int64_t* prom
              (long long)eos_id);
   SB_REQUIRE(llm->cfg.vocab >= sb::CONTRAST_MAX_K, "llama_contrastive_generate: vocabulary below %d",
              sb::CONTRAST_MAX_K);
+  SB_REQUIRE(outputs == nullptr || outputs->scores_pitch >= llm->cfg.vocab,
+             "llama_contrastive_generate: outputs.scores_pitch %lld below the vocabulary %d",
+             (long long)outputs->scores_pitch, llm->cfg.vocab);
   SB_REQUIRE((size_t)cp->top_k * llm->cfg.hidden * 2 <= 200 * 1024,
              "llama_contrastive_generate: top_k %d x hidden %d exceed the rank kernel's shared memory", cp->top_k,
              llm->cfg.hidden);
   SB_PROPAGATE(sb::llama_linears_ready(llm));
   sb::DeviceGuard guard(llm->device);
   return sb::llama_contrastive_generate(llm, prompt_ids, B, S, max_new_tokens, cp, eos_id, pad_id, use_graph,
-                                        tokens_out, n_generated_host, lp, static_cast<cudaStream_t>(stream));
+                                        tokens_out, n_generated_host, lp, outputs, static_cast<cudaStream_t>(stream));
 }
 
 int seedb200_llama_reserve_rows(seedb200_llama* llm, int rows) {

@@ -59,7 +59,8 @@ int decode_attention_rope(const void* qkv, const int64_t* positions, int B, int 
 //   GS_CACHE_LEN   K/V positions in the cache
 //   GS_STEP        the step being generated
 //   GS_ARRIVE      sequences that have ended the current step
-//   GS_VALID       steps HF keeps: last step with an unfinished sequence + 1 (sampler and contrastive loops)
+//   GS_VALID       steps HF keeps: last step with an unfinished sequence + 1 (sampler and contrastive loops); in the
+//                  beam loop the step at which every search became done + 1 (0: not done)
 //   GS_UNFINISHED  some sequence was unfinished at the current step (sampler and contrastive loops)
 //   GS_ALL_DONE    every sequence's beam search is done (beam loop)
 enum GenSlot { GS_CACHE_LEN, GS_STEP, GS_ARRIVE, GS_VALID, GS_UNFINISHED, GS_ALL_DONE, GS_SLOTS };
@@ -82,8 +83,13 @@ inline bool logits_history_active(const LogitsProc& p) {
          (p.eos >= 0 && (p.lp.min_length > 0 || p.lp.min_new_tokens > 0));
 }
 int logits_params_check(const char* who, const seedb200_logits_params* p);   // NULL passes
-// out[b, proc.S + step] = token (the device loop keeps the prompt in out[b, 0:S])
-struct GenParams { seedb200_sample_params sp; long long eos, pad; LogitsProc proc; };
+// out[b, proc.S + step] = token (the device loop keeps the prompt in out[b, 0:S]).  scores (NULL: none): the step's
+// scores row of row b goes to scores + step * scores_step + b * scores_pitch (seedb200_gen_outputs); it lives here,
+// in the device-resident parameters each call rewrites, so that a replayed graph writes into this call's buffer.
+struct GenParams {
+  seedb200_sample_params sp; long long eos, pad; LogitsProc proc;
+  __half* scores; long long scores_pitch, scores_step;
+};
 // gp (host, by value) or gp_dev (device, read at run time); state (device, optional): the GenSlot counters, which
 // give the step and which the last CTA advances.
 int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, const GenParams* gp_dev, uint64_t step,
@@ -108,6 +114,10 @@ struct BeamParams {                    // read by the beam kernels at run time (
   long long eos, pad;
   LogitsProc proc;                     // top_k (beam sampling) and the history processors
   int processed;                       // 1: the rows already hold the processed fp16 log_softmax (logits_process)
+  // outputs (seedb200_gen_outputs; NULL: none), here so that a replayed graph writes into this call's buffers: the
+  // scores row of (step t, beam row r) at scores + t * scores_step + r * scores_pitch; beam_indices [B, bi_ld]
+  __half* scores; long long scores_pitch, scores_step;
+  long long* beam_indices; long long bi_ld;
 };
 inline BeamParams beam_params(const seedb200_beam_params& p, long long eos, long long pad, int S, int max_new, int B,
                               const seedb200_logits_params* lp = nullptr, int gpp = 1) {
@@ -117,12 +127,16 @@ inline BeamParams beam_params(const seedb200_beam_params& p, long long eos, long
   b.seed = p.seed; b.offset = p.offset; b.eos = eos; b.pad = pad;
   b.proc = logits_proc(lp, eos, S);
   b.processed = logits_history_active(b.proc) ? 1 : 0;
+  b.scores = nullptr; b.scores_pitch = 0; b.scores_step = 0; b.beam_indices = nullptr; b.bi_ld = 0;
   return b;
 }
-// logits row of (sequence i, beam j) = logits + i * seq_ld + j * beam_ld; -> cand_score / cand_idx [B, 2k]
+// logits row of (sequence i, beam j) = logits + i * seq_ld + j * beam_ld; -> cand_score / cand_idx [B, 2k].  With a
+// scores buffer in the parameters the row statistics launch also writes each beam row's fp16 log_softmax there;
+// warp_scores (beam sampling with scores) adds one launch that warps those rows in place.
 int beam_select(const void* logits, int64_t seq_ld, int64_t beam_ld, int B, int k, int V, const float* beam_scores,
                 const BeamParams* bp, const BeamParams* bp_dev, uint64_t step, const int* state, float* row_stats,
-                float* cand_score, int* cand_idx, cudaStream_t stream);   // row_stats: [B*k, 5] scratch
+                float* cand_score, int* cand_idx, cudaStream_t stream,
+                bool warp_scores = false);   // row_stats: [B*k, 5] scratch
 // the device state of one beam-search run (rows = B * k <= max_batch; hyps: k per sequence)
 struct BeamState {
   BeamParams* params;
@@ -161,10 +175,11 @@ struct ContrastParams { int k; float c_prob, c_pen; };   // c_prob = fp32(1 - al
 int contrastive_params_check(const char* who, const seedb200_contrastive_params* cp);   // NULL is refused
 ContrastParams contrast_params(const seedb200_contrastive_params& cp);
 // candidates of B rows (logits + b * ld): ids / probs [B*k]; p (host) or p_dev (device); slot (optional)
-// [B*k, max_seq] gets slot[r, pos] = r with pos = state[GS_CACHE_LEN] when state is given
+// [B*k, max_seq] gets slot[r, pos] = r with pos = state[GS_CACHE_LEN] when state is given; gp_dev (optional, with
+// state): each row is also copied to gp_dev's scores buffer at step state[GS_STEP] when it has one
 int contrastive_candidates(const void* logits, int64_t ld, int B, int V, const ContrastParams* p,
                            const ContrastParams* p_dev, const int* state, int pos, int* slot, int max_seq,
-                           int64_t* ids, void* probs, cudaStream_t stream);
+                           int64_t* ids, void* probs, cudaStream_t stream, const GenParams* gp_dev = nullptr);
 // one rank + select launch (see RankArgs in contrastive.cu); the loop fields are NULL in the standalone entry point
 struct ContrastRank {
   __half* ctx; int64_t ctx_ld; int ctx_rows, H;

@@ -250,7 +250,13 @@ sample_kernel(const SampleArgs a) {
   mx = red[0]; mi = red_i[0];
   if (mi == 0x7fffffff) mi = 0;
   int pick = mi;
+  // this step's scores row of sequence b (seedb200_gen_outputs), formed where it is written
+  auto scores_row = [&]() { return gp.scores + (long long)step * gp.scores_step + (long long)b * gp.scores_pitch; };
 
+  if (sp.do_sample == 0 && gp.scores != nullptr) {     // greedy_search's scores: the processed row, no warpers
+    __half* srow = scores_row();
+    for (int i = tid; i < V; i += SEL_THREADS) srow[i] = row[i];
+  }
   if (sp.do_sample != 0) {
     // p_i = exp((x_i - max) / T)  (unnormalised; TemperatureLogitsWarper then softmax)
     const float inv_t = 1.0f / fmaxf(sp.temperature, 1e-6f);
@@ -287,6 +293,17 @@ sample_kernel(const SampleArgs a) {
     // nucleus threshold: smallest t with mass{p > t} < top_p * Z; kept = {p >= t}.  top_p >= 1 keeps everything.
     float thr = 0.0f;
     if (sp.top_p < 1.0f) thr = nucleus_threshold(prob, i0, i1, sp.top_p * Z, red);
+    // sample's scores (4.30.2 generation/utils.py sample: next_token_scores after the warpers): the tempered fp16 logit
+    // on the kept set the draw below uses, -inf elsewhere (the filter value of TopK / TopP)
+    if (gp.scores != nullptr) {
+      __half* srow = scores_row();
+      const float inv_tk = 1.0f / sp.temperature;
+      for (int i = tid; i < V; i += SEL_THREADS) {
+        const float x = __half2float(row[i]);
+        const __half v = sp.temperature == 1.0f ? row[i] : __float2half_rn(x * inv_tk);
+        srow[i] = (x >= xmin && prob(i) >= thr) ? v : __float2half_rn(-INFINITY);
+      }
+    }
     // inverse CDF over the kept tokens in index order
     float k = 0.0f;
     for (int i = i0; i < i1; ++i) { const float p = prob(i); k += p >= thr ? p : 0.0f; }
@@ -336,6 +353,7 @@ int sample(const void* logits, int64_t ld, int B, int V, const GenParams* gp, co
   else {
     a.gp.sp.do_sample = 0; a.gp.sp.temperature = 1.0f; a.gp.sp.top_p = 1.0f; a.gp.sp.seed = 0; a.gp.sp.offset = 0;
     a.gp.eos = -1; a.gp.pad = 0; a.gp.proc = logits_proc(nullptr, -1, 0);
+    a.gp.scores = nullptr; a.gp.scores_pitch = 0; a.gp.scores_step = 0;
   }
   a.gp_dev = gp_dev; a.step = step; a.state = state; a.advance_cache = advance_cache;
   a.tokens = reinterpret_cast<long long*>(tokens);
@@ -407,6 +425,15 @@ beam_row_stats_kernel(const BeamSelectArgs a) {
   const bool processed = bp.processed != 0;
   float lz = 0.0f;
   if (!processed) lz = logf(block_exp_sum(row, i0, i1, m1, red));
+  // beam_search's scores (4.30.2 generation/utils.py: scores += (next_token_scores_processed,)): the processed fp16
+  // log_softmax, before the beam score.  At step 0 every beam row reads its sequence's one row (beam_ld 0), so the k
+  // rows of a sequence are identical.
+  if (bp.scores != nullptr) {
+    const long long step = a.state ? a.state[GS_STEP] : (long long)a.step;
+    __half* srow = bp.scores + step * bp.scores_step + (long long)(sq * k + j) * bp.scores_pitch;
+    for (int i = tid; i < V; i += SEL_THREADS)
+      srow[i] = processed ? row[i] : __float2half_rn((__half2float(row[i]) - m1) - lz);
+  }
   const float bsc = a.beam_scores[sq * k + j];
   // s = float(fp16 log_softmax) + beam score, fp32 (processed rows hold the fp16 log_softmax already)
   auto score = [&](float x) { return beam_s(processed, x, m1, lz, bsc); };
@@ -507,9 +534,55 @@ beam_select_kernel(const BeamSelectArgs a) {
   }
 }
 
+// beam_sample's scores (4.30.2 generation/utils.py: scores += (logits_warper(input_ids,
+// next_token_scores_processed),)): the warpers on the processed fp16 row, without the beam score, in place on the rows
+// beam_row_stats_kernel wrote.  One CTA per (beam row j, sequence).  Temperature v = fp16(x * fp32(1 / T)) (x at
+// T == 1); TopK keeps v >= the k'-th largest v, k' = min(max(top_k, 2), V); TopP keeps p = exp(v - max) >= the nucleus
+// threshold of the TopK-kept tokens, lowered to the second largest v's p (min_tokens_to_keep 2).  Removed: -inf.
+__global__ void __launch_bounds__(SEL_THREADS)
+beam_scores_warp_kernel(const BeamSelectArgs a) {
+  __shared__ float red[SEL_WARPS];
+  __shared__ unsigned s_hist[256];
+  __shared__ int s_sel[2];
+  const int j = blockIdx.x, sq = blockIdx.y, tid = threadIdx.x;
+  pdl_trigger();
+  pdl_wait();
+  const BeamParams bp = a.bp_dev ? *a.bp_dev : a.bp;
+  const int k = bp.k, V = a.V;
+  if (j >= k || bp.scores == nullptr) return;
+  const long long step = a.state ? a.state[GS_STEP] : (long long)a.step;
+  __half* row = bp.scores + step * bp.scores_step + (long long)(sq * k + j) * bp.scores_pitch;
+  const int per = (V + SEL_THREADS - 1) / SEL_THREADS;
+  const int i0 = min(V, tid * per), i1 = min(V, i0 + per);
+  const float T = bp.temperature, inv = 1.0f / T;
+  auto val = [&](int i) { return T == 1.0f ? row[i] : __float2half_rn(__half2float(row[i]) * inv); };
+  const float vmax = kth_largest(val, i0, i1, 1, s_hist, s_sel);
+  float vk = -INFINITY;
+  const int top_k = min(max(bp.proc.lp.top_k, 2), V);
+  if (bp.proc.lp.top_k > 0 && top_k < V) vk = kth_largest(val, i0, i1, top_k, s_hist, s_sel);
+  auto prob = [&](int i) {
+    const float v = __half2float(val(i));
+    return v < vk ? 0.0f : exp2f((v - vmax) * 1.4426950408889634f);
+  };
+  float thr = 0.0f;
+  if (bp.top_p < 1.0f) {
+    float z = 0.0f;
+    for (int i = i0; i < i1; ++i) z += prob(i);
+    const float Z = block_sum(z, red);
+    const float v2 = kth_largest(val, i0, i1, 2, s_hist, s_sel);
+    thr = fminf(nucleus_threshold(prob, i0, i1, bp.top_p * Z, red),
+                v2 == -INFINITY ? 0.0f : exp2f((v2 - vmax) * 1.4426950408889634f));
+  }
+  // every reduction above has completed (each ends in a block barrier); each element is read and written by one thread
+  for (int i = tid; i < V; i += SEL_THREADS) {
+    const __half v = val(i);
+    row[i] = (__half2float(v) >= vk && prob(i) >= thr) ? v : __float2half_rn(-INFINITY);
+  }
+}
+
 int beam_select(const void* logits, int64_t seq_ld, int64_t beam_ld, int B, int k, int V, const float* beam_scores,
                 const BeamParams* bp, const BeamParams* bp_dev, uint64_t step, const int* state, float* row_stats,
-                float* cand_score, int* cand_idx, cudaStream_t stream) {
+                float* cand_score, int* cand_idx, cudaStream_t stream, bool warp_scores) {
   SB_REQUIRE(logits && beam_scores && row_stats && cand_score && cand_idx && (bp || bp_dev), "beam_select: null operand");
   SB_REQUIRE(B >= 1 && k >= 1 && k <= BEAM_MAX && V >= 2 && (int64_t)k * V < 0x7fffffff,
              "beam_select: bad sizes (B %d, k %d in [1,%d], V %d >= 2)", B, k, BEAM_MAX, V);
@@ -528,6 +601,10 @@ int beam_select(const void* logits, int64_t seq_ld, int64_t beam_ld, int B, int 
   a.cand_score = cand_score; a.cand_idx = cand_idx;
   SB_CHECK_CUDA(launch_chain(beam_row_stats_kernel, dim3(k, B), dim3(SEL_THREADS), 0, stream, a));
   SB_LAUNCH_CHECK();
+  if (warp_scores) {
+    SB_CHECK_CUDA(launch_chain(beam_scores_warp_kernel, dim3(k, B), dim3(SEL_THREADS), 0, stream, a));
+    SB_LAUNCH_CHECK();
+  }
   const int n2 = 2 * k;
   auto kern = n2 <= 4 ? beam_select_kernel<4> : (n2 <= 8 ? beam_select_kernel<8> : beam_select_kernel<16>);
   SB_CHECK_CUDA(launch_chain(kern, dim3(B), dim3(SEL_THREADS), 0, stream, a));
@@ -571,11 +648,23 @@ int seedb200_sample(const void* logits, int64_t ld, int B, int V, const seedb200
 int seedb200_sample_processed(void* logits, int64_t ld, int B, int V, const seedb200_sample_params* sp, uint64_t step,
                               int64_t* tokens_out, void* stream, const seedb200_logits_params* lp,
                               const int64_t* history, int64_t hist_ld, int hist_len, int prompt_len, int64_t eos_id) {
+  return seedb200_sample_scores(logits, ld, B, V, sp, step, tokens_out, stream, lp, history, hist_ld, hist_len,
+                                prompt_len, eos_id, nullptr, 0);
+}
+
+int seedb200_sample_scores(void* logits, int64_t ld, int B, int V, const seedb200_sample_params* sp, uint64_t step,
+                           int64_t* tokens_out, void* stream, const seedb200_logits_params* lp,
+                           const int64_t* history, int64_t hist_ld, int hist_len, int prompt_len, int64_t eos_id,
+                           void* scores_out, int64_t scores_ld) {
   SB_REQUIRE(sp != nullptr, "seedb200_sample: null parameters");
   SB_PROPAGATE(sb::logits_params_check("seedb200_sample_processed", lp));
+  SB_REQUIRE(scores_out == nullptr || (scores_ld >= V && scores_ld % 8 == 0 && (uintptr_t)scores_out % 16 == 0),
+             "seedb200_sample_scores: scores rows need a pitch >= V %d that is a multiple of 8 (got %lld) and a "
+             "16-byte aligned base", V, (long long)scores_ld);
   sb::GenParams gp;
   gp.sp = *sp; gp.eos = -1; gp.pad = 0;
   gp.proc = sb::logits_proc(lp, eos_id, prompt_len);
+  gp.scores = static_cast<__half*>(scores_out); gp.scores_pitch = scores_ld; gp.scores_step = 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (sb::logits_history_active(gp.proc)) {
     SB_REQUIRE(history != nullptr && hist_len >= 0 && hist_ld >= hist_len && prompt_len >= 0 && prompt_len <= hist_len,

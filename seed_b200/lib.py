@@ -49,6 +49,8 @@ EXPORTS = [
     "seedb200_contrastive_context_init",
     "seedb200_llama_generate_n", "seedb200_llama_generate_n_processed", "seedb200_llama_beam_generate_n",
     "seedb200_llama_beam_generate_n_processed",
+    "seedb200_sample_scores", "seedb200_llama_generate_ex", "seedb200_llama_contrastive_generate_ex",
+    "seedb200_llama_beam_generate_ex",
 ]
 
 DTYPE_F16, DTYPE_F32, DTYPE_I8 = 0, 1, 4
@@ -137,6 +139,17 @@ class LogitsParams(C.Structure):
 
 class ContrastiveParams(C.Structure):
     _fields_ = [("top_k", C.c_int32), ("penalty_alpha", C.c_double)]
+
+
+class GenOutputs(C.Structure):
+    _fields_ = [("scores", C.c_void_p), ("scores_pitch", C.c_int64), ("beam_indices", C.c_void_p),
+                ("n_steps_out", C.c_int32)]
+
+
+def scores_buffer(steps: int, rows: int, V: int, device) -> torch.Tensor:
+    """the fp16 [steps, rows, pitch] buffer the scores outputs write: the pitch is V rounded up to a multiple of 8, so
+    every row starts 16-byte aligned; callers see the [..., :V] view"""
+    return torch.empty((steps, rows, (V + 7) // 8 * 8), dtype=torch.float16, device=device)
 
 
 def logits_params(top_k: int = 0, repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
@@ -300,6 +313,13 @@ def load() -> C.CDLL:
                                                    + lib.seedb200_llama_beam_generate.argtypes[5:])
     lib.seedb200_llama_beam_generate_n_processed.argtypes = (lib.seedb200_llama_beam_generate_n.argtypes
                                                              + [C.POINTER(LogitsParams)])
+    lib.seedb200_sample_scores.argtypes = lib.seedb200_sample_processed.argtypes + [C.c_void_p, C.c_int64]
+    lib.seedb200_llama_generate_ex.argtypes = (lib.seedb200_llama_generate_n_processed.argtypes
+                                               + [C.POINTER(GenOutputs)])
+    lib.seedb200_llama_beam_generate_ex.argtypes = (lib.seedb200_llama_beam_generate_n_processed.argtypes
+                                                    + [C.POINTER(GenOutputs)])
+    lib.seedb200_llama_contrastive_generate_ex.argtypes = (lib.seedb200_llama_contrastive_generate.argtypes
+                                                           + [C.POINTER(GenOutputs)])
     lib.seedb200_contrastive_candidates.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                                     C.c_void_p, C.c_void_p]
     lib.seedb200_contrastive_rank.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p,
@@ -930,10 +950,13 @@ def decode_attention_rope(qkv: torch.Tensor, positions: Optional[torch.Tensor], 
 def sample(logits: torch.Tensor, do_sample: bool = False, temperature: float = 1.0, top_p: float = 1.0,
            seed: int = 0, offset: int = 0, step: int = 0, history: Optional[torch.Tensor] = None, top_k: int = 0,
            repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_length: int = 0,
-           min_new_tokens: int = 0, prompt_len: int = 0, eos_token_id: int = -1) -> torch.Tensor:
+           min_new_tokens: int = 0, prompt_len: int = 0, eos_token_id: int = -1,
+           scores_out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """logits [B, V] fp16 (row stride free) -> next token per row, int64 [B].  The further controls are those of
     seedb200_logits_params; history [B, L] int64 (device) holds each row's input ids (prompt_len of them the prompt)
-    and is needed by the penalty, n-gram and length controls.  `logits` is left unchanged."""
+    and is needed by the penalty, n-gram and length controls.  `logits` is left unchanged.  scores_out (optional,
+    fp16 [B, >= V] on the same device, rows 16-byte aligned and a multiple of 8 halves apart) receives each row's
+    generation score, as seedb200_gen_outputs defines it (seedb200_sample_scores)."""
     _need_cuda_f16(logits, "sample.logits")
     if logits.dim() != 2 or logits.stride(1) != 1:
         raise RuntimeError("sample: logits must be [B, V] with contiguous rows")
@@ -941,7 +964,12 @@ def sample(logits: torch.Tensor, do_sample: bool = False, temperature: float = 1
     out = torch.empty((B,), dtype=torch.int64, device=logits.device)
     sp = SampleParams(int(bool(do_sample)), float(temperature), float(top_p), int(seed), int(offset))
     lp = logits_params(top_k, repetition_penalty, no_repeat_ngram_size, min_length, min_new_tokens)
-    if lp is None:
+    if scores_out is not None:
+        _need_cuda_f16(scores_out, "sample.scores_out")
+        if scores_out.device != logits.device or scores_out.dim() != 2 or scores_out.shape[0] != B \
+                or scores_out.shape[1] < V or scores_out.stride(1) != 1:
+            raise RuntimeError(f"sample: scores_out must be [{B}, >= {V}] fp16 with contiguous rows on {logits.device}")
+    if lp is None and scores_out is None:
         with on(logits.device):
             check(load().seedb200_sample(logits.data_ptr(), logits.stride(0), B, V, C.byref(sp), int(step),
                                          out.data_ptr(), stream_ptr(logits.device)), "seedb200_sample")
@@ -954,11 +982,15 @@ def sample(logits: torch.Tensor, do_sample: bool = False, temperature: float = 1
         hist = history if history.stride(1) == 1 else history.contiguous()
         hist_len = hist.shape[1]
         logits = logits.clone()                 # the processors rewrite the rows in place
+    args = (logits.data_ptr(), logits.stride(0), B, V, C.byref(sp), int(step), out.data_ptr(),
+            stream_ptr(logits.device), C.byref(lp) if lp is not None else None, _p(hist),
+            hist.stride(0) if hist is not None else 0, hist_len, int(prompt_len), int(eos_token_id))
     with on(logits.device):
-        check(load().seedb200_sample_processed(logits.data_ptr(), logits.stride(0), B, V, C.byref(sp), int(step),
-                                               out.data_ptr(), stream_ptr(logits.device), C.byref(lp), _p(hist),
-                                               hist.stride(0) if hist is not None else 0, hist_len, int(prompt_len),
-                                               int(eos_token_id)), "seedb200_sample_processed")
+        if scores_out is None:
+            check(load().seedb200_sample_processed(*args), "seedb200_sample_processed")
+        else:
+            check(load().seedb200_sample_scores(*args, scores_out.data_ptr(), scores_out.stride(0)),
+                  "seedb200_sample_scores")
     return out
 
 
@@ -1241,11 +1273,13 @@ class Llama:
     def generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, do_sample: bool = False,
                  temperature: float = 1.0, top_p: float = 1.0, seed: int = 0, offset: int = 0,
                  eos_token_id: int = -1, pad_token_id: int = 0, use_graph: bool = True,
-                 num_return_sequences: int = 1, **controls) -> torch.Tensor:
+                 num_return_sequences: int = 1, scores: Optional[torch.Tensor] = None, **controls) -> torch.Tensor:
         """prompt [B,S] int64 (device) -> generated tokens [B * num_return_sequences, n] (n <= max_new_tokens; shorter
         only when every row hit eos), row b * num_return_sequences + j being sample j of prompt b.  Prefill + sampler
         + cached decode steps, all on the device; see seedb200_llama_generate_n.  Needs B * num_return_sequences <=
-        max_batch (reserve_rows).  `controls`: the keywords of logits_params (top_k, repetition_penalty, ...)."""
+        max_batch (reserve_rows).  `controls`: the keywords of logits_params (top_k, repetition_penalty, ...).
+        scores (optional): a scores_buffer(max_new_tokens, B * num_return_sequences, ...) that receives each step's
+        generation scores (seedb200_llama_generate_ex); steps [0, n) are valid."""
         if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
             raise RuntimeError(f"generate: prompt_ids must be int64 on {self.device}")
         prompt_ids = prompt_ids.contiguous()
@@ -1258,7 +1292,11 @@ class Llama:
         args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, rs, C.byref(sp), int(eos_token_id),
                 int(pad_token_id), int(bool(use_graph)), out.data_ptr(), C.byref(n), stream_ptr(self.device))
         with on(self.device):
-            if lp is None:
+            if scores is not None:
+                o = self._outputs(scores, max_new_tokens, B * rs, "generate")
+                check(load().seedb200_llama_generate_ex(*args, C.byref(lp) if lp is not None else None, C.byref(o)),
+                      "seedb200_llama_generate_ex")
+            elif lp is None:
                 check(load().seedb200_llama_generate_n(*args), "seedb200_llama_generate_n")
             else:
                 check(load().seedb200_llama_generate_n_processed(*args, C.byref(lp)),
@@ -1268,11 +1306,15 @@ class Llama:
     def beam_generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, num_beams: int, do_sample: bool = False,
                       temperature: float = 1.0, top_p: float = 1.0, length_penalty: float = 1.0, early_stopping=False,
                       seed: int = 0, offset: int = 0, eos_token_id: int = -1, pad_token_id: int = 0,
-                      use_graph: bool = True, num_return_sequences: int = 1, **controls):
+                      use_graph: bool = True, num_return_sequences: int = 1, scores: Optional[torch.Tensor] = None,
+                      beam_indices: Optional[torch.Tensor] = None, **controls):
         """prompt [B,S] int64 (device) -> (generated tokens [G, n] of the best hypothesis per search, fp32 scores [G]),
         G = B * num_return_sequences independent searches, prompt-major (beam sampling only when
         num_return_sequences > 1); see seedb200_llama_beam_generate_n.  Needs G * num_beams <= max_batch
-        (reserve_rows).  `controls`: the keywords of logits_params."""
+        (reserve_rows).  `controls`: the keywords of logits_params.
+        scores (optional): a scores_buffer(max_new_tokens, G * num_beams, ...) that receives each step's beam scores,
+        with beam_indices (optional) an int64 [G, S + max_new_tokens] tensor (seedb200_llama_beam_generate_ex); the
+        call then returns (tokens, scores [G], number of valid scores steps)."""
         if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
             raise RuntimeError(f"beam_generate: prompt_ids must be int64 on {self.device}")
         prompt_ids = prompt_ids.contiguous()
@@ -1280,7 +1322,7 @@ class Llama:
         rs = int(num_return_sequences)
         G = B * max(rs, 1)
         out = torch.empty((G, max_new_tokens), dtype=torch.int64, device=self.device)
-        scores = torch.empty((G,), dtype=torch.float32, device=self.device)
+        scores_out, scores = scores, torch.empty((G,), dtype=torch.float32, device=self.device)
         bp = beam_params(num_beams, do_sample, temperature, top_p, length_penalty, early_stopping, seed, offset)
         lp = logits_params(**controls)
         n = C.c_int(0)
@@ -1288,6 +1330,17 @@ class Llama:
                 int(pad_token_id), int(bool(use_graph)), out.data_ptr(), C.byref(n), scores.data_ptr(),
                 stream_ptr(self.device))
         with on(self.device):
+            if scores_out is not None:
+                o = self._outputs(scores_out, max_new_tokens, G * int(num_beams), "beam_generate")
+                if beam_indices is not None:
+                    if beam_indices.dtype != torch.int64 or beam_indices.device != self.device \
+                            or tuple(beam_indices.shape) != (G, S + max_new_tokens) or not beam_indices.is_contiguous():
+                        raise RuntimeError(f"beam_generate: beam_indices must be a contiguous int64 "
+                                           f"[{G}, {S + max_new_tokens}] tensor on {self.device}")
+                    o.beam_indices = beam_indices.data_ptr()
+                check(load().seedb200_llama_beam_generate_ex(*args, C.byref(lp) if lp is not None else None,
+                                                             C.byref(o)), "seedb200_llama_beam_generate_ex")
+                return out[:, :n.value], scores, o.n_steps_out
             if lp is None:
                 check(load().seedb200_llama_beam_generate_n(*args), "seedb200_llama_beam_generate_n")
             else:
@@ -1297,10 +1350,12 @@ class Llama:
 
     def contrastive_generate(self, prompt_ids: torch.Tensor, max_new_tokens: int, top_k: int, penalty_alpha: float,
                              eos_token_id: int = -1, pad_token_id: int = 0, use_graph: bool = True,
-                             **controls) -> torch.Tensor:
+                             scores: Optional[torch.Tensor] = None, **controls) -> torch.Tensor:
         """prompt [B,S] int64 (device) -> generated tokens [B, n] of contrastive search (n < max_new_tokens only when
         every sequence hit eos); see seedb200_llama_contrastive_generate.  Needs B * top_k <= max_batch
-        (reserve_rows).  `controls`: the processor keywords of logits_params (their top_k is not used)."""
+        (reserve_rows).  `controls`: the processor keywords of logits_params (their top_k is not used).
+        scores (optional): a scores_buffer(max_new_tokens, B, ...) that receives each step's processed logits
+        (seedb200_llama_contrastive_generate_ex); steps [0, n) are valid."""
         if not prompt_ids.is_cuda or prompt_ids.dtype != torch.int64 or prompt_ids.device != self.device:
             raise RuntimeError(f"contrastive_generate: prompt_ids must be int64 on {self.device}")
         prompt_ids = prompt_ids.contiguous()
@@ -1309,14 +1364,25 @@ class Llama:
         cp = ContrastiveParams(int(top_k), float(penalty_alpha))
         lp = logits_params(**dict(controls, top_k=0))
         n = C.c_int(0)
+        args = (self._h, prompt_ids.data_ptr(), B, S, max_new_tokens, C.byref(cp), int(eos_token_id),
+                int(pad_token_id), int(bool(use_graph)), out.data_ptr(), C.byref(n), stream_ptr(self.device),
+                C.byref(lp) if lp is not None else None)
         with on(self.device):
-            check(load().seedb200_llama_contrastive_generate(self._h, prompt_ids.data_ptr(), B, S, max_new_tokens,
-                                                             C.byref(cp), int(eos_token_id), int(pad_token_id),
-                                                             int(bool(use_graph)), out.data_ptr(), C.byref(n),
-                                                             stream_ptr(self.device),
-                                                             C.byref(lp) if lp is not None else None),
-                  "seedb200_llama_contrastive_generate")
+            if scores is None:
+                check(load().seedb200_llama_contrastive_generate(*args), "seedb200_llama_contrastive_generate")
+            else:
+                o = self._outputs(scores, max_new_tokens, B, "contrastive_generate")
+                check(load().seedb200_llama_contrastive_generate_ex(*args, C.byref(o)),
+                      "seedb200_llama_contrastive_generate_ex")
         return out[:, :n.value]
+
+    def _outputs(self, scores: torch.Tensor, steps: int, rows: int, who: str) -> GenOutputs:
+        """seedb200_gen_outputs over a scores_buffer(steps, rows, ...)"""
+        if scores.dtype != torch.float16 or scores.device != self.device or scores.dim() != 3 \
+                or tuple(scores.shape[:2]) != (steps, rows) or not scores.is_contiguous():
+            raise RuntimeError(f"{who}: scores must be a contiguous fp16 [{steps}, {rows}, pitch] tensor on "
+                               f"{self.device}")
+        return GenOutputs(scores.data_ptr(), scores.stride(1), None, 0)
 
     def reserve_rows(self, rows: int) -> None:
         """grow every max_batch-sized buffer to `rows` rows (drops the cache contents and the captured graphs)"""

@@ -30,6 +30,8 @@ from typing import List, Optional, Tuple, Union
 
 import torch
 import torch.nn as nn
+from transformers.generation import GenerateBeamDecoderOnlyOutput, GenerateDecoderOnlyOutput
+from transformers.generation.utils import GenerationMixin
 from transformers.modeling_outputs import CausalLMOutputWithPast
 from transformers.models.llama.configuration_llama import LlamaConfig
 
@@ -371,7 +373,8 @@ class LlamaForCausalLM(nn.Module):
     _GEN_DEFAULTS = {"max_new_tokens": 20, "do_sample": False, "temperature": 1.0, "top_p": 1.0, "num_beams": 1,
                      "length_penalty": 1.0, "early_stopping": False, "num_return_sequences": 1,
                      "top_k": 0, "repetition_penalty": 1.0, "no_repeat_ngram_size": 0, "min_length": 0,
-                     "min_new_tokens": 0, "penalty_alpha": None}
+                     "min_new_tokens": 0, "penalty_alpha": None, "output_scores": False,
+                     "return_dict_in_generate": False, "output_attentions": False, "output_hidden_states": False}
 
     @staticmethod
     def _controls(opts) -> dict:
@@ -397,7 +400,9 @@ class LlamaForCausalLM(nn.Module):
                  early_stopping=None, num_return_sequences: Optional[int] = None, top_k: Optional[int] = None,
                  repetition_penalty: Optional[float] = None, no_repeat_ngram_size: Optional[int] = None,
                  min_length: Optional[int] = None, min_new_tokens: Optional[int] = None,
-                 penalty_alpha: Optional[float] = None, **_):
+                 penalty_alpha: Optional[float] = None, output_scores: Optional[bool] = None,
+                 return_dict_in_generate: Optional[bool] = None, output_attentions: Optional[bool] = None,
+                 output_hidden_states: Optional[bool] = None, **_):
         """Call pattern of scripts/seed_llama_inference_8B.py:33 (temperature=1.0, num_beams=1, max_new_tokens=512,
         top_p=0.5, do_sample=True); returns [B, S + n_new] like HF generate.
 
@@ -428,13 +433,25 @@ class LlamaForCausalLM(nn.Module):
         and it must be given: transformers' default of 50 would mean 50 cache rows), the processors above still
         apply, and B * top_k rows must fit the handle, which grows as for beams.  With `num_beams` > 1 or
         `do_sample=True` penalty_alpha is ignored, as in transformers.
+        `return_dict_in_generate=True` returns transformers' GenerateDecoderOnlyOutput (GenerateBeamDecoderOnlyOutput
+        with beams) instead of the tensor; with `output_scores=True` as well, greedy decoding, sampling and
+        contrastive search fill `scores` as transformers 4.30.2 does (one fp16 [rows, V] tensor per step: the
+        processed logits when greedy, the warped row with -inf off the kept tokens when sampling, the processed logits
+        the candidates are taken from in contrastive search), written on the device by the kernel that holds the row (include/seedb200.h,
+        seedb200_gen_outputs).  Every route (device loop, per-token loop, num_return_sequences) returns them.  Beam
+        search and beam sampling fill `scores` (one [G * num_beams, V] tensor per BeamSearchScorer.process call: the
+        processed fp16 log_softmax, warped without the beam score when sampling), `sequences_scores` and
+        `beam_indices`, as 4.30.2 does.  `output_attentions` / `output_hidden_states` with
+        return_dict_in_generate=True raise NotImplementedError, as forward() does.
         `generation_config` (a transformers GenerationConfig) supplies these fields and its eos / pad ids, and
         explicit keyword arguments override it, as in transformers."""
         given = {"max_new_tokens": max_new_tokens, "do_sample": do_sample, "temperature": temperature, "top_p": top_p,
                  "num_beams": num_beams, "length_penalty": length_penalty, "early_stopping": early_stopping,
                  "num_return_sequences": num_return_sequences, "top_k": top_k,
                  "repetition_penalty": repetition_penalty, "no_repeat_ngram_size": no_repeat_ngram_size,
-                 "min_length": min_length, "min_new_tokens": min_new_tokens, "penalty_alpha": penalty_alpha}
+                 "min_length": min_length, "min_new_tokens": min_new_tokens, "penalty_alpha": penalty_alpha,
+                 "output_scores": output_scores, "return_dict_in_generate": return_dict_in_generate,
+                 "output_attentions": output_attentions, "output_hidden_states": output_hidden_states}
         opts = dict(self._GEN_DEFAULTS)
         if generation_config is not None:
             for name in opts:
@@ -449,6 +466,14 @@ class LlamaForCausalLM(nn.Module):
         max_new_tokens, do_sample, temperature, top_p = (int(opts["max_new_tokens"]), bool(opts["do_sample"]),
                                                          float(opts["temperature"]), float(opts["top_p"]))
         num_beams = int(opts["num_beams"])
+        return_dict = bool(opts["return_dict_in_generate"])
+        for name in ("output_attentions", "output_hidden_states"):
+            if return_dict and opts[name]:
+                raise NotImplementedError(f"{name}=True: attention weights and hidden states are not produced by the "
+                                          f"fused path")
+        # transformers computes the scores with output_scores alone and drops them; here they are only made when
+        # they are returned
+        want_scores = return_dict and bool(opts["output_scores"])
         controls = self._controls(opts)
         n_ret = int(opts["num_return_sequences"])
         if n_ret < 1:
@@ -484,24 +509,28 @@ class LlamaForCausalLM(nn.Module):
                                  "candidates, 2..8): pass top_k explicitly")
             if controls["top_k"] > 1:
                 return self._contrastive_generate(input_ids, max_new_tokens, controls["top_k"], float(alpha),
-                                                  eos_list, pad, padded, use_graph, controls)
+                                                  eos_list, pad, padded, use_graph, controls, return_dict,
+                                                  want_scores)
         if num_beams > 1:
-            return self._beam_generate(input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p,
-                                       float(opts["length_penalty"]), opts["early_stopping"], eos_list, pad, padded,
-                                       rng_seed, offset, use_graph, controls, n_ret)
+            out = self._beam_generate(input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p,
+                                      float(opts["length_penalty"]), opts["early_stopping"], eos_list, pad, padded,
+                                      rng_seed, offset, use_graph, controls, n_ret, want_scores)
+            return out if return_dict else out.sequences
         if device_loop is None:
             device_loop = (not padded) and len(eos_list) <= 1 and (B <= 4 or n_ret > 1)
         if device_loop:
             if padded or len(eos_list) > 1:
                 raise ValueError("device_loop needs an unpadded batch and at most one eos id")
             self._reserve(B * n_ret)
+            buf = L.scores_buffer(max_new_tokens, B * n_ret, self._llm.vocab, self._device) if want_scores else None
             new = self._llm.generate(input_ids, max_new_tokens, do_sample=do_sample, temperature=temperature,
                                      top_p=top_p, seed=rng_seed, offset=offset,
                                      eos_token_id=eos_list[0] if eos_list else -1, pad_token_id=pad,
-                                     use_graph=use_graph, num_return_sequences=n_ret, **controls)
+                                     use_graph=use_graph, num_return_sequences=n_ret, scores=buf, **controls)
             self._draws += max_new_tokens
             self._cache_len, self._cache_batch = 0, 0       # the handle's cache now belongs to that generation
-            return torch.cat([input_ids.repeat_interleave(n_ret, 0), new], dim=1)
+            seq = torch.cat([input_ids.repeat_interleave(n_ret, 0), new], dim=1)
+            return self._decoder_output(seq, buf, new.shape[1]) if return_dict else seq
         # ---- HF-shaped loop (padding masks, several eos ids): one forward per token from Python ----
         if n_ret > 1:   # transformers' _expand_inputs_for_generation: every prompt n_ret times, prompt-major
             input_ids = input_ids.repeat_interleave(n_ret, 0)
@@ -509,6 +538,7 @@ class LlamaForCausalLM(nn.Module):
             B = input_ids.shape[0]
             self._reserve(B)
         mask = attention_mask.to(self._device) if attention_mask is not None else None
+        buf = L.scores_buffer(max_new_tokens, B, self._llm.vocab, self._device) if want_scores else None
         seq, past = input_ids, None
         unfinished = torch.ones(B, dtype=torch.bool, device=self._device)
         for step in range(max_new_tokens):
@@ -518,7 +548,8 @@ class LlamaForCausalLM(nn.Module):
             past = out.past_key_values
             nxt = L.sample(out.logits[:, -1], do_sample=do_sample, temperature=temperature, top_p=top_p,
                            seed=rng_seed, offset=offset, step=step, history=seq, prompt_len=S,
-                           eos_token_id=eos_list[0] if eos_list else -1, **controls)
+                           eos_token_id=eos_list[0] if eos_list else -1,
+                           scores_out=buf[step] if buf is not None else None, **controls)
             nxt = torch.where(unfinished, nxt, torch.full_like(nxt, pad))
             seq = torch.cat([seq, nxt[:, None]], dim=1)
             if mask is not None:
@@ -528,7 +559,23 @@ class LlamaForCausalLM(nn.Module):
             if eos_list and not bool(unfinished.any()):
                 break
         self._draws += max_new_tokens
-        return seq
+        return self._decoder_output(seq, buf, seq.shape[1] - S) if return_dict else seq
+
+    def _decoder_output(self, seq, buf, steps):
+        """transformers' GenerateDecoderOnlyOutput; `scores` are views of the first `steps` steps of the scores
+        buffer (None when none was made)"""
+        scores = None if buf is None else tuple(buf[t, :, :self._llm.vocab] for t in range(steps))
+        return GenerateDecoderOnlyOutput(sequences=seq, scores=scores)
+
+    def compute_transition_scores(self, sequences: torch.Tensor, scores: Tuple[torch.Tensor],
+                                  beam_indices: Optional[torch.Tensor] = None,
+                                  normalize_logits: bool = False) -> torch.Tensor:
+        """transformers' GenerationMixin.compute_transition_scores: the score of each generated token, gathered from
+        the stacked `scores` (log_softmax over the vocabulary first when normalize_logits), beams followed through
+        `beam_indices` (-1: past the hypothesis' end, scored 0).  The installed implementation is called: it is the
+        algorithm of transformers 4.30.2 and reads only self.config."""
+        return GenerationMixin.compute_transition_scores(self, sequences, scores, beam_indices=beam_indices,
+                                                         normalize_logits=normalize_logits)
 
     def _reserve(self, rows):
         """grow the handle to `rows` rows; the cache is reallocated, so earlier past_key_values are void"""
@@ -537,7 +584,9 @@ class LlamaForCausalLM(nn.Module):
             self.max_batch = rows
 
     def _beam_generate(self, input_ids, max_new_tokens, num_beams, do_sample, temperature, top_p, length_penalty,
-                       early_stopping, eos_list, pad, padded, rng_seed, offset, use_graph, controls, n_ret=1):
+                       early_stopping, eos_list, pad, padded, rng_seed, offset, use_graph, controls, n_ret=1,
+                       want_scores=False):
+        """-> GenerateBeamDecoderOnlyOutput; with want_scores its scores, sequences_scores and beam_indices are set"""
         if num_beams > 8:
             raise ValueError(f"num_beams={num_beams}: at most 8 beams (the scorer runs one CTA per sequence)")
         if padded:
@@ -548,21 +597,32 @@ class LlamaForCausalLM(nn.Module):
             raise ValueError(f"early_stopping must be False, True or 'never' (got {early_stopping!r})")
         if do_sample and temperature <= 0.0:
             raise ValueError(f"temperature must be > 0 when sampling (got {temperature})")
-        B = input_ids.shape[0]
-        self._reserve(B * n_ret * num_beams)
-        new, _ = self._llm.beam_generate(input_ids, max_new_tokens, num_beams, do_sample=do_sample,
-                                         temperature=temperature if do_sample else 1.0, top_p=top_p,
-                                         length_penalty=length_penalty, early_stopping=early_stopping, seed=rng_seed,
-                                         offset=offset, eos_token_id=eos_list[0] if eos_list else -1,
-                                         pad_token_id=pad, use_graph=use_graph, num_return_sequences=n_ret,
-                                         **controls)
+        B, S = input_ids.shape
+        G = B * n_ret
+        self._reserve(G * num_beams)
+        buf = bi = None
+        if want_scores:
+            buf = L.scores_buffer(max_new_tokens, G * num_beams, self._llm.vocab, self._device)
+            bi = torch.empty((G, S + max_new_tokens), dtype=torch.int64, device=self._device)
+        res = self._llm.beam_generate(input_ids, max_new_tokens, num_beams, do_sample=do_sample,
+                                      temperature=temperature if do_sample else 1.0, top_p=top_p,
+                                      length_penalty=length_penalty, early_stopping=early_stopping, seed=rng_seed,
+                                      offset=offset, eos_token_id=eos_list[0] if eos_list else -1,
+                                      pad_token_id=pad, use_graph=use_graph, num_return_sequences=n_ret, scores=buf,
+                                      beam_indices=bi, **controls)
         self._draws += max_new_tokens
         self._cache_len, self._cache_batch = 0, 0
-        return torch.cat([input_ids.repeat_interleave(n_ret, 0), new], dim=1)
+        seq = torch.cat([input_ids.repeat_interleave(n_ret, 0), res[0]], dim=1)
+        if not want_scores:     # 4.30.2 drops sequences_scores without output_scores
+            return GenerateBeamDecoderOnlyOutput(sequences=seq)
+        # len(scores): BeamSearchScorer.process calls, recorded on the device; it can exceed the generated width
+        return GenerateBeamDecoderOnlyOutput(sequences=seq, sequences_scores=res[1],
+                                             scores=tuple(buf[t, :, :self._llm.vocab] for t in range(res[2])),
+                                             beam_indices=bi[:, :seq.shape[1]])
 
 
     def _contrastive_generate(self, input_ids, max_new_tokens, top_k, penalty_alpha, eos_list, pad, padded, use_graph,
-                              controls):
+                              controls, return_dict=False, want_scores=False):
         if top_k > 8:
             raise ValueError(f"top_k={top_k} with penalty_alpha: contrastive search takes at most 8 candidates")
         if not math.isfinite(penalty_alpha):
@@ -571,13 +631,16 @@ class LlamaForCausalLM(nn.Module):
             raise NotImplementedError("a padding attention_mask is not supported with contrastive search")
         if len(eos_list) > 1:
             raise NotImplementedError("several eos_token_id values are not supported with contrastive search")
-        self._reserve(input_ids.shape[0] * top_k)
+        B = input_ids.shape[0]
+        self._reserve(B * top_k)
+        buf = L.scores_buffer(max_new_tokens, B, self._llm.vocab, self._device) if want_scores else None
         new = self._llm.contrastive_generate(input_ids, max_new_tokens, top_k, penalty_alpha,
                                              eos_token_id=eos_list[0] if eos_list else -1, pad_token_id=pad,
-                                             use_graph=use_graph,
+                                             use_graph=use_graph, scores=buf,
                                              **{k: v for k, v in controls.items() if k != "top_k"})
         self._cache_len, self._cache_batch = 0, 0
-        return torch.cat([input_ids, new], dim=1)
+        seq = torch.cat([input_ids, new], dim=1)
+        return self._decoder_output(seq, buf, new.shape[1]) if return_dict else seq
 
 
 def get_pretrained_llama_causal_model(pretrained_model_name_or_path=None, torch_dtype="fp16", **kwargs):

@@ -200,6 +200,9 @@ class PeftModel:
     def generate(self, *args, **kwargs):
         return self.base_model.generate(*args, **kwargs)
 
+    def compute_transition_scores(self, *args, **kwargs):
+        return self.base_model.compute_transition_scores(*args, **kwargs)
+
     def prepare_inputs_for_generation(self, *args, **kwargs):
         return self.base_model.prepare_inputs_for_generation(*args, **kwargs)
 
